@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — WAL GB/s and events/s of the batched pgoutput decode path on N B200s of one node.
+"""bench.py — WAL GB/s and events/s of the batched pgoutput decode path on N H100s of one node.
 
-  python bench.py --gpus 1 --steps 5 --warmup 3                      (driver launches N>1 via torchrun)
+  python bench.py --gpus 1 --steps 5 --warmup 3                      (N>1: launch under torchrun)
   python bench.py --impl reference ...                                (the CPU path on the host cores)
 
 A "step" is one pass of the decode hot path over the staged synthetic stream:
@@ -13,13 +13,16 @@ ONE stream (its Relation messages appear once, in the first megabytes).  With N 
 byte ranges at record starts that fall INSIDE transactions (strong scaling: total work fixed, default); the
 library exchanges the Relation frames and the 64-byte seam summaries over NCCL (etl_dec_decode_sharded) — no host
 round trip between the index pass and the record pass.  `--scaling weak` gives every GPU a full 10 GiB range.
-Inputs are far larger than L2 (126 MB), so no flush is needed between steps.
+Inputs are far larger than L2 (50 MB), so no flush is needed between steps.
 
 After the timed legs, and outside them, rank 0 of a single-GPU run also (a) checks the CUDA path against the CPU
 oracle on EVERY segment of c5 and of c2 / c3 / c4 at their BASELINE sizes (canonical plane digests), (b) times
 c2 / c3 / c4 the same way as the headline and (c) times back-to-back decodes at the reference's own batch size
 (BatchConfig::DEFAULT_MAX_BYTES = 8 MiB, etl-config/src/shared/pipeline.rs:54-68) with carry-in/out chaining.
 All of it goes into the ONE JSON line.
+
+--dump-outputs DIR writes what the last timed step computed (the result planes a caller of that path receives) as
+DIR/<name>.npy, float64, for output-by-output comparison of two builds on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -68,15 +71,13 @@ def parse_args():
     ap.add_argument("--no-extras", action="store_true", help="skip the post-timing legs (parity at size, c2/c3/c4, 8 MiB batches)")
     ap.add_argument("--extras-scale", type=float, default=1.0, help="scale of the c2/c3/c4 legs (1.0 = BASELINE sizes)")
     ap.add_argument("--batch-calls", type=int, default=1000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result planes of the last timed step as DIR/<name>.npy (float64; a fixed sample, < 64 MB)")
     return ap.parse_args()
 
 
 def measured_peak():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, STREAM-style copy)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not a measured ceiling)"
 
 
 def host_cores():
@@ -195,8 +196,8 @@ def cpu_decode_segments(w, seg_arrays, threads, preamble=None, digests=False):
 
 
 def run_reference(args, rank, world):
-    """The reference arm: the CPU implementation of the path (oracle port — the Rust reference cannot be built in
-    this image) on every host core this process may use, on a bounded sample of the same workload."""
+    """The reference arm: the CPU implementation of the path (oracle port — the Rust reference is not built here)
+    on every host core this process may use, on a bounded sample of the same workload."""
     if rank != 0:
         return
     from etl_b200 import workloads as wl
@@ -275,22 +276,25 @@ def decode_once(dec, st, resident, sharded, carry=None, timing=True):
     return bh, s
 
 
-def time_steps(torch, dist, dec, st, resident, sharded, steps, dev, world):
+def time_steps(torch, dist, dec, st, resident, sharded, steps, dev, world, keep_last=False):
     """K decode calls as a production caller makes them (ETL_DECODE_NO_TIMING: no per-kernel event queries on the host),
     bracketed by barrier + synchronize and CUDA events, max over ranks.  The per-kernel breakdown comes from two more calls
-    with the summary timings on, after the timed region."""
+    with the summary timings on, after the timed region.  keep_last: the last timed step's batch is returned unfreed."""
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    rows, launches, last = [], 0, None
+    rows, launches, last, kept = [], 0, None, None
     e0.record()
-    for _ in range(steps):
+    for i in range(steps):
         bh, s = decode_once(dec, st, resident, sharded, timing=False)
         launches += s.gpu_launches
         last = dict(h2d=int(s.h2d_bytes), d2h=int(s.d2h_bytes), span_bytes=int(s.span_bytes), n_records=int(bh.planes(False).n_records),
                     n_cells=int(bh.planes(False).n_cells))
-        bh.free()
+        if keep_last and i == steps - 1:
+            kept = bh
+        else:
+            bh.free()
     e1.record()
     torch.cuda.synchronize()
     ms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
@@ -301,7 +305,68 @@ def time_steps(torch, dist, dec, st, resident, sharded, steps, dev, world):
         bh, s = decode_once(dec, st, resident, sharded, timing=True)
         rows.append((s.index_ms, s.frames_ms, s.walk_ms, s.cells_ms, s.spans_ms, s.kernel_ms, s.long_ms))
         bh.free()
+    if keep_last:
+        return float(ms.item()), np.mean(np.array(rows, dtype=np.float64), axis=0), launches, last, kept
     return float(ms.item()), np.mean(np.array(rows, dtype=np.float64), axis=0), launches, last
+
+
+DUMP_RECORDS, DUMP_CELLS = 1 << 17, 1 << 19      # sampled rows: 128 B per record and 32 B per cell as float64, 32 MiB at most
+HEAP_TAGS = (9, 14, 16, 17)                        # ETL_CELL_NUMERIC / UUID / BYTES / ARRAY: val is a heap offset
+
+
+def _device_plane(torch, dev, ptr, n, typestr):
+    """Zero-copy torch view of a device plane of the library (the batch owns the memory)."""
+    class _Plane:
+        __cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr), False), "version": 3}
+    return torch.as_tensor(_Plane(), device=dev)
+
+
+def _split_u64(a):
+    """uint64 → (n, 2) float64 [high 32 bits, low 32 bits]: exact, which one float64 column is not above 2^53."""
+    a = a.astype(np.uint64)
+    return np.stack([(a >> np.uint64(32)).astype(np.float64), (a & np.uint64(0xFFFFFFFF)).astype(np.float64)], axis=-1)
+
+
+def dump_outputs(torch, dev, bh, out_dir, prefix=""):
+    """The planes of a resident decode (device memory) as DIR/<prefix><plane>.npy.  Records and cells are a fixed sample
+    (seeded, the same indices for the same input), so the files stay under 64 MB for any stream size; the sample indices
+    are written too.  Heap offsets (numeric / uuid / bytes / array cells) depend on the order in which k_heavy's CTAs
+    allocate, so those cells' values are written as 0: their payloads are covered by the parity digest instead."""
+    os.makedirs(out_dir, exist_ok=True)
+    p, s = bh.planes(False), bh.summary()
+    n, m = int(p.n_records), int(p.n_cells)
+    rng = np.random.default_rng(0xD0D0)
+    ridx = np.unique(rng.integers(0, n, size=min(n, DUMP_RECORDS))) if n else np.zeros(0, np.int64)
+    cidx = np.unique(rng.integers(0, m, size=min(m, DUMP_CELLS))) if m else np.zeros(0, np.int64)
+
+    def take(ptr, count, typestr, idx):
+        if not len(idx):
+            return np.zeros(0, dtype=np.dtype(typestr))
+        t = _device_plane(torch, dev, ptr, count, typestr)
+        return t.index_select(0, torch.from_numpy(idx.astype(np.int64)).to(dev)).cpu().numpy()
+
+    out = {"record_sample_index": ridx.astype(np.float64), "cell_sample_index": cidx.astype(np.float64)}
+    for name, ptr, typestr in (("rec_off", p.rec_off, "<i8"), ("rec_kind", p.rec_kind, "|u1"), ("rec_flags", p.rec_flags, "|u1"),
+                               ("rec_rel", p.rec_rel, "<i4"), ("rec_schema", p.rec_schema, "<i4"), ("rec_start_lsn", p.rec_start_lsn, "<i8"),
+                               ("rec_commit_lsn", p.rec_commit_lsn, "<i8"), ("rec_tx_ordinal", p.rec_tx_ordinal, "<i8"),
+                               ("rec_cell_base", p.rec_cell_base, "<i8"), ("rec_tuple_bytes", p.rec_tuple_bytes, "<i4"),
+                               ("rec_heap_hint", p.rec_heap_hint, "<i4")):
+        a = take(ptr, n, typestr, ridx)
+        if typestr == "<i8":
+            out[name] = _split_u64(a.view(np.uint64))
+        else:
+            out[name] = (a.view(np.uint32) if typestr == "<i4" and name != "rec_schema" else a).astype(np.float64)
+    tag = take(p.cell_tag, m, "|u1", cidx)
+    val = take(p.cell_val, m, "<i8", cidx).view(np.uint64).copy()
+    val[np.isin(tag, HEAP_TAGS)] = 0
+    out["cell_tag"] = tag.astype(np.float64)
+    out["cell_val"] = _split_u64(val)
+    out["cell_aux"] = take(p.cell_aux, m, "<i4", cidx).view(np.uint32).astype(np.float64)
+    fe, co = s.first_error, s.carry_out
+    out["summary"] = _split_u64(np.array([n, m, s.insert_bytes, s.update_bytes, s.delete_bytes, s.n_events, fe.record_index, fe.seq,
+                                          fe.code, co.in_tx, co.final_lsn, co.next_tx_ordinal], dtype=np.uint64))
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, prefix + name + ".npy"), a)
 
 
 def materialise_leg(dec, st):
@@ -323,7 +388,7 @@ def materialise_leg(dec, st):
     return out
 
 
-def roofline_block(wname, nbytes, n_anchors, km, ms_per_step, last, scale):
+def roofline_block(nbytes, n_anchors, km, ms_per_step, last):
     """roofline of the dominant kernel + the whole pipeline.  km = mean (index, records, bins, rows, dead, kernel, long cells) ms."""
     peak, peak_src = measured_peak()
     algo_bytes = nbytes + 8 * (n_anchors + 1)              # SURVEY §8d: every staged byte once + the anchor index
@@ -336,23 +401,12 @@ def roofline_block(wname, nbytes, n_anchors, km, ms_per_step, last, scale):
     ktime = {"k_utf8_dead": float(km[4]), "k_rows": float(km[3])}
     dominant = max(ktime, key=lambda k: ktime[k])
     achieved = kbytes[dominant] / max(ktime[dominant], 1e-9) / 1e6
-    traffic, alone_us = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            tj = json.load(f)
-        traffic = tj.get(f"{wname}/{dominant}")
-        alone_us = tj.get(f"{wname}/{dominant}/serialised_us") if scale == 1.0 else None
-    except Exception:
-        pass
     kern = {"k_act*+k_chase": float(km[0]), "k_records": float(km[1]), "k_bin_scan+k_perm": float(km[2]),
             "k_rows+k_heavy+k_fix" + (" (k_rows streams the dead segments too)" if fused_dead else ""): float(km[3]),
             "k_utf8_dead (separate launch)": float(km[4]), "k_long_cells": float(km[6])}
     return {"bound": "hbm", "kernel": dominant, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": traffic, "peak_source": peak_src, "algorithmic_bytes_per_launch": kbytes[dominant],
+            "peak_source": peak_src, "algorithmic_bytes_per_launch": kbytes[dominant],
             "avg_launch_ms": ktime[dominant],
-            "alone_under_ncu": ({"ms": alone_us / 1e3, "achieved": kbytes[dominant] / (alone_us * 1e-6) / 1e9,
-                                 "frac": kbytes[dominant] / (alone_us * 1e-6) / 1e9 / peak,
-                                 "source": "profiles/traffic.json (ncu launch list: kernels serialised, not sharing HBM)"} if alone_us else None),
             "kernels_ms": kern,
             "k_rows": {"algorithmic_bytes": kbytes["k_rows"], "ms": ktime["k_rows"], "frac": kbytes["k_rows"] / max(ktime["k_rows"], 1e-9) / 1e6 / peak},
             "k_utf8_dead": {"algorithmic_bytes": span, "ms": ktime["k_utf8_dead"], "fused_into_k_rows": fused_dead,
@@ -360,7 +414,7 @@ def roofline_block(wname, nbytes, n_anchors, km, ms_per_step, last, scale):
             "pipeline": {"algorithmic_bytes": algo_bytes, "ms": ms_per_step,
                          "achieved": algo_bytes / (ms_per_step * 1e-3) / 1e9,
                          "frac": algo_bytes / (ms_per_step * 1e-3) / 1e9 / peak,
-                         "note": "algorithmic bytes ÷ the driver-visible step time (CUDA events around whole decode calls: every launch, memset, allocation and the final sync included)"}}
+                         "note": "algorithmic bytes ÷ the caller-visible step time (CUDA events around whole decode calls: every launch, memset, allocation and the final sync included)"}}
 
 
 def gpu_parity(dec_factory, w, arrays, preamble_needed, threads):
@@ -583,7 +637,7 @@ def measure_workload(torch, dev, name, scale, steps, warmup, stride, threads, cp
     _, box = host_cores()
     res = {"config": f"{w.name}: {w.description}", "scale": scale, "bytes": int(nbytes), "msgs": int(frames),
            "value": nbytes / (ms_step * 1e-3) / 1e9, "unit": "GB/s", "events_per_s": frames / (ms_step * 1e-3), "ms_per_step": ms_step,
-           "roofline": roofline_block(w.name, nbytes, st.n_anchors, km, ms_step, last, scale),
+           "roofline": roofline_block(nbytes, st.n_anchors, km, ms_step, last),
            "e2e": {"value": nbytes / (e_ms / steps * 1e-3) / 1e9, "unit": "GB/s", "ms_per_step": e_ms / steps,
                    "h2d_bytes_per_step": elast["h2d"], "d2h_bytes_per_step": elast["d2h"]},
            "e2e_materialised": ({"value": nbytes / ((e_ms / steps + mat["ms"]) * 1e-3) / 1e9, "unit": "GB/s", "shim": mat,
@@ -688,8 +742,11 @@ def main():
         decode_once(dec, st, True, sharded)[0].free()
     sampler = ClockSampler(local_rank)
     with sampler:
-        total_ms, km, launches, last = time_steps(torch, dist, dec, st, True, sharded, args.steps, dev, world)
+        total_ms, km, launches, last, last_bh = time_steps(torch, dist, dec, st, True, sharded, args.steps, dev, world, keep_last=True)
     ms_per_step = total_ms / args.steps
+    if args.dump_outputs:
+        dump_outputs(torch, dev, last_bh, args.dump_outputs, f"rank{rank}_" if world > 1 else "")
+    last_bh.free()
 
     e2e = None
     if not args.no_e2e:
@@ -778,10 +835,10 @@ def main():
                                        (f"{n_gpus} full-size byte ranges of one longer stream (weak scaling), seam + relation-update exchange over NCCL inside the library"
                                         if n_gpus > 1 else "single GPU")),
                        "scaling_note": "efficiency = value_N / (N * value_1): total bytes are fixed under strong scaling, per-GPU bytes under weak",
-                       "anchor_stride": args.stride, "l2_policy": "inputs (>=1.25 GiB per GPU) larger than the 126 MB L2",
+                       "anchor_stride": args.stride, "l2_policy": "inputs (>=1.25 GiB per GPU) larger than the 50 MB L2",
                        "timed_calls": "etl_dec_decode(_sharded) with ETL_DECODE_NO_TIMING; roofline.kernels_ms from two more calls with the summary timings on, outside the timed region",
                        "generate_s": round(gen_s, 2), "host_cores": {"box": box, "usable": usable}},
-            "roofline": roofline_block(w.name, nbytes, n_anchors, km, ms_per_step, last, args.scale),
+            "roofline": roofline_block(nbytes, n_anchors, km, ms_per_step, last),
             "gpu_launches": launches,
             "clocks": sampler.report(),
         }

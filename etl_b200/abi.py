@@ -1,7 +1,7 @@
 """ctypes binding of include/etl_decode.h (libetl_decode.so).
 
 This is the same binding a Rust / cgo / JNI shim would write (see INTEGRATION.md): plain pointers
-and sizes, no torch types.  The library is built in-tree by etl_b200.build (nvcc, sm_100a) and the
+and sizes, no torch types.  The library is built in-tree by etl_b200.build (nvcc, sm_90a) and the
 import fails loudly if it is missing — there is no CPU fallback for the decode path.
 """
 from __future__ import annotations
@@ -101,8 +101,8 @@ def load(build: bool = True):
     global _lib
     if _lib is not None:
         return _lib
-    # an existing in-tree library is loaded as is (the GPU box receives the prebuilt .so; file times are
-    # not preserved by the snapshot, so no staleness check here — `python -m etl_b200.build` rebuilds)
+    # an existing in-tree library is loaded as is (a copied tree need not preserve file times, so no staleness
+    # check here — build() and `python -m etl_b200.build` rebuild when the sources are newer)
     path = _build.DECODE_LIB
     if build and not os.path.exists(path):
         path = _build.build_decode()

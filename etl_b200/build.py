@@ -1,7 +1,7 @@
-"""In-tree native builds: libetl_decode.so (nvcc, sm_100a) and libwalgen.so (gcc).
+"""In-tree native builds: libetl_decode.so (nvcc, sm_90a — H100) and libwalgen.so (gcc).
 
-Built artefacts live next to the sources (git-ignored, shipped to the GPU box by gpurun).
-nvcc cross-compiles sm_100a without a GPU, so this also serves as the CPU-side "does it build" gate.
+Built artefacts live next to the sources (git-ignored).  nvcc cross-compiles sm_90a without a GPU, so the
+library can be built, and the build checked, on a machine that has none.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ INCLUDE = os.path.join(ROOT, "include")
 DECODE_LIB = os.path.join(PKG, "libetl_decode%s.so" % os.environ.get("ETL_LIB_SUFFIX", ""))
 WALGEN_LIB = os.path.join(PKG, "libwalgen.so")
 
-NVCC_ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
               "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

@@ -1,4 +1,4 @@
-// cell_parsers.cuh — device-side Postgres text → typed Cell parsers (sm_100a).
+// cell_parsers.cuh — device-side Postgres text → typed Cell parsers (sm_90a).
 //
 // Each parser is the GPU counterpart of one arm of parse_cell_from_postgres_text
 // (crates/etl/src/conversions/text.rs:28-173) and takes the cell's bytes through a generic pointer

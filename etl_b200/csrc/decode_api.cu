@@ -1,10 +1,10 @@
-// decode_api.cu — extern "C" ABI (include/etl_decode.h) of the B200 pgoutput decode engine.
+// decode_api.cu — extern "C" ABI (include/etl_decode.h) of the H100 pgoutput decode engine.
 //
 // Host side only does what the reference does per batch / per Relation message (rare, control
 // path): staging, schema catalogue, Relation → ReplicationMask / IdentityMask
 // (apply.rs:2012-2089, event.rs:325-369, etl-postgres/src/types/schema.rs:288-323,406-438,527-535),
 // buffer management and kernel orchestration.  Every per-row / per-cell operation of the hot path
-// runs in the sm_100a kernels of wal_kernels.cuh / rows_kernel.cuh; there is no CPU decode fallback.
+// runs in the sm_90a kernels of wal_kernels.cuh / rows_kernel.cuh; there is no CPU decode fallback.
 //
 // One decode = one host synchronisation, at the end.  The planes are sized from what the previous
 // batches needed per staged byte; k_chase / k_records compare the real totals with the reservation on the device and,
@@ -591,7 +591,7 @@ void etl_dec_batch_free(etl_dec_batch* b) {
 // Where the structure-blind UTF-8 pass (k_utf8_dead, HBM-bound) runs relative to the latency-bound passes.
 // 0: side stream from the start of the index pass; 1: side stream from the start of the tuple pass (default);
 // 2 (default): main stream after the tuple pass; 3: inside k_rows — its warps stream the dead segments after their rows.
-// Measured on C5 (10 GiB, round 2): 2 → 3.66 ms per decode, 0 → 3.96, 1 → 4.10, 3 → 4.24: k_rows fills the register file and
+// Measured on C5 (10 GiB): 2 is the fastest, then 0, 1 and 3: k_rows fills the register file and
 // is bound by instruction issue, the UTF-8 pass needs every SM's warps to saturate HBM — sharing the SMs helps neither.
 // ETL_DEAD_MODE is a tuning knob for measurement, not part of the ABI.
 static int dead_mode() {
@@ -610,7 +610,7 @@ static uint32_t dead_grid(const DecodeParams& P) {   // 8 warps per CTA, kDeadSe
 }
 static int sm_count(etl_dec_ctx* ctx) {
   static int sms = 0;
-  if (!sms) { sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device); }
+  if (!sms) { sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device); }
   return sms;
 }
 static cudaError_t launch_dead_side(etl_dec_ctx* ctx, cudaStream_t st) {
@@ -1223,7 +1223,7 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
   etl_dec_summary& S = b->summary;
   memset(&S, 0, sizeof S);
   float h2d_ms = 0, index_ms = 0, emit_ms = 0, d2h_ms = 0;
-  if (!(ctx->pending_flags & ETL_DECODE_NO_TIMING)) {          // ten event queries: ~25 us of host time on an 8 MiB batch
+  if (!(ctx->pending_flags & ETL_DECODE_NO_TIMING)) {          // ten event queries: host time an 8 MiB batch notices
     cudaEventElapsedTime(&h2d_ms, ctx->ev[0], ctx->ev[1]);
     cudaEventElapsedTime(&index_ms, ctx->ev[1], ctx->ev[2]);
     cudaEventElapsedTime(&emit_ms, ctx->ev[3], ctx->ev[4]);

@@ -7,7 +7,7 @@
 //   * ArrayCell construction from the heap's element lists,
 //   * Event::size_hint per event (types/event.rs:288-312 over types/table_row.rs:250-345) so that the byte-budget
 //     flush of the apply loop (apply.rs:1611-1624) sees the numbers the reference would have computed.
-// No Rust toolchain exists in this image, so this is C++ with the Rust struct sizes as parameters (etl_rust_layout:
+// The build needs no Rust toolchain, so this is C++ with the Rust struct sizes as parameters (etl_rust_layout:
 // a real shim passes std::mem::size_of values).  Pure host code: it never touches the GPU and is timed separately
 // (bench.py `e2e_materialised`).
 #include <algorithm>

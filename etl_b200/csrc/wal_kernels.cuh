@@ -1,4 +1,4 @@
-// wal_kernels.cuh — sm_100a kernels of the batched pgoutput decode path (launch order):
+// wal_kernels.cuh — sm_90a kernels of the batched pgoutput decode path (launch order):
 //
 //   k_act_count/scan/scatter  list the anchor segments that contain a frame start (`act`) and those that do
 //                       not (`dead`): TOAST-heavy streams leave most segments empty.
@@ -449,7 +449,7 @@ __global__ void __launch_bounds__(kActThreads) k_act_small(DecodeParams P) {
 // counts of its predecessors), and a second walk over the now cached length fields writes every frame's offset
 // into `frame_off` in stream order.  Everything after this pass is record-parallel: one thread per frame, coalesced.
 // (Round 1/2a walked the chain twice with the whole per-frame state machine inside the walk — k_index, k_frames:
-// 10 serial hops of ~5 µs each for a 2 KiB segment of 200-byte frames, 60 % of the time of an 8 MiB batch.)
+// 10 serial hops for a 2 KiB segment of 200-byte frames, most of the time of an 8 MiB batch.)
 __device__ __forceinline__ Summ ld_summ_cg(const Summ* p) {      // L2 (another CTA wrote it)
   const uint4 a = __ldcg(reinterpret_cast<const uint4*>(p)), b = __ldcg(reinterpret_cast<const uint4*>(p) + 1);
   Summ r;
@@ -733,7 +733,7 @@ __device__ __forceinline__ bool utf8_range_bad(const uint8_t* cell, uint32_t cel
 // (4 coalesced 16-byte loads per lane) per pass; the bitmap is written only where a violation is found.
 // Short-lived CTAs (a warp takes kDeadSegsPerWarp consecutive dead segments and retires): the pass runs on a low-priority
 // side stream underneath latency-bound kernels, and a persistent grid would sit on every SM's thread slots until it is
-// done — k_bin_scan / k_perm waited 1.6 ms for a slot behind it (round-2 sweep).  The grid is sized for "every segment dead".
+// done — k_bin_scan / k_perm waited for a slot behind it (round-2 sweep).  The grid is sized for "every segment dead".
 constexpr uint32_t kDeadSegsPerWarp = 4;
 // Work item i of the dead-segment pass = 2 KiB pass (i % ppseg) of dead segment (i / ppseg), ppseg = passes per segment.
 // The verdict of one lane's 64 bytes [off, off + 64) of a dead-segment item that ends at s1: x = the four 16-byte chunks,
@@ -763,7 +763,7 @@ __device__ __forceinline__ void utf8_dead_verdict(const DecodeParams& P, const u
 // One item per warp step: every lane owns 64 contiguous bytes (half a 128-byte line), four 16-byte loads in flight before the
 // first byte is looked at; the three bytes before a lane's first chunk come from one 4-byte load that hits L1 — no shuffles
 // (round 1 paid three __shfl per 16 bytes).  Measured: 4 items (16 loads) per lane cost 102 registers and a quarter of the
-// warps — 2.14 ms instead of 1.46 ms on C5.
+// warps, and the pass was slower on C5.
 __device__ __forceinline__ void utf8_dead_items(const DecodeParams& P, uint32_t it, uint32_t, uint32_t n_items, uint32_t ppseg, uint32_t lane) {
   uint4 x[4];
   uint32_t pw = 0;
@@ -867,7 +867,7 @@ __global__ void __launch_bounds__(1024) k_bin_scan(DecodeParams P) {
 }
 // k_perm: CTA-local counting first (shared-memory histogram), then ONE global atomic per occupied bin per CTA.
 // (Round 1 issued one global atomic per bin per WARP: a single-table stream has ~8 occupied bins, so 75 k warps
-// queued on 8 addresses — 0.2 ms on C5 for what is a 10 MB permutation.)
+// queued on 8 addresses, a visible cost for what is a 10 MB permutation.)
 constexpr int kPermThreads = 1024;
 __global__ void __launch_bounds__(kPermThreads) k_perm(DecodeParams P) {
   __shared__ uint32_t hist[kMaxBins];                 // count of the CTA's records per bin, then the CTA's base in the bin
@@ -914,9 +914,9 @@ __global__ void __launch_bounds__(kPermThreads) k_perm(DecodeParams P) {
 #ifndef ETL_REC_THREADS
 #define ETL_REC_THREADS 512
 #endif
-// Records per CTA, one thread each.  The look-back chain advances one window of 32 CTAs per L2 round trip (~1.5 us with
-// the fold): with 256 records per CTA that alone capped the pass at 5.5 records/ns on every workload (C2 / C4 / C5:
-// 0.164 / 0.185 / 0.158 ns per record, ncu: a third of the samples at the barrier behind the look-back warp).
+// Records per CTA, one thread each.  The look-back chain advances one window of 32 CTAs per L2 round trip (with the
+// fold): with 256 records per CTA that alone capped the pass on every workload (ncu: a third of the samples at the
+// barrier behind the look-back warp).
 constexpr int kRecThreads = ETL_REC_THREADS;
 constexpr int kRecCtaThreads = kRecThreads + 32;      // + the look-back warp
 struct ScanSlot { Summ aggr; Summ incl; };

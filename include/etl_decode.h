@@ -1,5 +1,5 @@
 /*
- * etl_decode.h — C ABI of the B200 batched pgoutput (CDC) decode engine.
+ * etl_decode.h — C ABI of the H100 batched pgoutput (CDC) decode engine.
  *
  * This is the drop-in boundary for supabase/etl's streaming-replication hot path. The reference
  * has no FFI seam at the decoder; the entry points below are what a Rust shim in `crates/etl`
@@ -291,7 +291,7 @@ enum {
   ETL_DECODE_SEAM_DEFER = 0x2,      /* multi-GPU shard: carry_in unknown, run only the local scan;
                                        caller exchanges etl_dec_seam and calls etl_dec_decode_finish */
   ETL_DECODE_NO_TIMING = 0x4,       /* leave the *_ms fields of the summary at 0: the CUDA-event queries behind them cost
-                                       ~25 us of host time per call, which an 8 MiB batch notices */
+                                       host time on every call, which an 8 MiB batch notices */
 };
 
 /* per-shard seam summary exchanged with ONE all-gather across the GPUs of a box (SURVEY §8e) */

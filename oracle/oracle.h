@@ -4,10 +4,10 @@
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
  * load this. The product (etl_b200/, libetl_decode.so) never links or calls it.
  *
- * Parity status: the reference (Rust) cannot be built in this image (no cargo/rustc, un-vendored
- * crates), so this is a restatement ("port"). It is pinned against every known-answer test the
+ * Parity status: the reference (Rust) needs a Rust toolchain and its un-vendored crates to build,
+ * so this is a restatement ("port"). It is pinned against every known-answer test the
  * reference holds for the path (tests/test_oracle_reference_vectors.py quotes them with
- * file:line). Behaviour that lives in third-party crates absent from /root/reference and is not
+ * file:line). Behaviour that lives in third-party crates absent from the reference tree and is not
  * covered by an in-tree reference test is marked "parity unpinned" where it is implemented
  * (chrono leniency, uuid alternate spellings, serde_json depth limit, pgoutput Begin/Commit/
  * Relation/Insert/Truncate layouts which follow the PostgreSQL protocol documentation).

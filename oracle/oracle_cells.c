@@ -2,7 +2,7 @@
  * oracle_cells.c — CPU restatement of crates/etl/src/conversions/{text,numeric,hex,bool}.rs.
  * TEST INFRASTRUCTURE ONLY (see oracle.h). Each function cites the reference lines it follows.
  *
- * Library behaviour restated here because the crates are not under /root/reference:
+ * Library behaviour restated here because the crates are not part of the reference tree:
  *   Rust core str::parse (ints, floats)      — toolchain 1.93.1 (rust-toolchain.toml)
  *   chrono 0.4.44 parse_from_str             — Cargo.lock:1122-1123   (leniency: parity unpinned)
  *   uuid 1.23.1 Uuid::parse_str              — Cargo.lock:6946-6947   (alt spellings: parity unpinned)

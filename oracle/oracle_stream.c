@@ -2,7 +2,7 @@
  * oracle_stream.c — CPU restatement of the streaming hot path driver.  TEST INFRASTRUCTURE ONLY.
  *
  *   frame / message parse : third-party postgres-replication 0.6.7 (git rev 31acf55, Cargo.lock:4486-4498),
- *                           not under /root/reference → follows the PostgreSQL protocol docs
+ *                           not part of the reference tree → follows the PostgreSQL protocol docs
  *                           ("Logical Replication Message Formats", proto v1) and the bytes the
  *                           reference's own tests hand-encode (event.rs:1068-1146). parity unpinned
  *                           for Begin/Commit/Relation/Insert/Truncate/Message/XLogData header.

@@ -1,6 +1,6 @@
 // host_parsers.cpp — TEST INFRASTRUCTURE ONLY.
 // Compiles the DEVICE cell parsers (etl_b200/csrc/cell_parsers.cuh, float_parse.cuh — the very sources nvcc
-// compiles for sm_100a) for the host with one-lane stand-ins for the warp intrinsics, so that the CPU suite can
+// compiles for sm_90a) for the host with one-lane stand-ins for the warp intrinsics, so that the CPU suite can
 // fuzz them against the oracle with millions of spellings (tests/test_device_parsers_on_host.py).  It is not a
 // product path and nothing outside tests/ loads it: the product has no CPU fallback.
 //

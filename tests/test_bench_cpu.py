@@ -1,5 +1,5 @@
 """bench.py's reference arm runs on the CPU (oracle port on the host cores): exercise it on the tiny C1
-workload and check the JSON contract the driver reads."""
+workload and check the JSON contract of its output line."""
 import json
 import os
 import subprocess

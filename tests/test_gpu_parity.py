@@ -1,6 +1,6 @@
 """GPU parity: the CUDA decode path (through the C ABI) vs the CPU oracle, bit-exact.
 
-Runs on the B200 box (`pytest -m gpu`).  Nothing here reads /root/reference.
+Runs on an H100 (`pytest -m gpu`).  Nothing here reads the reference checkout.
 """
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
 """Sharded decode on several GPUs of one box (etl_dec_decode_sharded: NCCL seam all-gather + device-side fold +
 relation-update exchange, all inside the library), checked against the oracle's decode of the whole stream.
-Needs >= 2 GPUs (`gpurun --gpus 2`); skipped otherwise.  Also: context leak check and parity at BASELINE sizes."""
+The NCCL cases need one GPU per rank and skip on a smaller machine.  Also: context leak check and parity at BASELINE sizes."""
 import os
 import subprocess
 import sys

@@ -1,7 +1,7 @@
 """Type oid → decode class: the product's catalogue table (etl_b200/csrc/oid_classes.h, through the C ABI) and the
 oracle's switch (oracle/oracle_cells.c) are two independent statements of text.rs:28-173 + utils.rs:7-16; both are
 checked against tests/golden/oid_classes.json, extracted from the reference's own match arms by
-tools/make_oid_golden.py (which needs /root/reference and therefore ran in the build container)."""
+tools/make_oid_golden.py (which needs a checkout of the reference, so its output is committed)."""
 import json
 import os
 

@@ -1,6 +1,6 @@
 """Pins the CPU oracle against every known-answer test the reference holds for the path
 (SURVEY.md §8c).  Each block quotes the reference test it restates (file:line under
-/root/reference/crates/etl/src/conversions/).  Pure CPU; no GPU, no /root/reference access.
+crates/etl/src/conversions/ of supabase/etl).  Pure CPU; no GPU, no access to the reference checkout.
 """
 import datetime as dt
 import struct

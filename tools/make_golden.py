@@ -3,7 +3,7 @@
 small instances of the five BASELINE workloads.  The digest is over `repr(planes_to_events(...))` (typed
 values dereferenced from the stream / heap, so heap placement does not matter).
 
-The reference is a Rust workspace that cannot be built in this image (no cargo), so these fixtures pin the
+The reference is a Rust workspace that the build does not compile (no Rust toolchain needed), so these fixtures pin the
 ORACLE (which is itself pinned to the reference's known-answer tests, see tests/test_oracle_*.py) and
 let the GPU path be checked against committed bytes instead of against a freshly built checker.
 Usage: python tools/make_golden.py"""

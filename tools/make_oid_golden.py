@@ -1,15 +1,16 @@
 #!/usr/bin/env python
 """Writes tests/golden/oid_classes.json from the reference's own dispatch: every `Type::NAME` in the match arms of
-parse_cell_from_postgres_text (/root/reference/crates/etl/src/conversions/text.rs:28-173) is mapped to the ETL_K_*
+parse_cell_from_postgres_text (crates/etl/src/conversions/text.rs:28-173 of supabase/etl) is mapped to the ETL_K_*
 class of its arm and to its oid (PostgreSQL's pg_type catalogue, the constants `postgres-types` generates its
-`Type::NAME` items from).  Runs only where /root/reference exists (the build container); the JSON is committed.
-Usage: python tools/make_oid_golden.py"""
+`Type::NAME` items from).  Needs a checkout of the reference; the JSON is committed, so the tests do not.
+Usage: python tools/make_oid_golden.py <supabase/etl checkout>"""
 import json
 import os
 import re
+import sys
 
 ROOT = os.path.normpath(os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-SRC = "/root/reference/crates/etl/src/conversions/text.rs"
+SRC = os.path.join(sys.argv[1] if len(sys.argv) > 1 else ".", "crates/etl/src/conversions/text.rs")
 # pg_type.dat: typname → oid for the names the reference dispatches on
 PG = dict(BOOL=16, BYTEA=17, CHAR=18, NAME=19, INT8=20, INT2=21, INT4=23, TEXT=25, OID=26, JSON=114, FLOAT4=700, FLOAT8=701, MONEY=790,
           BPCHAR=1042, VARCHAR=1043, DATE=1082, TIME=1083, TIMESTAMP=1114, TIMESTAMPTZ=1184, NUMERIC=1700, UUID=2950, JSONB=3802,

@@ -36,8 +36,9 @@ CLASSES = [("LDG.E.U8 (byte loads from global)", r"\bLDG\.E\.U8"), ("LDG (all gl
            ("SHFL", r"\bSHFL\b"), ("VOTE / MATCH", r"\b(VOTE|MATCH|VOTEU)\b"), ("MEMBAR", r"\bMEMBAR"), ("ATOM/RED (global atomics)", r"\b(ATOMG|ATOM|RED)\b")]
 want = ["k_rows", "k_heavy", "k_records", "k_chase", "k_utf8_dead", "k_long_cells", "k_copy_rows", "k_perm", "k_fix"]
 out = os.path.join(ROOT, "profiles", f"{rnd}_sass.txt")
+os.makedirs(os.path.dirname(out), exist_ok=True)
 with open(out, "w") as f:
-    f.write("cuobjdump -sass / -res-usage etl_b200/libetl_decode.so (sm_100a), per kernel: resources, instruction-class counts,\n"
+    f.write("cuobjdump -sass / -res-usage etl_b200/libetl_decode.so (sm_90a), per kernel: resources, instruction-class counts,\n"
             "and the SASS around every bulk copy / mbarrier operation (tools/sass_excerpt.py)\n\n")
     for name, lines in kernels.items():
         short = next((w for w in want if w in name), None)
