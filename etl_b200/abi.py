@@ -67,7 +67,7 @@ class Summary(C.Structure):
                 ("n_schemas", C.c_uint32), ("gpu_launches", C.c_uint32), ("kernel_ms", C.c_float),
                 ("h2d_ms", C.c_float), ("d2h_ms", C.c_float), ("index_ms", C.c_float),
                 ("emit_ms", C.c_float), ("frames_ms", C.c_float), ("walk_ms", C.c_float), ("spans_ms", C.c_float), ("cells_ms", C.c_float), ("long_ms", C.c_float), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("span_bytes", C.c_uint64),
-                ("record_index_base", C.c_uint64), ("abi_version", C.c_uint32), ("_pad2", C.c_uint32)]
+                ("record_index_base", C.c_uint64), ("abi_version", C.c_uint32), ("sizing", C.c_uint32)]
 
 
 class SchemaInfo(C.Structure):
@@ -171,3 +171,15 @@ def load(build: bool = True):
 
 RESULTS_TO_HOST = 0x1
 NO_TIMING = 0x4
+
+# etl_dec_summary.sizing bits (ETL_SIZING_*)
+SIZING_EXACT = 0x01
+SIZING_OPTIMISTIC = 0x02
+SIZING_RERUN_RECORDS = 0x04
+SIZING_RERUN_CELLS = 0x08
+SIZING_SCRATCH_RESTART = 0x10
+SIZING_ARRAY_HEAP_RETRY = 0x20
+SIZING_LONG_PASSES_LATE = 0x40
+SIZING_NAMES = {SIZING_EXACT: "EXACT", SIZING_OPTIMISTIC: "OPTIMISTIC", SIZING_RERUN_RECORDS: "RERUN_RECORDS",
+                SIZING_RERUN_CELLS: "RERUN_CELLS", SIZING_SCRATCH_RESTART: "SCRATCH_RESTART",
+                SIZING_ARRAY_HEAP_RETRY: "ARRAY_HEAP_RETRY", SIZING_LONG_PASSES_LATE: "LONG_PASSES_LATE"}

@@ -1037,7 +1037,10 @@ static int launch_emit_kernels(etl_dec_ctx* ctx) {
     cudaEventRecord(ctx->evk[3], st);
     if (cap_r && !ctx->long_skipped) { k_long_cells<<<sm_count(ctx) * 8, 256, 0, st>>>(P); ctx->launches += 1; }
     CK(cudaGetLastError());
-  } else { CK(cudaMemsetAsync(P.total, 0, sizeof(Summ), st)); cudaEventRecord(ctx->evk[0], st); cudaEventRecord(ctx->evk[2], st); cudaEventRecord(ctx->evk[1], st); cudaEventRecord(ctx->evk[3], st); cudaEventRecord(ctx->ev_l0, st); cudaEventRecord(ctx->ev_l1, st); }
+  } else {
+    // an empty batch: no k_records writes rec_cell_base[0] (the planes come from the pool, not zeroed)
+    CK(cudaMemsetAsync(P.total, 0, sizeof(Summ), st)); CK(cudaMemsetAsync(P.rec_cell_base, 0, 8, st));
+    cudaEventRecord(ctx->evk[0], st); cudaEventRecord(ctx->evk[2], st); cudaEventRecord(ctx->evk[1], st); cudaEventRecord(ctx->evk[3], st); cudaEventRecord(ctx->ev_l0, st); cudaEventRecord(ctx->ev_l1, st); }
   CK(cudaEventRecord(ctx->ev[4], st));
   CK(cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars.ptr(), kScalarWords * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
@@ -1051,15 +1054,19 @@ static int launch_emit_kernels(etl_dec_ctx* ctx) {
 static Summ carry_of(const etl_stream_state* cin) {
   Summ carry = summ_identity();
   if (cin) {
-    if (cin->in_tx) { carry.flags = S_HAS_B; carry.lsn = cin->final_lsn; }
+    if (cin->in_tx) carry.flags = S_HAS_B;
+    // final_lsn of the last Begin passes through a batch without one even outside a transaction (only read while
+    // in_tx): a batch of keepalives hands on the carry it received, as one decode of the joined batches would
+    carry.lsn = cin->final_lsn;
     carry.ord = cin->next_tx_ordinal;
   }
   return carry;
 }
 
-// one decode, common to every entry point.  mode 0: one-shot (optimistic sizing); 1: after decode_begin (totals known)
+// one decode, common to every entry point.  mode 0: one-shot (optimistic sizing); 1: after decode_begin (totals known).
+// `sizing`: ETL_SIZING_* bits of an abandoned attempt (scratch restart), reported together with this one's
 static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64_t record_index_base, bool sharded, bool totals_known,
-                      etl_dec_batch** out, bool force_exact = false) {
+                      etl_dec_batch** out, bool force_exact = false, uint32_t sizing = 0) {
   cudaStream_t st = ctx->stream;
   DecodeParams& P = ctx->P;
   etl_dec_batch* b = new etl_dec_batch();
@@ -1092,6 +1099,7 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
     memcpy(ctx->h_scalars + kScalarWords, &dc, sizeof dc);
     CKB(cudaMemcpyAsync(ctx->d_scalars.ptr() + kScalarWords * 8, ctx->h_scalars + kScalarWords, sizeof dc, cudaMemcpyHostToDevice, st));
   }
+  sizing |= exact ? ETL_SIZING_EXACT : ETL_SIZING_OPTIMISTIC;
   PlaneLayout L{};
   uint64_t scalar_heap = 0, array_heap = 0, heap_used = 0;
   if (!totals_known && !exact) {
@@ -1140,6 +1148,7 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
     if (ctx->long_skipped && ctx->h_scalars[7] && !ctx->h_scalars[13]) {
       // the frame-length hint was wrong: long values exist.  Run the passes that were left out, read the scalars again.
       ctx->long_skipped = false;
+      sizing |= ETL_SIZING_LONG_PASSES_LATE;
       CKB(cudaMemsetAsync(P.line_bad, 0, ((P.len + 4095) / 4096 + 1) * 4, st));
       k_utf8_dead<<<dead_grid(P), 256, 0, st>>>(P);
       k_long_cells<<<sm_count(ctx) * 8, 256, 0, st>>>(P);
@@ -1156,9 +1165,10 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
       // Sharded: every rank sees the same gathered blocks, so every rank takes this branch and the exchange is repeated.
       if (force_exact) { ctx->last_error = "offset scratch overflow on the exact path"; return fail(ETL_ERR_CUDA); }
       fail(0);
-      return run_decode(ctx, carry_in, record_index_base, sharded, false, out, true);
+      return run_decode(ctx, carry_in, record_index_base, sharded, false, out, true, sizing | ETL_SIZING_SCRATCH_RESTART);
     }
     if (aborted) {                                     // did not fit the optimistic planes: exact sizes, pass C again
+      sizing |= ((aborted & ABORT_RECORDS) ? ETL_SIZING_RERUN_RECORDS : 0u) | ((aborted & ABORT_CELLS) ? ETL_SIZING_RERUN_CELLS : 0u);
       CKB(reset_abort());
       if (int rc = launch_summary(ctx)) return fail(rc);
       CKB(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
@@ -1174,6 +1184,7 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
     if (ctx->h_scalars[9]) {                          // an array reservation did not fit: larger array region, pass C again
       if (attempt >= 4) { ctx->last_error = "array heap reservation overflow after retries"; return fail(ETL_ERR_CUDA); }
       array_heap = (P.heap_cap - scalar_heap) * 4;
+      sizing |= ETL_SIZING_ARRAY_HEAP_RETRY;
       exact = true;
       ctx->lines_launched = false;
       CKB(cudaMemsetAsync(P.line_bad, 0, ((P.len + 4095) / 4096 + 1) * 4, st));
@@ -1269,6 +1280,7 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
   S.carry_out.final_lsn = endst.lsn;
   S.carry_out.next_tx_ordinal = endst.ord;
   S.abi_version = ETL_DECODE_ABI_VERSION;
+  S.sizing = sizing;
 
   // ---- note_ready (apply.rs:2079): the Relation frames of the valid prefix become the state of the next batch.
   // After a data error the reference has bailed out before caching anything that follows it.
@@ -1462,6 +1474,7 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
   cudaEventElapsedTime(&S.d2h_ms, ctx->ev[4], ctx->ev[5]);
   S.kernel_ms = S.emit_ms; S.cells_ms = S.emit_ms;
   S.h2d_bytes = h2d; S.d2h_bytes = d2h; S.gpu_launches = ctx->launches; S.abi_version = ETL_DECODE_ABI_VERSION;
+  S.sizing = ETL_SIZING_EXACT | (array_heap > (any_array ? 3 * in->len + 4096 : 0) ? ETL_SIZING_ARRAY_HEAP_RETRY : 0u);
   const unsigned long long key = ctx->h_scalars[0];
   if (key == ~0ull) S.first_error.record_index = UINT64_MAX;
   else {

@@ -75,6 +75,7 @@ class DecodedBatch:
     h2d_bytes: int = 0
     d2h_bytes: int = 0
     record_index_base: int = 0
+    sizing: int = 0      # abi.SIZING_* bits: how the planes were sized (diagnostic)
 
 
 @dataclass
@@ -381,4 +382,4 @@ class BatchHandle:
             n_events=int(s.n_events), schemas=self.schemas(), kernel_ms=float(s.kernel_ms), h2d_ms=float(s.h2d_ms),
             d2h_ms=float(s.d2h_ms), gpu_launches=int(s.gpu_launches), result_bytes=int(nbytes),
             index_ms=float(s.index_ms), emit_ms=float(s.emit_ms), h2d_bytes=int(s.h2d_bytes), d2h_bytes=int(s.d2h_bytes),
-            record_index_base=int(s.record_index_base))
+            record_index_base=int(s.record_index_base), sizing=int(s.sizing))

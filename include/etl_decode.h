@@ -371,8 +371,28 @@ typedef struct etl_dec_summary {
   uint64_t span_bytes;    /* bytes streamed by k_utf8_dead (its algorithmic bytes) */
   uint64_t record_index_base; /* global index of this batch's first record (sharded decode: Σ records of the ranks before) */
   uint32_t abi_version;
-  uint32_t _pad2;
+  uint32_t sizing;        /* ETL_SIZING_* bits: how the planes of this batch were sized, every branch the decode went through */
 } etl_dec_summary;
+
+/* etl_dec_summary.sizing — diagnostic only (the planes are the same whichever path was taken; a shim may log how often
+ * the optimistic sizes miss).  The first batch of a context, decode_finish and COPY rows size the planes from exact
+ * counts (EXACT).  Every later batch reserves planes from what earlier batches needed per staged byte (OPTIMISTIC); when
+ * the device reports that the batch does not fit, the host counts it exactly and runs the tuple pass again
+ * (RERUN_RECORDS: more records than reserved, nothing was written; RERUN_CELLS: more cells than reserved, the records
+ * of the CTAs before the overflow were written and are overwritten).  More frames than the offset scratch holds
+ * abandons the attempt and decodes the batch again on the exact path (SCRATCH_RESTART, together with the bits of the
+ * abandoned attempt and EXACT).  An array value that did not fit its heap reservation: larger heap, tuple pass again
+ * (ARRAY_HEAP_RETRY).  The frame-length hint promised no long values but there were some: the long-value passes ran
+ * after the tuple pass (LONG_PASSES_LATE). */
+enum {
+  ETL_SIZING_EXACT = 0x01,
+  ETL_SIZING_OPTIMISTIC = 0x02,
+  ETL_SIZING_RERUN_RECORDS = 0x04,
+  ETL_SIZING_RERUN_CELLS = 0x08,
+  ETL_SIZING_SCRATCH_RESTART = 0x10,
+  ETL_SIZING_ARRAY_HEAP_RETRY = 0x20,
+  ETL_SIZING_LONG_PASSES_LATE = 0x40,
+};
 
 int etl_dec_batch_planes(const etl_dec_batch*, int host, etl_dec_planes* out);
 int etl_dec_batch_summary(const etl_dec_batch*, etl_dec_summary* out);

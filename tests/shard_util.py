@@ -22,6 +22,29 @@ def mid_tx_cuts(full, n_parts: int) -> List[int]:
     return cuts
 
 
+def schema_maps(full, parts: Sequence, cuts: Sequence[int]) -> List[List[int]]:
+    """Per range: local schema index → index in `full.schemas` (the whole-stream decode).  A range numbers its
+    schema versions itself: the versions in force at its first byte (effective_off 0), then its own Relation frames
+    (effective_off = offset inside the range).  A range must therefore not start with a Relation frame: its
+    effective_off would be 0 as well."""
+    want_index = {}
+    for i, s in enumerate(full.schemas):
+        want_index.setdefault(int(s.table_id), []).append((int(s.effective_off), i))
+    maps = []
+    for k, p in enumerate(parts):
+        m = []
+        for s in p.schemas:
+            off = s.effective_off + cuts[k] if s.effective_off else None      # None: the version in force at the range's first byte
+            cands = want_index[s.table_id]
+            if off is None:
+                prior = [i for (o, i) in cands if o < cuts[k]] or [cands[0][1]]
+                m.append(prior[-1])
+            else:
+                m.append(next(i for (o, i) in cands if o == off))
+        maps.append(m)
+    return maps
+
+
 def stitch(parts: Sequence, cuts: Sequence[int], schema_maps=None):
     """Concatenate per-range DecodedBatch objects (range k starts at byte cuts[k]) into one batch in the layout of
     a whole-stream decode.  Array cells are left out of the heap fix-up (not used by these tests).

@@ -11,7 +11,7 @@ import pytest
 
 from canon import assert_planes_equal
 from etl_b200 import workloads as wl
-from shard_util import mid_tx_cuts, stitch
+from shard_util import mid_tx_cuts, schema_maps, stitch
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -67,22 +67,7 @@ def test_sharded_decode_matches_oracle(oracle_mod, tmp_path, name, scale, world,
         base += p.n_records
     assert base == full.n_records
     # schema numbering is per range (carried-in versions first): map every range's indices to the whole-stream numbering
-    want_index = {}
-    for i, s in enumerate(full.schemas):
-        want_index.setdefault(int(s.table_id), []).append((int(s.effective_off), i))
-    maps = []
-    for k, p in enumerate(parts):
-        m = []
-        for s in p.schemas:
-            off = s.effective_off + cuts[k] if s.effective_off else None      # None: the version in force at the range's first byte
-            cands = want_index[s.table_id]
-            if off is None:
-                prior = [i for (o, i) in cands if o < cuts[k]] or [cands[0][1]]
-                m.append(prior[-1])
-            else:
-                m.append(next(i for (o, i) in cands if o == off))
-        maps.append(m)
-    got = stitch(parts, cuts, maps)
+    got = stitch(parts, cuts, schema_maps(full, parts, cuts))
     got.schemas = full.schemas                          # compared through the mapping above
     got.carry_out = parts[-1].carry_out
     assert_planes_equal(got, full, raw)
