@@ -438,7 +438,8 @@ int etl_dec_copy_decode(etl_dec_ctx*, uint32_t table_id, const etl_copy_input*, 
  * Replaces the per-row walk of the destinations' encoders (crates/etl-destinations/src/iceberg/encoding.rs:61-330:
  * build_array_for_field and the cell_to_* converters; the DuckLake / BigQuery encoders walk the same Vec<TableRow>) for
  * the column types whose Arrow value depends on the decoded cell alone.  Numeric / Json / Array columns (cell_to_string
- * formatting in the reference) come back as ETL_ARROW_UNSUPPORTED and stay on the shim's row path.
+ * formatting in the reference) come back as ETL_ARROW_UNSUPPORTED and stay on the shim's row path unless row_kinds has
+ * ETL_ARROW_ALL_COLUMNS (below): then they are built on the device too.
  * row_kinds: bit 0 inserts, bit 1 updates (new image, Full rows only), bit 2 deletes (old image, when Full); rows keep
  * stream order and etl_dec_arrow_row_records gives the record index of each (for the CDC columns). */
 enum {
@@ -455,7 +456,21 @@ enum {
   ETL_ARROW_TIMESTAMP_US = 10,  /* naive, microseconds since the epoch (:284-289) */
   ETL_ARROW_TIMESTAMPTZ_US = 11,/* UTC, microseconds since the epoch (:297-302) */
   ETL_ARROW_UUID = 12,          /* FixedSizeBinary(16) */
+  ETL_ARROW_LIST = 13,          /* List<child>: validity + int32 offsets[n_rows + 1]; values / data NULL; the child column
+                                   through etl_dec_arrow_list_child (ETL_ARROW_ALL_COLUMNS only) */
 };
+/* row_kinds bit: build every column type of the reference's Iceberg schema (iceberg/schema.rs:9-63).  Numeric and Json
+ * columns come back as ETL_ARROW_UTF8 holding cell_to_string's text (encoding.rs:338-360): PgNumeric's Display
+ * (numeric.rs:503-590) and serde_json::Value's Display — compact, object keys sorted by their unescaped UTF-8 bytes, the
+ * last of duplicate keys kept, numbers verbatim, strings escaped the serde_json way (third-party behaviour, parity
+ * unpinned).  Array columns come back as ETL_ARROW_LIST (build_list_array, encoding.rs:386-776): a non-array or NULL cell
+ * is a null list, `{}` a list of length 0, a NULL element a null child entry; child types Bool → BOOLEAN,
+ * I16 / I32 → INT32, I64 / U32 → INT64, F32, F64, Date → DATE32, Time → TIME64_US, Timestamp / TimestampTz →
+ * TIMESTAMP_US / TIMESTAMPTZ_US, Uuid → UUID, Bytes → LARGE_BINARY, String / Numeric / Json → UTF8 (formatted as above).
+ * Without the bit the output is that of the emitter before it existed.  More than INT32_MAX elements in one List column,
+ * or more than 2 GiB of text in a Utf8 child, fail like an oversize Utf8 column (ETL_ERR_INVALID_ARG: split the batch); a
+ * Json value that does not parse again (the decode validated it) is ETL_ERR_INTERNAL. */
+#define ETL_ARROW_ALL_COLUMNS 0x100u
 typedef struct etl_arrow_column {
   uint32_t arrow_type;
   uint32_t _pad;
@@ -471,6 +486,8 @@ uint64_t etl_dec_arrow_rows(const etl_arrow_batch*);
 uint32_t etl_dec_arrow_cols(const etl_arrow_batch*);
 const uint64_t* etl_dec_arrow_row_records(const etl_arrow_batch*, int host);
 int etl_dec_arrow_column(const etl_arrow_batch*, uint32_t column, int host, etl_arrow_column* out);
+/* the child column of an ETL_ARROW_LIST column (n_elems entries; Utf8: int32 offsets, LargeBinary: int64 offsets) */
+int etl_dec_arrow_list_child(const etl_arrow_batch*, uint32_t column, int host, etl_arrow_column* out, uint64_t* n_elems);
 void etl_dec_arrow_free(etl_arrow_batch*);
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
