@@ -85,7 +85,7 @@ EXPORTS = [
     "etl_dec_batch_summary", "etl_dec_batch_schema", "etl_dec_decode_sharded", "etl_dec_comm_unique_id", "etl_dec_comm_init", "etl_dec_comm_init_host",
     "etl_dec_kind_for_type_oid", "etl_dec_mem_info",
     "etl_dec_copy_decode", "etl_dec_arrow_emit", "etl_dec_arrow_rows", "etl_dec_arrow_cols", "etl_dec_arrow_row_records",
-    "etl_dec_arrow_column", "etl_dec_arrow_list_child", "etl_dec_arrow_free", "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
+    "etl_dec_arrow_column", "etl_dec_arrow_list_child", "etl_dec_arrow_first_skipped", "etl_dec_arrow_free", "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
 ]
 
@@ -152,6 +152,8 @@ def load(build: bool = True):
     L.etl_dec_arrow_row_records.restype = C.c_void_p
     L.etl_dec_arrow_column.argtypes = [vp, C.c_uint32, C.c_int, C.POINTER(ArrowColumn)]
     L.etl_dec_arrow_list_child.argtypes = [vp, C.c_uint32, C.c_int, C.POINTER(ArrowColumn), C.POINTER(C.c_uint64)]
+    L.etl_dec_arrow_first_skipped.argtypes = [vp]
+    L.etl_dec_arrow_first_skipped.restype = C.c_uint64
     L.etl_dec_arrow_free.argtypes = [vp]
     L.etl_dec_arrow_free.restype = None
     L.etl_dec_batch_device_stream.argtypes = [vp]
@@ -176,6 +178,8 @@ NO_TIMING = 0x4
 # etl_dec_arrow_emit row_kinds bit: Numeric / Json columns as formatted Utf8, array columns as List (ETL_ARROW_ALL_COLUMNS)
 ARROW_ALL_COLUMNS = 0x100
 ARROW_LIST = 13
+# row_kinds bit: append cdc_operation and sequence_number, the Iceberg CDC columns (ETL_ARROW_CDC_COLUMNS)
+ARROW_CDC_COLUMNS = 0x200
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

@@ -29,6 +29,9 @@
 //     offset (array_parse.cuh), a top-level String / Json cell a span of the staged stream.
 // Each stage that sizes a buffer syncs once: after the row lengths, after the Json / List child lengths, and after the
 // Json children's canonical lengths (only when a List has Json elements).
+// A COPY batch (rec_kind == NULL) is one implicit schema: k_copy_sel maps every row of the valid prefix to its cells
+// (no selection sync), then every column stage runs unchanged; String / Json text with ETL_COPY_VAL_IN_HEAP is read from
+// the heap.  ETL_ARROW_CDC_COLUMNS appends cdc_operation / sequence_number, sized from n_rows alone and written by k_cdc.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -38,6 +41,7 @@
 
 #include "etl_decode.h"
 #include "arrow_format.cuh"
+#include "batch_internal.h"
 
 namespace {
 
@@ -50,25 +54,38 @@ struct SelParams {
   uint32_t* blk;          // per-block counts → exclusive offsets
   uint64_t* row_cell0;    // out: first cell of the row's image, per selected row
   uint64_t* row_rec;      // out: record index per selected row
-  unsigned long long* n_rows;
+  unsigned long long* n_rows;   // [0] rows, [1] first skipped record (UINT64_MAX = none)
 };
-// which image of record r is a row of this batch? returns false or the cell offset of the image inside the record
-__device__ __forceinline__ bool row_of(const SelParams& S, uint64_t r, uint64_t* cell0) {
-  if (r >= S.n_records || S.rec_schema[r] != S.schema) return false;
+enum { kNotRow = 0, kRow = 1, kSkipped = 2 };
+// which image of record r is a row of this batch?  kRow and the cell offset of the image inside the record; kSkipped
+// for a record whose kind row_kinds selects but which has no full image to emit (write_events, iceberg/core.rs:311-322
+// and :336-357, returns InvalidState there); kNotRow otherwise
+__device__ __forceinline__ int row_of(const SelParams& S, uint64_t r, uint64_t* cell0) {
+  if (r >= S.n_records || S.rec_schema[r] != S.schema) return kNotRow;
   const uint32_t k = S.rec_kind[r], f = S.rec_flags[r];
-  if (!(f & ETL_RF_EVENT)) return false;
+  if (!(f & ETL_RF_EVENT)) return kNotRow;
   const uint64_t c0 = S.rec_cell_base[r];
-  if (k == 'I' && (S.row_kinds & 1u)) { *cell0 = c0; return true; }
-  if (k == 'U' && (S.row_kinds & 2u) && !(f & ETL_RF_NEW_PARTIAL)) {      // UpdatedTableRow::Full only: a partial row has holes
+  if (k == 'I' && (S.row_kinds & 1u)) { *cell0 = c0; return kRow; }
+  if (k == 'U' && (S.row_kinds & 2u)) {
+    if (f & ETL_RF_NEW_PARTIAL) return kSkipped;                          // UpdatedTableRow::Full only: a partial row has holes
     *cell0 = S.rec_cell_base[r + 1] - S.n_cols;                           // the new image is the record's last n_cols cells
-    return true;
+    return kRow;
   }
-  if (k == 'D' && (S.row_kinds & 4u) && (f & ETL_RF_OLD_FULL)) { *cell0 = c0; return true; }
-  return false;
+  if (k == 'D' && (S.row_kinds & 4u)) {
+    if (!(f & ETL_RF_OLD_FULL)) return kSkipped;
+    *cell0 = c0;
+    return kRow;
+  }
+  return kNotRow;
 }
 __global__ void __launch_bounds__(kSelThreads) k_sel_count(SelParams S) {
   uint64_t c0;
-  const int c = __syncthreads_count(row_of(S, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, &c0));
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int sel = row_of(S, r, &c0);
+  const int c = __syncthreads_count(sel == kRow);
+  // record indices of a batch are 32-bit: one min per warp, one atomicMin per warp that has a skipped record
+  const unsigned skip = __reduce_min_sync(0xffffffffu, sel == kSkipped ? (unsigned)r : 0xffffffffu);
+  if ((threadIdx.x & 31) == 0 && skip != 0xffffffffu) atomicMin(S.n_rows + 1, (unsigned long long)skip);
   if (threadIdx.x == 0) S.blk[blockIdx.x] = (uint32_t)c;
 }
 __global__ void __launch_bounds__(kSelThreads) k_blk_scan(uint32_t* blk, uint32_t nb, unsigned long long* total) {
@@ -94,7 +111,7 @@ __global__ void __launch_bounds__(kSelThreads) k_sel_scatter(SelParams S) {
   __shared__ uint32_t warp_cnt[kSelThreads / 32];
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   uint64_t c0 = 0;
-  const bool sel = row_of(S, r, &c0);
+  const bool sel = row_of(S, r, &c0) == kRow;
   const unsigned bal = __ballot_sync(0xffffffffu, sel);
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   if (lane == 0) warp_cnt[wid] = __popc(bal);
@@ -105,6 +122,11 @@ __global__ void __launch_bounds__(kSelThreads) k_sel_scatter(SelParams S) {
     const uint64_t at = (uint64_t)S.blk[blockIdx.x] + before + __popc(bal & ((1u << lane) - 1u));
     S.row_cell0[at] = c0; S.row_rec[at] = r;
   }
+}
+// COPY rows (etl_dec_copy_decode): every row of the valid prefix is an insert image, row r's cells are r * n_cols + c
+__global__ void __launch_bounds__(256) k_copy_sel(uint64_t n_rows, uint32_t n_cols, uint64_t* row_cell0, uint64_t* row_rec) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n_rows) { row_cell0[r] = r * n_cols; row_rec[r] = r; }
 }
 
 struct ColParams {
@@ -118,6 +140,11 @@ struct ColParams {
 // the cell of item `row`: a row's cell of column `col`, or (row_cell0 == NULL) the row-th entry of a list child's
 // element planes, where `stream` is the heap (an array element's String / Json text lives in the heap)
 __device__ __forceinline__ uint64_t cell_of(const ColParams& C, uint64_t row) { return C.row_cell0 ? C.row_cell0[row] + C.col : row; }
+// the text of a String / Json cell: a span of `stream`, or (COPY rows whose field needed unescaping, bit 63 of val) of
+// the heap.  A stream offset is below 1 TiB, so the bit is checked unconditionally
+__device__ __forceinline__ const uint8_t* text_of(const ColParams& C, uint64_t val) {
+  return val & ETL_COPY_VAL_IN_HEAP ? C.heap + (val & ~ETL_COPY_VAL_IN_HEAP) : C.stream + val;
+}
 // iceberg/encoding.rs:200-318: value of a cell for the column's Arrow type, or "null"
 __device__ __forceinline__ bool fixed_value(uint32_t at, uint32_t tag, uint64_t val, uint32_t aux, int64_t* out) {
   switch (at) {
@@ -237,7 +264,7 @@ __global__ void __launch_bounds__(256) k_gather(ColParams C, const OffT* offs, u
   const uint32_t tag = C.cell_tag[cell];
   const bool str = C.arrow_type == ETL_ARROW_UTF8;
   if (tag != (str ? (uint32_t)ETL_CELL_STRING : (uint32_t)ETL_CELL_BYTES)) return;
-  const uint8_t* src = (str ? C.stream : C.heap) + C.cell_val[cell];
+  const uint8_t* src = str ? text_of(C, C.cell_val[cell]) : C.heap + C.cell_val[cell];
   const uint32_t n = C.cell_aux[cell];
   uint8_t* dst = data + (uint64_t)offs[row];
   for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
@@ -257,7 +284,7 @@ __global__ void __launch_bounds__(128) k_json_canon(ColParams C, const uint64_t*
   if (C.cell_tag[cell] != ETL_CELL_JSON) return;
   const uint64_t at = in_off[row];
   const uint32_t n = C.cell_aux[cell];
-  const uint32_t r = etl_fmt::json_canon(C.stream + C.cell_val[cell], n, canon + at, work + kJsonWorkPerByte * at + kJsonWorkPerItem * row);
+  const uint32_t r = etl_fmt::json_canon(text_of(C, C.cell_val[cell]), n, canon + at, work + kJsonWorkPerByte * at + kJsonWorkPerItem * row);
   if (r == etl_fmt::kJsonCanonBad) { atomicOr(bad, 1u); C.lens[row] = 0; return; }   // json_valid let through what it must reject
   C.lens[row] = r;
 }
@@ -276,7 +303,7 @@ __global__ void __launch_bounds__(256) k_gather_text(ColParams C, const int32_t*
     if (lane == 0) etl_fmt::numeric_write(C.heap + C.cell_val[cell], C.cell_aux[cell], dst);
     return;
   }
-  if (tag == ETL_CELL_STRING) { src = C.stream + C.cell_val[cell]; n = C.cell_aux[cell]; }
+  if (tag == ETL_CELL_STRING) { src = text_of(C, C.cell_val[cell]); n = C.cell_aux[cell]; }
   else if (tag == ETL_CELL_JSON && canon) { src = canon + in_off[row]; n = (uint32_t)(offs[row + 1] - offs[row]); }
   else return;
   for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
@@ -295,6 +322,37 @@ __global__ void __launch_bounds__(256) k_list_elems(ColParams C, const int32_t* 
   const uint8_t* el = C.heap + C.cell_val[cell] + sizeof(etl_array_hdr) + sizeof(etl_array_elem) * (e - (uint32_t)loffs[lo]);
   const etl_array_elem x = *reinterpret_cast<const etl_array_elem*>(el);
   el_tag[e] = x.tag; el_val[e] = x.val; el_aux[e] = x.aux;
+}
+
+// ---------------------------------------------------------------- ETL_ARROW_CDC_COLUMNS
+// thread per row: cdc_operation and sequence_number (write_table_rows / write_events, iceberg/core.rs:239-366), two
+// never-null Utf8 columns whose texts have fixed lengths, so their offsets are 6 * row and 33 * row.  COPY rows
+// (rec_kind == NULL) are INSERT with the key of (0, 0).
+struct CdcParams {
+  const uint64_t* row_rec; const uint8_t* rec_kind; const uint64_t* rec_commit_lsn; const uint64_t* rec_tx_ordinal;
+  uint64_t n_rows;
+  uint32_t* op_validity; int32_t* op_offs; uint8_t* op_data;
+  uint32_t* seq_validity; int32_t* seq_offs; uint8_t* seq_data;
+};
+__global__ void __launch_bounds__(256) k_cdc(CdcParams Q) {
+  const uint64_t row = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= Q.n_rows) return;
+  uint32_t kind = 'I';
+  uint64_t lsn = 0, ord = 0;
+  if (Q.rec_kind) {
+    const uint64_t r = Q.row_rec[row];
+    kind = Q.rec_kind[r]; lsn = Q.rec_commit_lsn[r]; ord = Q.rec_tx_ordinal[r];
+  }
+  etl_fmt::cdc_op_write(kind, Q.op_data + etl_fmt::kCdcOpLen * row);
+  etl_fmt::seq_key_write(lsn, ord, Q.seq_data + etl_fmt::kSeqKeyLen * row);
+  Q.op_offs[row] = (int32_t)(etl_fmt::kCdcOpLen * row);
+  Q.seq_offs[row] = (int32_t)(etl_fmt::kSeqKeyLen * row);
+  if (row + 1 == Q.n_rows) { Q.op_offs[Q.n_rows] = (int32_t)(etl_fmt::kCdcOpLen * Q.n_rows); Q.seq_offs[Q.n_rows] = (int32_t)(etl_fmt::kSeqKeyLen * Q.n_rows); }
+  if ((row & 31) == 0) {                               // validity: every row of the word that exists
+    const uint64_t left = Q.n_rows - row;
+    const uint32_t w = left >= 32 ? 0xffffffffu : (1u << left) - 1u;
+    Q.op_validity[row >> 5] = w; Q.seq_validity[row >> 5] = w;
+  }
 }
 
 uint32_t arrow_type_of(uint32_t k, bool all) {
@@ -347,6 +405,7 @@ struct etl_arrow_batch {
   uint8_t* dev = nullptr;     // one device allocation: row_rec | per column validity, values / offsets | data | children
   uint8_t* host = nullptr;    // pinned host image (to_host)
   uint64_t bytes = 0, row_rec_off = 0;
+  uint64_t first_skipped = UINT64_MAX;   // etl_dec_arrow_first_skipped
   std::string error;
 };
 
@@ -355,12 +414,17 @@ extern "C" {
 int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32_t row_kinds, int to_host, etl_arrow_batch** out) {
   if (!batch || !out) return ETL_ERR_INVALID_ARG;
   const bool all = (row_kinds & ETL_ARROW_ALL_COLUMNS) != 0;
+  const bool cdc = (row_kinds & ETL_ARROW_CDC_COLUMNS) != 0;
   const uint8_t* dev_stream = etl_dec_batch_device_stream(batch);
   etl_dec_planes P;
   etl_dec_summary S;
-  etl_dec_schema_info sc;
+  etl_dec_schema_info sc{};
   if (etl_dec_batch_planes(batch, 0, &P) != ETL_OK || etl_dec_batch_summary(batch, &S) != ETL_OK) return ETL_ERR_INVALID_ARG;
-  if (etl_dec_batch_schema(batch, schema_index, &sc) != ETL_OK) return ETL_ERR_INVALID_ARG;
+  // a COPY batch (no record kinds) has one implicit schema: the columns it was decoded with
+  const bool copy = P.rec_kind == nullptr;
+  if (copy) {
+    if (schema_index != 0 || !etl_copy_batch_columns(batch, &sc.table_id, &sc.col_kind, &sc.n_cols)) return ETL_ERR_INVALID_ARG;
+  } else if (etl_dec_batch_schema(batch, schema_index, &sc) != ETL_OK) return ETL_ERR_INVALID_ARG;
   cudaStream_t st = cudaStreamPerThread;
   etl_arrow_batch* A = new etl_arrow_batch();
   // scratch of the ETL_ARROW_ALL_COLUMNS stages, freed on every exit
@@ -376,11 +440,18 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
   auto free_tmp = [&]() { cudaFree(d_blk); cudaFree(d_cell0); cudaFree(d_rec); cudaFree(d_n); };
   SelParams Sp{P.rec_kind, P.rec_flags, P.rec_schema, P.rec_cell_base, n_valid, (int32_t)schema_index, row_kinds, sc.n_cols, d_blk, d_cell0, d_rec, d_n};
   unsigned long long n_rows = 0;
-  if (nb) {
+  if (copy) {                                           // every row of the valid prefix when inserts are selected: no sync
+    n_rows = (row_kinds & 1u) ? n_valid : 0;
+    if (n_rows) k_copy_sel<<<(uint32_t)((n_rows + 255) / 256), 256, 0, st>>>(n_rows, sc.n_cols, d_cell0, d_rec);
+  } else if (nb) {
+    unsigned long long sel[2] = {0, UINT64_MAX};        // rows, first skipped record
+    cudaMemsetAsync(d_n + 1, 0xff, 8, st);
     k_sel_count<<<nb, kSelThreads, 0, st>>>(Sp);
     k_blk_scan<<<1, kSelThreads, 0, st>>>(d_blk, nb, d_n);
     k_sel_scatter<<<nb, kSelThreads, 0, st>>>(Sp);
-    if (cudaMemcpyAsync(&n_rows, d_n, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { free_tmp(); return fail(ETL_ERR_CUDA); }
+    if (cudaMemcpyAsync(sel, d_n, 16, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { free_tmp(); return fail(ETL_ERR_CUDA); }
+    n_rows = sel[0];
+    A->first_skipped = sel[1];
   }
   A->n_rows = n_rows;
   // pass 1: validity + fixed values + lengths (into a scratch), per column; var-width sizes need a sync before the data buffers exist
@@ -564,6 +635,19 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
     cur += fixed_part + ((kid.data_bytes + 63) & ~63ull);
     if (kid.arrow_type == ETL_ARROW_UTF8 && kid.data_bytes > 0x7FFFFFFFull) { A->error = "Utf8 list child exceeds 2 GiB: split the batch"; }
   }
+  // ETL_ARROW_CDC_COLUMNS: cdc_operation and sequence_number after the table's columns, validity | offsets | data each;
+  // their sizes follow from n_rows alone
+  if (cdc) {
+    for (uint32_t len : {etl_fmt::kCdcOpLen, etl_fmt::kSeqKeyLen}) {
+      Col col;
+      col.arrow_type = ETL_ARROW_UTF8;
+      col.validity_off = cur; cur += vbytes;
+      col.offsets_off = cur; col.offsets_bytes = ((n_rows + 1) * 4 + 63) & ~63ull; cur += col.offsets_bytes;
+      col.data_off = cur; col.data_bytes = n_rows * len; cur += (col.data_bytes + 63) & ~63ull;
+      if (col.data_bytes > 0x7FFFFFFFull) A->error = "Utf8 column exceeds 2 GiB: split the batch";
+      A->cols.push_back(col);
+    }
+  }
   A->bytes = cur + 64;
   bool ok = A->error.empty() && cudaMalloc(&A->dev, A->bytes) == cudaSuccess;
   if (ok) ok = cudaMemcpyAsync(A->dev, d_fixed, fixed_bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
@@ -587,6 +671,16 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
     if (kid.arrow_type == ETL_ARROW_UTF8) k_gather_text<<<grid, 256, 0, st>>>(Kp, (const int32_t*)(A->dev + kid.offsets_off), A->dev + kid.data_off, ks.in_off, ks.canon);
     else k_gather<int64_t><<<grid, 256, 0, st>>>(Kp, (const int64_t*)(A->dev + kid.offsets_off), A->dev + kid.data_off);
   }
+  if (ok && cdc) {
+    const Col& op = A->cols[sc.n_cols];
+    const Col& seq = A->cols[sc.n_cols + 1];
+    for (const Col* c : {&op, &seq})                   // validity padding; offsets[0] of 0 rows
+      if (ok) ok = cudaMemsetAsync(A->dev + c->validity_off, 0, c->data_off - c->validity_off, st) == cudaSuccess;
+    CdcParams Q{d_rec, P.rec_kind, P.rec_commit_lsn, P.rec_tx_ordinal, n_rows,
+                (uint32_t*)(A->dev + op.validity_off), (int32_t*)(A->dev + op.offsets_off), A->dev + op.data_off,
+                (uint32_t*)(A->dev + seq.validity_off), (int32_t*)(A->dev + seq.offsets_off), A->dev + seq.data_off};
+    if (ok && n_rows) k_cdc<<<(uint32_t)((n_rows + 255) / 256), 256, 0, st>>>(Q);
+  }
   if (ok && to_host) {
     ok = cudaHostAlloc((void**)&A->host, A->bytes, cudaHostAllocDefault) == cudaSuccess;
     if (ok) ok = cudaMemcpyAsync(A->host, A->dev, A->bytes, cudaMemcpyDeviceToHost, st) == cudaSuccess;
@@ -604,6 +698,7 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
 }
 uint64_t etl_dec_arrow_rows(const etl_arrow_batch* a) { return a ? a->n_rows : 0; }
 uint32_t etl_dec_arrow_cols(const etl_arrow_batch* a) { return a ? (uint32_t)a->cols.size() : 0; }
+uint64_t etl_dec_arrow_first_skipped(const etl_arrow_batch* a) { return a ? a->first_skipped : UINT64_MAX; }
 const uint64_t* etl_dec_arrow_row_records(const etl_arrow_batch* a, int host) {
   if (!a) return nullptr;
   const uint8_t* base = host ? a->host : a->dev;

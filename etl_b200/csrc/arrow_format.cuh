@@ -383,4 +383,27 @@ __device__ inline uint32_t json_canon(const uint8_t* s, uint32_t n, uint8_t* out
 #undef JPUT
 }
 
+// ------------------------------------------------------------------------------------------------ CDC columns
+// EventSequenceKey's Display (crates/etl/src/types/event.rs:331-336): "{commit_lsn:016x}/{tx_ordinal:016x}", always
+// kSeqKeyLen bytes; generate_sequence_number(0, 0) of a table-copy row (etl-postgres/src/types/utils.rs:119-139) is the
+// key of (0, 0).  Every cdc_operation name ("INSERT" / "UPDATE" / "DELETE") is kCdcOpLen bytes.
+constexpr uint32_t kSeqKeyLen = 33, kCdcOpLen = 6;
+__device__ __forceinline__ void hex16_write(uint64_t v, uint8_t* out) {
+  for (int k = 15; k >= 0; k--) {
+    const uint32_t d = (uint32_t)(v & 15u);
+    out[k] = (uint8_t)(d < 10u ? '0' + d : 'a' - 10u + d);
+    v >>= 4;
+  }
+}
+__device__ __forceinline__ void seq_key_write(uint64_t commit_lsn, uint64_t tx_ordinal, uint8_t* out) {
+  hex16_write(commit_lsn, out);
+  out[16] = '/';
+  hex16_write(tx_ordinal, out + 17);
+}
+// the cdc_operation of a record kind: 'U' → UPDATE, 'D' → DELETE, anything else (an insert, a COPY row) → INSERT
+__device__ __forceinline__ void cdc_op_write(uint32_t rec_kind, uint8_t* out) {
+  const char* s = rec_kind == 'U' ? "UPDATE" : (rec_kind == 'D' ? "DELETE" : "INSERT");
+  for (uint32_t k = 0; k < kCdcOpLen; k++) out[k] = (uint8_t)s[k];
+}
+
 }  // namespace etl_fmt

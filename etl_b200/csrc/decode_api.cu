@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "etl_decode.h"
+#include "batch_internal.h"
 #include "oid_classes.h"
 #include "wal_kernels.cuh"
 
@@ -199,6 +200,9 @@ struct etl_dec_batch {
   etl_dec_summary summary{};
   std::vector<RelVersion> schemas;
   const uint8_t* dev_stream = nullptr;   // the staged bytes the planes point into
+  bool copy = false;                     // COPY rows: the table and column classes they were decoded with
+  uint32_t copy_table = 0;
+  std::vector<uint8_t> copy_kinds;
 };
 
 struct etl_dec_ctx {
@@ -1483,6 +1487,7 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
   }
   S.n_events = nr;
   b->dev_stream = P.buf;
+  b->copy = true; b->copy_table = table_id; b->copy_kinds = std::move(kinds);
   *out = b;
   return ETL_OK;
 #undef CKB
@@ -1518,3 +1523,9 @@ int etl_dec_mem_info(etl_dec_ctx* ctx, uint64_t* free_bytes, uint64_t* total_byt
 }
 
 }  // extern "C"
+
+bool etl_copy_batch_columns(const etl_dec_batch* b, uint32_t* table_id, const uint8_t** col_kind, uint32_t* n_cols) {
+  if (!b || !b->copy) return false;
+  *table_id = b->copy_table; *col_kind = b->copy_kinds.data(); *n_cols = (uint32_t)b->copy_kinds.size();
+  return true;
+}

@@ -441,7 +441,13 @@ int etl_dec_copy_decode(etl_dec_ctx*, uint32_t table_id, const etl_copy_input*, 
  * formatting in the reference) come back as ETL_ARROW_UNSUPPORTED and stay on the shim's row path unless row_kinds has
  * ETL_ARROW_ALL_COLUMNS (below): then they are built on the device too.
  * row_kinds: bit 0 inserts, bit 1 updates (new image, Full rows only), bit 2 deletes (old image, when Full); rows keep
- * stream order and etl_dec_arrow_row_records gives the record index of each (for the CDC columns). */
+ * stream order and etl_dec_arrow_row_records gives the record index of each (for the CDC columns).
+ * A COPY batch (etl_dec_copy_decode; rec_kind == NULL in its planes) is emitted the same way: schema_index must be 0
+ * (anything else is ETL_ERR_INVALID_ARG), the columns are those the batch was decoded with (a later
+ * etl_dec_put_table_schema does not change them), every row of the valid prefix [0, first_error.record_index) is an
+ * insert image selected by bit 0 (without it: zero rows, the columns still typed), and etl_dec_arrow_row_records gives
+ * the row index.  The same type mapping, null rules and size limits apply; a String / Json cell with
+ * ETL_COPY_VAL_IN_HEAP is read from the heap. */
 enum {
   ETL_ARROW_UNSUPPORTED = 0,
   ETL_ARROW_BOOLEAN = 1,        /* values bit-packed like the validity bitmap */
@@ -471,6 +477,18 @@ enum {
  * or more than 2 GiB of text in a Utf8 child, fail like an oversize Utf8 column (ETL_ERR_INVALID_ARG: split the batch); a
  * Json value that does not parse again (the decode validated it) is ETL_ERR_INTERNAL. */
 #define ETL_ARROW_ALL_COLUMNS 0x100u
+/* row_kinds bit: append the two columns both Iceberg write paths add to every row (crates/etl-destinations/src/iceberg/
+ * core.rs: write_table_rows :239-267, write_events :276-366), so etl_dec_arrow_cols returns n_cols + 2:
+ *   column n_cols     cdc_operation:   ETL_ARROW_UTF8, never null, "INSERT" / "UPDATE" / "DELETE" from the row's record
+ *                                      kind; COPY rows are "INSERT";
+ *   column n_cols + 1 sequence_number: ETL_ARROW_UTF8, never null, EventSequenceKey's Display
+ *                                      (crates/etl/src/types/event.rs:331-336) "{rec_commit_lsn:016x}/{rec_tx_ordinal:016x}"
+ *                                      in lowercase hex; COPY rows get generate_sequence_number(0, 0)
+ *                                      (etl-postgres/src/types/utils.rs:119-139) = "0000000000000000/0000000000000000".
+ * Every name is 6 bytes and every key 33, so their offsets are 6 * i and 33 * i.  More than INT32_MAX bytes of keys
+ * (about 65 M rows in one emit) fail like an oversize Utf8 column (ETL_ERR_INVALID_ARG: split the batch).  The column
+ * names (find_unique_column_name, core.rs:679) are host metadata.  Without the bit the output is what it was before. */
+#define ETL_ARROW_CDC_COLUMNS 0x200u
 typedef struct etl_arrow_column {
   uint32_t arrow_type;
   uint32_t _pad;
@@ -488,6 +506,11 @@ const uint64_t* etl_dec_arrow_row_records(const etl_arrow_batch*, int host);
 int etl_dec_arrow_column(const etl_arrow_batch*, uint32_t column, int host, etl_arrow_column* out);
 /* the child column of an ETL_ARROW_LIST column (n_elems entries; Utf8: int32 offsets, LargeBinary: int64 offsets) */
 int etl_dec_arrow_list_child(const etl_arrow_batch*, uint32_t column, int host, etl_arrow_column* out, uint64_t* n_elems);
+/* the smallest batch-local record index, among the records of the emitted schema version in the valid prefix, whose
+ * kind row_kinds selects but which cannot become a row: an Update with ETL_RF_NEW_PARTIAL (bit 1) or a Delete without
+ * ETL_RF_OLD_FULL (bit 2) — where write_events returns InvalidState (iceberg/core.rs:311-322, :336-357) while the emit
+ * leaves the record out.  UINT64_MAX if there is none; always UINT64_MAX for a COPY batch. */
+uint64_t etl_dec_arrow_first_skipped(const etl_arrow_batch*);
 void etl_dec_arrow_free(etl_arrow_batch*);
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
