@@ -849,8 +849,6 @@ static int prepare(etl_dec_ctx* ctx, const etl_dec_input* in, uint32_t flags, bo
   const uint32_t act_blocks = (P.n_anchors + kActThreads - 1) / kActThreads;
   CK(ctx->d_act.ensure(P.n_anchors + 1)); CK(ctx->d_act_blk.ensure(act_blocks + 1));
   P.act = ctx->d_act.ptr(); P.act_blk = ctx->d_act_blk.ptr();
-  CK(ctx->d_bin_count.ensure(kMaxBins)); CK(ctx->d_bin_cursor.ensure(kMaxBins));
-  P.bin_count = ctx->d_bin_count.ptr(); P.bin_cursor = ctx->d_bin_cursor.ptr();
   P.rank = (uint32_t)ctx->rank; P.n_ranks = sharded ? (uint32_t)ctx->n_ranks : 1u;
   if (sharded) {
     CK(ctx->d_seam.ensure(1 + (size_t)ctx->n_ranks));
@@ -974,6 +972,8 @@ static void fill_planes(etl_dec_planes& pl, uint8_t* bs, const PlaneLayout& L, u
 }
 
 // ---------------------------------------------------------------- pass C into planes of capacity (cap_r, cap_c)
+// entries of the binned record order: the records plus at most 31 padding lanes per (tile, bin)
+static size_t perm_capacity(const DecodeParams& P) { return P.cap_records + 32ull * P.n_bin_tiles * P.n_bins + 256; }
 static int launch_emit(etl_dec_ctx* ctx, etl_dec_batch* b, uint64_t cap_r, uint64_t cap_c, uint64_t array_heap, PlaneLayout* Lout, uint64_t* scalar_heap_out) {
   DecodeParams& P = ctx->P;
   cudaStream_t st = ctx->stream;
@@ -998,8 +998,13 @@ static int launch_emit(etl_dec_ctx* ctx, etl_dec_batch* b, uint64_t cap_r, uint6
   P.cell_aux = (uint32_t*)b->dev.cell_aux; P.heap = (uint8_t*)b->dev.heap;
   P.heap_cap = nh; P.arr_base = *scalar_heap_out;
   P.cap_records = cap_r; P.cap_cells = cap_c;
-  const size_t perm_cap = cap_r + 32ull * P.n_bins + 256;
-  CK(ctx->d_perm.ensure(perm_cap)); CK(ctx->d_rec_flen.ensure(cap_r + 1));
+  // shape bins per tile of consecutive records; a tile has room for 1024 records per bin, so that the warp padding
+  // (≤ 31 lanes per occupied bin) stays a few per cent of it
+  P.bin_tile = std::max<uint32_t>(kBinTileMin, 1024u * P.n_bins);
+  P.n_bin_tiles = (uint32_t)std::max<uint64_t>(1, (cap_r + P.bin_tile - 1) / P.bin_tile);
+  CK(ctx->d_bin_count.ensure((size_t)P.n_bin_tiles * P.n_bins)); CK(ctx->d_bin_cursor.ensure((size_t)P.n_bin_tiles * P.n_bins));
+  P.bin_count = ctx->d_bin_count.ptr(); P.bin_cursor = ctx->d_bin_cursor.ptr();
+  CK(ctx->d_perm.ensure(perm_capacity(P))); CK(ctx->d_rec_flen.ensure(cap_r + 1));
   P.perm = ctx->d_perm.ptr(); P.rec_flen = ctx->d_rec_flen.ptr();
   return ETL_OK;
 }
@@ -1007,9 +1012,9 @@ static int launch_emit_kernels(etl_dec_ctx* ctx) {
   DecodeParams& P = ctx->P;
   cudaStream_t st = ctx->stream;
   const uint64_t cap_r = P.cap_records;
-  const size_t perm_cap = cap_r + 32ull * P.n_bins + 256;
+  const size_t perm_cap = perm_capacity(P);
   CK(cudaEventRecord(ctx->ev[3], st));
-  CK(cudaMemsetAsync(P.bin_count, 0, P.n_bins * 4, st));
+  CK(cudaMemsetAsync(P.bin_count, 0, (size_t)P.n_bin_tiles * P.n_bins * 4, st));
   // k_heavy / k_fix read every cell tag: a record that failed leaves cells unwritten, and a stale tag must not look pending
   if (P.cap_cells) CK(cudaMemsetAsync(P.cell_tag, 0, P.cap_cells, st));
   ctx->long_skipped = long_passes_skippable(ctx);
@@ -1022,8 +1027,7 @@ static int launch_emit_kernels(etl_dec_ctx* ctx) {
       k_bin_scan<<<1, 1024, 0, st>>>(P);
       k_perm<<<(uint32_t)((cap_r + kPermThreads - 1) / kPermThreads), kPermThreads, 0, st>>>(P);
       cudaEventRecord(ctx->evk[2], st);
-      const uint32_t chunks = (uint32_t)((perm_cap + kRowsThreads - 1) / kRowsThreads);
-      k_rows<<<((chunks + 63u) / 64u) * 64u, kRowsThreads, kRowsSmemBytes, st>>>(P);
+      k_rows<<<(uint32_t)((perm_cap + kRowsThreads - 1) / kRowsThreads), kRowsThreads, kRowsSmemBytes, st>>>(P);
       k_heavy<<<std::min<uint32_t>((uint32_t)((P.cap_cells + kHeavyTile - 1) / kHeavyTile) + 1u, (uint32_t)sm_count(ctx) * 3u), kHeavyThreads, kHeavySmemBytes, st>>>(P);
       k_fix<<<sm_count(ctx) * 2, 256, 0, st>>>(P);
       ctx->launches += 5;

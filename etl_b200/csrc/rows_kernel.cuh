@@ -1,6 +1,7 @@
 // rows_kernel.cuh — pass C2: tuples → rows, fused (replaces the round-1 k_walk → descriptors → k_cells → k_copy chain).
 //
-//   k_rows   one THREAD per DML record in shape-bin order, one WARP per 32 structurally identical records.
+//   k_rows   one THREAD per DML record in shape-bin order (bins per tile of consecutive records, tile after
+//            tile), one WARP per 32 structurally identical records.
 //            Every pass each lane stages a window of its record's frame into shared memory with one 1-D bulk
 //            async copy (cp.async.bulk → UBLKCP, completion on a per-warp mbarrier), then the 32 lanes walk
 //            their tuples in lockstep: wire cell i is the same column in every lane, so one parser runs for
@@ -289,12 +290,12 @@ __device__ __forceinline__ uint32_t rk_step(const DecodeParams& P, Wk& w, TextCe
 __device__ __forceinline__ void rows_body(const DecodeParams& P, uint8_t* smem) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t n_perm = *P.perm_len;
-  // chunk of the binned order for this CTA.  Bins are contiguous and differ in cost per record (an update
-  // with a full old image walks twice the cells of an insert): consecutive CTAs take chunks 1/64 of the
-  // order apart so that every SM gets the same mix.  The grid is sized for the worst-case padding.
-  const uint32_t n_chunks = (n_perm + blockDim.x - 1) / blockDim.x, cols = (n_chunks + 63u) / 64u;
-  const uint32_t chunk = (blockIdx.x & 63u) * cols + (blockIdx.x >> 6);
-  if ((blockIdx.x >> 6) >= cols || chunk >= n_chunks) return;
+  // chunk of the binned order for this CTA: consecutive CTAs, consecutive chunks.  The bins are per tile of
+  // consecutive records, so the CTAs resident together work on a narrow band of the stream, and every tile holds
+  // its natural mix of costs per record (an update with a full old image walks twice the cells of an insert).
+  // The grid is sized for the worst-case padding.
+  const uint32_t chunk = blockIdx.x;
+  if ((uint64_t)chunk * blockDim.x >= n_perm) return;
   // CTA set-up: one mbarrier per warp
   if (threadIdx.x == 0) {
     for (uint32_t k = 0; k < kRowsWarps; k++) mbar_init(smem_u32(smem + kRowsBarOff + 8u * k), 32u);

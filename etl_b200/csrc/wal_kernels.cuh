@@ -29,6 +29,12 @@ namespace etl {
 
 constexpr int kIndexThreads = 256;
 constexpr int kMaxBins = 4096;         // 16 frame shapes x 256 schema versions (more versions share the last bins)
+#ifndef ETL_BIN_TILE
+#define ETL_BIN_TILE 16384
+#endif
+// Records per shape-bin tile at least (bin_tile = max(this, 1024 · n_bins)); a multiple of the k_perm and k_records CTAs
+constexpr uint32_t kBinTileMin = ETL_BIN_TILE;
+static_assert(kBinTileMin % 1024 == 0, "a shape-bin tile holds whole k_perm / k_records CTAs");
 
 struct ScanSlot;
 struct LongCell { uint32_t rec_local, seq; uint64_t soff; uint32_t len, edges; };   // a text cell of ≥ kCoopLen bytes; edges: its head and tail are still to be validated
@@ -101,8 +107,10 @@ struct DecodeParams {
   Summ* chase_summ;          // multi-GPU: per-CTA state aggregates of k_chase (the seam block is their fold)
   unsigned int* chase_done;  // ... and the count of CTAs that have published theirs
   Summ* total;               // [0] = fold of everything (shard seam summary)
-  // global grouping of the DML records by frame shape (k_records counts, k_bin_scan lays out, k_perm fills)
+  // grouping of the DML records by frame shape within tiles of bin_tile consecutive records (k_records counts,
+  // k_bin_scan lays out, k_perm fills); entry (tile, bin) of bin_count / bin_cursor is tile * n_bins + bin
   uint32_t* bin_count; uint32_t* bin_cursor; uint32_t n_bins; uint32_t* perm; unsigned int* perm_len;
+  uint32_t bin_tile, n_bin_tiles;
   uint32_t n_batch_schemas;
   uint32_t* rec_flen;               // CopyData length + 1 of every record's frame (k_records → k_rows: sizes the staged window)
   unsigned int* abort_flag;         // ABORT_* bits: the batch does not fit the planes / scratch the host reserved (k_chase, k_records)
@@ -836,15 +844,21 @@ __device__ __noinline__ bool utf8_medium_bad(const uint8_t* cell, uint32_t len) 
 // record indices bin by bin, and k_rows thread t walks record perm[t].  Schema versions with identical
 // columns share a layout (a table whose Relation is re-sent keeps its bins); a batch with more layouts
 // than bins shares the last 16 bins, whose warps then hold mixed shapes (k_rows handles that per lane).
+// The records are binned within tiles of P.bin_tile consecutive records, tile after tile: the k_rows CTAs that
+// are resident together then read a narrow band of the stream and can finish each sector of the record and cell planes
+// while it is in L2 (bins over the whole batch scattered every warp's frames and plane writes over all of it).
 __device__ __forceinline__ uint32_t walk_bin(const DecodeParams& P, uint32_t layout, uint32_t kind, uint32_t rflags) {
   const uint32_t b = (layout << 4) | (kind == 'I' ? 0u : (kind == 'U' ? 4u : 8u)) | (rflags & 3u);
   return b < P.n_bins ? b : P.n_bins - 16u + (b & 15u);
 }
+// Exclusive scan of the warp-padded counts in (tile, bin) order.  bin_cursor ← the bin's start, bin_count ← the end of
+// its records: k_perm writes the padding lanes behind them.
 __global__ void __launch_bounds__(1024) k_bin_scan(DecodeParams P) {
   __shared__ uint32_t sh[1024];
   if (*P.abort_flag) return;
-  const uint32_t per = (P.n_bins + 1023u) / 1024u;
-  const uint32_t lo = threadIdx.x * per, hi = min(lo + per, P.n_bins);
+  const uint32_t n = P.n_bins * P.n_bin_tiles;
+  const uint32_t per = (n + 1023u) / 1024u;
+  const uint32_t lo = threadIdx.x * per, hi = min(lo + per, n);
   uint32_t acc = 0;
   for (uint32_t i = lo; i < hi; i++) acc += (P.bin_count[i] + 31u) & ~31u;
   sh[threadIdx.x] = acc;
@@ -858,10 +872,10 @@ __global__ void __launch_bounds__(1024) k_bin_scan(DecodeParams P) {
   }
   uint32_t run = threadIdx.x ? sh[threadIdx.x - 1] : 0u;
   for (uint32_t i = lo; i < hi; i++) {
-    const uint32_t c = P.bin_count[i], padded = (c + 31u) & ~31u;
+    const uint32_t c = P.bin_count[i];
     P.bin_cursor[i] = run;
-    for (uint32_t k = c; k < padded; k++) P.perm[run + k] = 0xFFFFFFFFu;   // the bin's padding lanes (k_perm fills [0, c))
-    run += padded;
+    P.bin_count[i] = run + c;
+    run += (c + 31u) & ~31u;
   }
   if (threadIdx.x == 1023) *P.perm_len = sh[1023];
 }
@@ -874,6 +888,7 @@ __global__ void __launch_bounds__(kPermThreads) k_perm(DecodeParams P) {
   if (*P.abort_flag) return;
   const uint64_t n_rec = P.total[0].n_rec;
   if ((uint64_t)blockIdx.x * blockDim.x >= n_rec) return;
+  const uint32_t tile_bins = (uint32_t)((uint64_t)blockIdx.x * kPermThreads / P.bin_tile) * P.n_bins;
   for (uint32_t i = threadIdx.x; i < P.n_bins; i += blockDim.x) hist[i] = 0;
   __syncthreads();
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -895,7 +910,14 @@ __global__ void __launch_bounds__(kPermThreads) k_perm(DecodeParams P) {
     local = base + __popc(mask & ((1u << lane) - 1u));
   }
   __syncthreads();
-  for (uint32_t i = threadIdx.x; i < P.n_bins; i += blockDim.x) { const uint32_t c = hist[i]; if (c) hist[i] = atomicAdd(&P.bin_cursor[i], c); }
+  for (uint32_t i = threadIdx.x; i < P.n_bins; i += blockDim.x) {
+    const uint32_t c = hist[i];
+    if (!c) continue;
+    const uint32_t at = atomicAdd(&P.bin_cursor[tile_bins + i], c), end = at + c;
+    hist[i] = at;
+    if (end == P.bin_count[tile_bins + i])            // the bin's last records: its padding lanes follow them
+      for (uint32_t k = end; k & 31u; k++) P.perm[k] = 0xFFFFFFFFu;
+  }
   __syncthreads();
   if (dml) P.perm[hist[bin] + local] = (uint32_t)r;
 }
@@ -918,6 +940,7 @@ __global__ void __launch_bounds__(kPermThreads) k_perm(DecodeParams P) {
 // fold): with 256 records per CTA that alone capped the pass on every workload (ncu: a third of the samples at the
 // barrier behind the look-back warp).
 constexpr int kRecThreads = ETL_REC_THREADS;
+static_assert(1024 % kRecThreads == 0, "a shape-bin tile holds whole k_records CTAs");
 constexpr int kRecCtaThreads = kRecThreads + 32;      // + the look-back warp
 struct ScanSlot { Summ aggr; Summ incl; };
 #define SUMM_SHFL(dst, src, fn, arg)                                                                     \
@@ -1165,7 +1188,9 @@ __global__ void __launch_bounds__(kRecCtaThreads, kRecThreads >= 512 ? 2 : 4) k_
   for (int d = 16; d > 0; d >>= 1) events += __shfl_down_sync(0xffffffffu, events, d);
   if (lane == 0 && events) atomicAdd(&P.metrics[3], (unsigned long long)events);
   __syncthreads();
-  for (uint32_t i = threadIdx.x; i < P.n_bins; i += blockDim.x) if (hist[i]) atomicAdd(&P.bin_count[i], hist[i]);
+  // the CTA's records are frames [blockIdx.x · kRecThreads, …) (one record per frame): all of them in one tile
+  const uint32_t tile_bins = (uint32_t)((uint64_t)blockIdx.x * kRecThreads / P.bin_tile) * P.n_bins;
+  for (uint32_t i = threadIdx.x; i < P.n_bins; i += blockDim.x) if (hist[i]) atomicAdd(&P.bin_count[tile_bins + i], hist[i]);
 }
 #undef SUMM_SHFL
 
