@@ -52,6 +52,14 @@ class ArrowColumn(C.Structure):
                 ("offsets", C.c_void_p), ("data", C.c_void_p), ("data_bytes", C.c_uint64)]
 
 
+class RbIssue(C.Structure):
+    _fields_ = [("row", C.c_uint64), ("column", C.c_uint32), ("element", C.c_uint32)]
+
+
+class RowBinaryIssues(C.Structure):
+    _fields_ = [("date_range", RbIssue), ("null_value", RbIssue), ("first_partial_update", C.c_uint64)]
+
+
 class Planes(C.Structure):
     _fields_ = [("n_records", C.c_uint64), ("n_cells", C.c_uint64), ("heap_bytes", C.c_uint64),
                 ("rec_off", C.c_void_p), ("rec_kind", C.c_void_p), ("rec_flags", C.c_void_p), ("rec_rel", C.c_void_p),
@@ -85,7 +93,9 @@ EXPORTS = [
     "etl_dec_batch_summary", "etl_dec_batch_schema", "etl_dec_decode_sharded", "etl_dec_comm_unique_id", "etl_dec_comm_init", "etl_dec_comm_init_host",
     "etl_dec_kind_for_type_oid", "etl_dec_mem_info",
     "etl_dec_copy_decode", "etl_dec_arrow_emit", "etl_dec_arrow_rows", "etl_dec_arrow_cols", "etl_dec_arrow_row_records",
-    "etl_dec_arrow_column", "etl_dec_arrow_list_child", "etl_dec_arrow_first_skipped", "etl_dec_arrow_free", "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
+    "etl_dec_arrow_column", "etl_dec_arrow_list_child", "etl_dec_arrow_first_skipped", "etl_dec_arrow_free", "etl_dec_rowbinary_emit", "etl_dec_rowbinary_rows", "etl_dec_rowbinary_bytes",
+    "etl_dec_rowbinary_data", "etl_dec_rowbinary_row_offsets", "etl_dec_rowbinary_row_records", "etl_dec_rowbinary_issues",
+    "etl_dec_rowbinary_free", "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
 ]
 
@@ -156,6 +166,16 @@ def load(build: bool = True):
     L.etl_dec_arrow_first_skipped.restype = C.c_uint64
     L.etl_dec_arrow_free.argtypes = [vp]
     L.etl_dec_arrow_free.restype = None
+    L.etl_dec_rowbinary_emit.argtypes = [vp, C.c_uint32, vp, C.c_uint32, C.c_int, C.POINTER(vp)]
+    for f in ("etl_dec_rowbinary_rows", "etl_dec_rowbinary_bytes"):
+        getattr(L, f).argtypes = [vp]
+        getattr(L, f).restype = C.c_uint64
+    for f in ("etl_dec_rowbinary_data", "etl_dec_rowbinary_row_offsets", "etl_dec_rowbinary_row_records"):
+        getattr(L, f).argtypes = [vp, C.c_int]
+        getattr(L, f).restype = C.c_void_p
+    L.etl_dec_rowbinary_issues.argtypes = [vp, C.POINTER(RowBinaryIssues)]
+    L.etl_dec_rowbinary_free.argtypes = [vp]
+    L.etl_dec_rowbinary_free.restype = None
     L.etl_dec_batch_device_stream.argtypes = [vp]
     L.etl_dec_batch_device_stream.restype = C.c_void_p
     L.etl_shim_materialise.argtypes = [vp, vp, vp, C.POINTER(vp)]

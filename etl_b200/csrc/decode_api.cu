@@ -51,6 +51,7 @@ struct RelVersion {  // ReplicatedTableSchema (schema.rs:651-900)
   uint32_t n_ident = 0;
   std::vector<uint8_t> kind, flags;
   std::vector<int32_t> index;
+  std::vector<uint8_t> pk;   // 1 = the stored column has a primary_key_ordinal_position (etl_schema_pk_columns)
 };
 
 bool kind_supported_on_device(uint32_t k) {
@@ -569,12 +570,13 @@ static uint32_t build_relation(etl_dec_ctx* ctx, const uint8_t* frame, uint64_t 
     if (!found) return ETL_E_UNKNOWN_COLUMNS;                  // schema.rs:288-309
   }
   out->table_id = rel_id; out->snapshot_id = t.snapshot_id; out->effective_off = off; out->n_ident = 0;
-  out->kind.clear(); out->flags.clear(); out->index.clear();
+  out->kind.clear(); out->flags.clear(); out->index.clear(); out->pk.clear();
   for (size_t k = 0; k < t.cols.size(); k++) {
     if (!repl[k]) continue;
     out->kind.push_back((uint8_t)etl_oid_decode_class(t.cols[k].type_oid));
     out->flags.push_back((uint8_t)((t.cols[k].nullable ? 1 : 0) | (ident[k] ? 2 : 0)));
     out->index.push_back((int32_t)k);
+    out->pk.push_back(t.cols[k].pk != -1 ? 1 : 0);
     if (ident[k]) out->n_ident++;
   }
   return 0;
@@ -1528,6 +1530,11 @@ int etl_dec_mem_info(etl_dec_ctx* ctx, uint64_t* free_bytes, uint64_t* total_byt
 
 }  // extern "C"
 
+bool etl_schema_pk_columns(const etl_dec_batch* b, uint32_t index, const uint8_t** pk) {
+  if (!b || index >= b->schemas.size()) return false;
+  *pk = b->schemas[index].pk.data();
+  return true;
+}
 bool etl_copy_batch_columns(const etl_dec_batch* b, uint32_t* table_id, const uint8_t** col_kind, uint32_t* n_cols) {
   if (!b || !b->copy) return false;
   *table_id = b->copy_table; *col_kind = b->copy_kinds.data(); *n_cols = (uint32_t)b->copy_kinds.size();

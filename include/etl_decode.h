@@ -512,6 +512,60 @@ int etl_dec_arrow_list_child(const etl_arrow_batch*, uint32_t column, int host, 
  * leaves the record out.  UINT64_MAX if there is none; always UINT64_MAX for a COPY batch. */
 uint64_t etl_dec_arrow_first_skipped(const etl_arrow_batch*);
 void etl_dec_arrow_free(etl_arrow_batch*);
+/* ---------------------------------------------------------------- ClickHouse RowBinary emitter
+ * The rows of ONE replicated-schema version of a decoded batch as the RowBinary byte stream the ClickHouse destination
+ * sends in its INSERT bodies, built on the device, plus n_rows + 1 u64 row offsets (row i = [off[i], off[i+1]) of the
+ * data).  Replaces the per-row host walk of crates/etl-destinations/src/clickhouse: write_events_inner /
+ * flush_pending_rows (core.rs:694-863) and write_table_rows_inner (:489-521) mapping each cell through
+ * cell_to_clickhouse_value (encoding.rs:50-78), expand_key_row / default_cell (core.rs:920-997), and
+ * encode_to_row_binary (encoding.rs:249-273) called row by row from insert_rows (client.rs:336-379).
+ * Rows, in record order, are the records of the version in the valid prefix that carry ETL_RF_EVENT: an Insert's new
+ * image; an Update's new image when Full (an Update with ETL_RF_NEW_PARTIAL is no row, see first_partial_update); a
+ * Delete's old image when ETL_RF_OLD_FULL, else its key image expanded column by column in schema order: a column whose
+ * stored TableSchema column has a primary_key_ordinal_position takes the next key cell (NULL once they run out), a
+ * source-nullable non-array column is NULL, any other column gets default_cell, on the wire all zero bytes (Bool 1;
+ * I16 2; I32 / U32 / F32 / Date 4; I64 / F64 / Timestamp / TimestampTz 8; Uuid 16; String, Numeric, Time, Json, Bytes
+ * and arrays 1: an empty string or array).  A COPY batch (rec_kind == NULL): every row of the valid prefix, schema_index
+ * must be 0.  Each row holds the n_cols user columns, then cdc_operation (String "INSERT" / "UPDATE" / "DELETE"; COPY
+ * rows "INSERT") and cdc_lsn (UInt64, the record's rec_commit_lsn; COPY rows 0).
+ * nullable_flags: n_cols + 2 bytes, non-zero = the ClickHouse column is Nullable(...) (the table's actual types,
+ * nullable_flags_from_clickhouse_columns, core.rs:102-142); any other n_flags is ETL_ERR_INVALID_ARG.  A flagged column
+ * writes a marker byte (1 NULL, 0 value) before its value.  Values follow the cell's variant (rb_encode_value,
+ * encoding.rs:201-246): Bool 1 byte; I16 / I32 / I64 / U32 and the IEEE bits of F32 / F64 little-endian; Date → Date32
+ * i32 days; Timestamp / TimestampTz → i64 micros (secs * 10^6 + nanos / 1000); Uuid → high u64 LE then low u64 LE of the
+ * big-endian bytes; String, and as Strings: Numeric (PgNumeric's Display), Json (serde_json's compact Display, the
+ * ETL_ARROW_ALL_COLUMNS text), Time (NaiveTime's Display) and Bytes (lowercase hex) → LEB128 length + bytes; arrays →
+ * LEB128 count + every element as Nullable.
+ * Data issues do not fail the call; the first of each kind is reported (etl_dec_rowbinary_issues).  Every row before
+ * the reported row of an issue is byte-exact; a row with an issue has consistent offsets but unspecified bytes.
+ * Scratch, beside the output: 4 B per (row, column) + 4 B per row + 16 B per record of the batch, and with Json columns
+ * 4 B per (row, Json column) + 8 B per such item + 17 B per input byte of Json text.  A row of 4 GiB or more is
+ * ETL_ERR_INVALID_ARG; a Json value that does not parse again (the decode validated it) is ETL_ERR_INTERNAL. */
+typedef struct etl_rb_issue {
+  uint64_t row;      /* emitted row; UINT64_MAX = no such issue */
+  uint32_t column;   /* column of the row (0 .. n_cols + 1) */
+  uint32_t element;  /* array element, UINT32_MAX for a scalar */
+} etl_rb_issue;
+typedef struct etl_rowbinary_issues {
+  etl_rb_issue date_range;       /* first Date outside 1900-01-01 ..= 2299-12-31 (ConversionError "Date out of ClickHouse
+                                    Date32 range", encoding.rs:131-148), in (row, column, element) order */
+  etl_rb_issue null_value;       /* first NULL in a column whose flag is clear (ConversionError "NULL value for
+                                    non-nullable ClickHouse column", encoding.rs:204-212) */
+  uint64_t first_partial_update; /* smallest batch-local record index of an Update with ETL_RF_NEW_PARTIAL (InvalidState
+                                    "ClickHouse update requires a full new row image", core.rs:721-735); UINT64_MAX if none */
+} etl_rowbinary_issues;
+typedef struct etl_rowbinary_batch etl_rowbinary_batch;
+int etl_dec_rowbinary_emit(const etl_dec_batch*, uint32_t schema_index, const uint8_t* nullable_flags, uint32_t n_flags,
+                           int to_host, etl_rowbinary_batch** out);
+uint64_t etl_dec_rowbinary_rows(const etl_rowbinary_batch*);
+uint64_t etl_dec_rowbinary_bytes(const etl_rowbinary_batch*);
+const uint8_t* etl_dec_rowbinary_data(const etl_rowbinary_batch*, int host);
+const uint64_t* etl_dec_rowbinary_row_offsets(const etl_rowbinary_batch*, int host);   /* n_rows + 1 */
+/* record index of each row (a COPY batch: the row index) */
+const uint64_t* etl_dec_rowbinary_row_records(const etl_rowbinary_batch*, int host);
+int etl_dec_rowbinary_issues(const etl_rowbinary_batch*, etl_rowbinary_issues* out);
+void etl_dec_rowbinary_free(etl_rowbinary_batch*);
+
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
 const uint8_t* etl_dec_batch_device_stream(const etl_dec_batch*);
