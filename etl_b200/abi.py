@@ -60,6 +60,14 @@ class RowBinaryIssues(C.Structure):
     _fields_ = [("date_range", RbIssue), ("null_value", RbIssue), ("first_partial_update", C.c_uint64)]
 
 
+class BqIssue(C.Structure):
+    _fields_ = [("row", C.c_uint64), ("column", C.c_uint32), ("element", C.c_uint32), ("kind", C.c_uint32), ("_pad", C.c_uint32)]
+
+
+class BigQueryIssues(C.Structure):
+    _fields_ = [("value", BqIssue), ("first_invalid_record", C.c_uint64)]
+
+
 class Planes(C.Structure):
     _fields_ = [("n_records", C.c_uint64), ("n_cells", C.c_uint64), ("heap_bytes", C.c_uint64),
                 ("rec_off", C.c_void_p), ("rec_kind", C.c_void_p), ("rec_flags", C.c_void_p), ("rec_rel", C.c_void_p),
@@ -95,7 +103,9 @@ EXPORTS = [
     "etl_dec_copy_decode", "etl_dec_arrow_emit", "etl_dec_arrow_rows", "etl_dec_arrow_cols", "etl_dec_arrow_row_records",
     "etl_dec_arrow_column", "etl_dec_arrow_list_child", "etl_dec_arrow_first_skipped", "etl_dec_arrow_free", "etl_dec_rowbinary_emit", "etl_dec_rowbinary_rows", "etl_dec_rowbinary_bytes",
     "etl_dec_rowbinary_data", "etl_dec_rowbinary_row_offsets", "etl_dec_rowbinary_row_records", "etl_dec_rowbinary_issues",
-    "etl_dec_rowbinary_free", "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
+    "etl_dec_rowbinary_free", "etl_dec_bigquery_emit", "etl_dec_bigquery_rows", "etl_dec_bigquery_bytes", "etl_dec_bigquery_data",
+    "etl_dec_bigquery_row_offsets", "etl_dec_bigquery_row_records", "etl_dec_bigquery_issues", "etl_dec_bigquery_free",
+    "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
 ]
 
@@ -176,6 +186,16 @@ def load(build: bool = True):
     L.etl_dec_rowbinary_issues.argtypes = [vp, C.POINTER(RowBinaryIssues)]
     L.etl_dec_rowbinary_free.argtypes = [vp]
     L.etl_dec_rowbinary_free.restype = None
+    L.etl_dec_bigquery_emit.argtypes = [vp, C.c_uint32, C.c_int, C.POINTER(vp)]
+    for f in ("etl_dec_bigquery_rows", "etl_dec_bigquery_bytes"):
+        getattr(L, f).argtypes = [vp]
+        getattr(L, f).restype = C.c_uint64
+    for f in ("etl_dec_bigquery_data", "etl_dec_bigquery_row_offsets", "etl_dec_bigquery_row_records"):
+        getattr(L, f).argtypes = [vp, C.c_int]
+        getattr(L, f).restype = C.c_void_p
+    L.etl_dec_bigquery_issues.argtypes = [vp, C.POINTER(BigQueryIssues)]
+    L.etl_dec_bigquery_free.argtypes = [vp]
+    L.etl_dec_bigquery_free.restype = None
     L.etl_dec_batch_device_stream.argtypes = [vp]
     L.etl_dec_batch_device_stream.restype = C.c_void_p
     L.etl_shim_materialise.argtypes = [vp, vp, vp, C.POINTER(vp)]
@@ -200,6 +220,11 @@ ARROW_ALL_COLUMNS = 0x100
 ARROW_LIST = 13
 # row_kinds bit: append cdc_operation and sequence_number, the Iceberg CDC columns (ETL_ARROW_CDC_COLUMNS)
 ARROW_CDC_COLUMNS = 0x200
+
+# etl_bq_issue.kind (ETL_BQ_ISSUE_*)
+BQ_ISSUE_ARRAY_NULL = 1
+BQ_ISSUE_NUMERIC_SCALE = 2
+BQ_ISSUE_JSON_INTEGER = 3
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

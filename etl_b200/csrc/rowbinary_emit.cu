@@ -13,13 +13,14 @@
 // Passes (one CUDA stream, three syncs: selection, Json sizes when a Json column exists, output size):
 //   1. k_sel_count / k_blk_scan / k_sel_scatter<ClickHouseRows> (emit_scan.cuh): rows in record order, first partial
 //      update.  COPY: k_copy_sel, no sync.
-//   2. Json: every Json cell and Json array element is canonicalised once (etl_fmt::json_canon) into scratch laid out
-//      per item (row, Json column) from a scan of the input lengths: [u32 canonical length][text] per document, each
-//      record 4 + input bytes long (the canonical text is never longer than the input).
+//   2. Json (k_json_len / k_json_canon, row_emit_common.cuh): every Json cell and Json array element is canonicalised
+//      once (etl_fmt::json_canon) into scratch laid out per item (row, Json column) from a scan of the input lengths:
+//      [u32 canonical length][text] per document, each record 4 + input bytes long (the canonical text is never longer
+//      than the input).
 //   3. k_rb_size: thread per (row, column) over W = n_cols + 2 in row-major order: the cell's byte length with its
 //      marker; the first Date32 violation and the first NULL under a cleared flag by warp-reduced atomicMin.
-//   4. k_rb_row_scan (warp per row): lengths → u32 in-row cell offsets + the row's length; the row lengths are scanned
-//      into u64 row offsets (k_len_blocks / k_blk_scan64 / k_offsets); the total sizes the output.
+//   4. k_row_scan (warp per row, row_emit_common.cuh): lengths → u32 in-row cell offsets + the row's length; the row
+//      lengths are scanned into u64 row offsets (k_len_blocks / k_blk_scan64 / k_offsets); the total sizes the output.
 //   5. k_rb_write: thread per (row, column), so consecutive lanes store adjacent bytes of a row; String / Json / hex
 //      payloads above kLongCell bytes are copied by the whole warp.  k_rb_date_elem finds the element of an array
 //      Date32 violation.
@@ -35,6 +36,7 @@
 #include "rowbinary_format.cuh"
 #include "batch_internal.h"
 #include "emit_scan.cuh"
+#include "row_emit_common.cuh"
 
 namespace {
 
@@ -195,44 +197,14 @@ __device__ __forceinline__ void report_min(unsigned long long key, unsigned long
 }
 
 // ---------------------------------------------------------------- Json
-// item i = (row, Json column j): 4 + input bytes per document (the Json cell, or each Json element of an array cell)
-__global__ void __launch_bounds__(256) k_rb_json_len(RbParams P, uint32_t* lens) {
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P.n_rows * P.n_json) return;
-  const uint64_t row = i / P.n_json;
-  uint64_t cell = 0, n = 0;
-  if (cell_at(P, row, P.json_col[i - row * P.n_json], &cell) == kFromCell) {
-    const uint32_t tag = P.cell_tag[cell], aux = P.cell_aux[cell];
-    if (tag == ETL_CELL_JSON) n = 4ull + aux;
-    else if (tag == ETL_CELL_ARRAY) {
-      const etl_array_elem* E = elems_of(P, P.cell_val[cell]);
-      for (uint32_t k = 0; k < aux; k++) if (E[k].tag == ETL_CELL_JSON) n += 4ull + E[k].aux;
-    }
+// item i = (row, Json column j), staged by row_emit_common.cuh
+struct RbJsonCells {
+  RbParams P;
+  __device__ __forceinline__ bool operator()(uint64_t i, uint64_t* cell) const {
+    const uint64_t row = i / P.n_json;
+    return cell_at(P, row, P.json_col[i - row * P.n_json], cell) == kFromCell;
   }
-  lens[i] = (uint32_t)n;
-}
-// thread per item: canonicalise its documents in order, each record [u32 canonical length][text]; a document's node
-// scratch sits at 4 words per byte of its record, which json_canon_work_words (<= 4n + 16) fits
-__global__ void __launch_bounds__(128) k_rb_json_canon(RbParams P) {
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P.n_rows * P.n_json) return;
-  const uint64_t row = i / P.n_json;
-  uint64_t cell = 0;
-  if (cell_at(P, row, P.json_col[i - row * P.n_json], &cell) != kFromCell) return;
-  const uint32_t tag = P.cell_tag[cell], aux = P.cell_aux[cell];
-  uint64_t at = P.json_off[i];
-  auto one = [&](const uint8_t* s, uint32_t n) {
-    uint32_t r = etl_fmt::json_canon(s, n, P.canon + at + 4, P.work + 4 * at);
-    if (r == etl_fmt::kJsonCanonBad) { atomicOr(P.issues + kIssueFlags, (unsigned long long)kFlagBadJson); r = 0; }   // json_valid let it through
-    etl_rb::le_write(r, 4, P.canon + at);
-    at += 4ull + n;
-  };
-  if (tag == ETL_CELL_JSON) one(text_of(P, P.cell_val[cell]), aux);
-  else if (tag == ETL_CELL_ARRAY) {
-    const etl_array_elem* E = elems_of(P, P.cell_val[cell]);
-    for (uint32_t k = 0; k < aux; k++) if (E[k].tag == ETL_CELL_JSON) one(P.heap + E[k].val, E[k].aux);
-  }
-}
+};
 
 // ---------------------------------------------------------------- size, offsets, write
 // the payload of a String / Json / Bytes scalar cell
@@ -276,30 +248,6 @@ __global__ void __launch_bounds__(256) k_rb_size(RbParams P) {
   }
   report_min(date_key, P.issues + kIssueDate);
   report_min(null_key, P.issues + kIssueNull);
-}
-
-// warp per row: the row's cell lengths → offsets inside the row, and the row's length
-__global__ void __launch_bounds__(256) k_rb_row_scan(RbParams P) {
-  const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t lane = threadIdx.x & 31;
-  if (row >= P.n_rows) return;                          // whole warps
-  uint32_t* L = P.cell_len + row * P.w;
-  unsigned long long run = 0;
-  for (uint32_t base = 0; base < P.w; base += 32) {
-    const uint32_t c = base + lane;
-    const unsigned long long v = c < P.w ? L[c] : 0u;
-    unsigned long long x = v;
-    for (int d = 1; d < 32; d <<= 1) {
-      const unsigned long long y = __shfl_up_sync(kFull, x, d);
-      if (lane >= (uint32_t)d) x += y;
-    }
-    if (c < P.w) L[c] = (uint32_t)(run + x - v);
-    run += __shfl_sync(kFull, x, 31);
-  }
-  if (lane == 0) {
-    if (run > 0xffffffffull) atomicOr(P.issues + kIssueFlags, (unsigned long long)kFlagRowTooLong);
-    P.row_len[row] = (uint32_t)run;
-  }
 }
 
 __global__ void __launch_bounds__(256) k_rb_write(RbParams P) {
@@ -476,7 +424,9 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
       uint64_t* joff = (uint64_t*)salloc((n_items + 1) * 8);
       unsigned long long* jblk = (unsigned long long*)salloc((jb + 1) * 8ull);
       if (!jl || !joff || !jblk) return fail(ETL_ERR_ALLOC);
-      k_rb_json_len<<<(uint32_t)((n_items + 255) / 256), 256, 0, st>>>(R, jl);
+      JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, dev_stream, n_items, joff, nullptr, nullptr,
+                  d_issues + kIssueFlags, (unsigned long long)kFlagBadJson};
+      k_json_len<RbJsonCells><<<(uint32_t)((n_items + 255) / 256), 256, 0, st>>>(J, RbJsonCells{R}, jl);
       k_len_blocks<<<jb, 1024, 0, st>>>(jl, n_items, jblk);
       k_blk_scan64<<<1, 1024, 0, st>>>(jblk, jb, jblk + jb);
       k_offsets<uint64_t><<<jb, 1024, 0, st>>>(jl, n_items, jblk, joff);
@@ -486,7 +436,9 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
       R.canon = (uint8_t*)salloc(jt);
       R.work = (uint32_t*)salloc(16 * jt);
       if (!R.canon || !R.work) return fail(ETL_ERR_ALLOC);
-      if (jt) k_rb_json_canon<<<(uint32_t)((n_items + 127) / 128), 128, 0, st>>>(R);
+      J.canon = R.canon;
+      J.work = R.work;
+      if (jt) k_json_canon<RbJsonCells><<<(uint32_t)((n_items + 127) / 128), 128, 0, st>>>(J, RbJsonCells{R});
     }
     // sizes → in-row offsets → row offsets (sync)
     const uint64_t n_cells = n_rows * W;
@@ -496,7 +448,8 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
     unsigned long long* rblk = (unsigned long long*)salloc((rb + 1) * 8ull);
     if (!R.cell_len || !R.row_len || !rblk) return fail(ETL_ERR_ALLOC);
     k_rb_size<<<(uint32_t)((n_cells + 255) / 256), 256, 0, st>>>(R);
-    k_rb_row_scan<<<(uint32_t)((n_rows * 32 + 255) / 256), 256, 0, st>>>(R);
+    k_row_scan<<<(uint32_t)((n_rows * 32 + 255) / 256), 256, 0, st>>>(R.cell_len, W, n_rows, R.row_len, d_issues + kIssueFlags,
+                                                                       (unsigned long long)kFlagRowTooLong);
     k_len_blocks<<<rb, 1024, 0, st>>>(R.row_len, n_rows, rblk);
     k_blk_scan64<<<1, 1024, 0, st>>>(rblk, rb, rblk + rb);
     k_offsets<uint64_t><<<rb, 1024, 0, st>>>(R.row_len, n_rows, rblk, (uint64_t*)B->meta);

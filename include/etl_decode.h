@@ -566,6 +566,75 @@ const uint64_t* etl_dec_rowbinary_row_records(const etl_rowbinary_batch*, int ho
 int etl_dec_rowbinary_issues(const etl_rowbinary_batch*, etl_rowbinary_issues* out);
 void etl_dec_rowbinary_free(etl_rowbinary_batch*);
 
+/* ---------------------------------------------------------------- BigQuery Storage Write emitter
+ * The rows of ONE replicated-schema version of a decoded batch as the serialized protobuf messages the BigQuery
+ * destination puts into ProtoRows.serialized_rows, built on the device, plus n_rows + 1 u64 row offsets: row i is
+ * data[off[i], off[i+1]), one message without a length prefix.  Replaces the per-row host walk of
+ * crates/etl-destinations/src/bigquery: write_events (core.rs:792-970) with bigquery_update_rows /
+ * bigquery_primary_key_changed (:1255-1403) and bigquery_delete_row (:1406-1524), write_table_rows (:530-546),
+ * BigQueryTableRow::try_from_tagged_cells (encoding.rs:49-83) with validate_cell_for_bigquery (validation.rs) and the
+ * prost serialisation (cell_encode_prost / array_cell_encode_prost, encoding.rs:151-342).
+ * Fields (column_schemas_to_table_descriptor, client.rs:1292-1385): column c is field c + 1, _CHANGE_TYPE (String
+ * "UPSERT" / "DELETE") field n_cols + 1, _CHANGE_SEQUENCE_NUMBER (String) field n_cols + 2, the 50 lowercase bytes
+ * "{rec_commit_lsn:016x}/{rec_tx_ordinal:016x}/{ordinal:016x}" (bigquery_sequence_key, core.rs:1235).
+ * Rows, in record order, come from the records of the version in the valid prefix that carry ETL_RF_EVENT:
+ *   Insert → UPSERT of the new image, ordinal 0;
+ *   Update → UPSERT of the new image, ordinal 0; when a primary-key cell changed, a DELETE of the old key (ordinal 0)
+ *            comes first and the UPSERT has ordinal 1.  Changed: with a Full old image, any primary-key column whose
+ *            old and new cells differ; with a key image, the key cells against the new image's primary-key cells in
+ *            order; no old image: unchanged.  Cells compare as Cell's PartialEq: same variant, F32 / F64 by IEEE ==
+ *            (a NaN key always changes, -0 equals +0), Numeric by sign, weight, scale and digits (1.0 != 1.00), Json by
+ *            its canonical text (serde_json Value equality), arrays element by element;
+ *   Delete → DELETE of the old key, ordinal 0.
+ * A DELETE row holds only the primary-key columns (the stored TableSchema column has a primary_key_ordinal_position),
+ * each under its own field, from the Full old image or from the key image taken in order.  No row, and the record
+ * counts for first_invalid_record (InvalidState in write_events): an Update with ETL_RF_NEW_PARTIAL (core.rs:837-850),
+ * a Delete with neither old image (:868-879), an Update or Delete with a key image when the version's identity columns
+ * are not its primary-key columns (identity_matches_primary_key, :1347-1359, :1439-1451).
+ * A COPY batch (rec_kind == NULL): every row of the valid prefix as an UPSERT without the sequence field (write_table_rows);
+ * schema_index must be 0, and etl_dec_bigquery_row_records gives the row index.
+ * Cells (prost; proto3's omission of default values does not apply, NULL writes nothing): the key is
+ * varint(field << 3 | wire type).  Bool wt 0, one byte; I16 / I32 / I64 wt 0, varint of the value sign-extended to 64
+ * bits; U32 wt 0, varint; F32 wt 5 / F64 wt 1, IEEE bits little-endian; Bytes wt 2, varint length + bytes; String, Uuid
+ * (lowercase, hyphenated), Numeric (PgNumeric's Display), Json (serde_json's compact Display, the ETL_ARROW_ALL_COLUMNS
+ * text), Date (%Y-%m-%d: years 0..=9999 as 4 digits, others with a sign and at least 4 digits), Time (%H:%M:%S%.f),
+ * Timestamp (%Y-%m-%d %H:%M:%S%.f) and TimestampTz (the same + "+00:00") wt 2, varint length + UTF-8 text.  Arrays of
+ * Bool / I16 / I32 / U32 / I64 / F32 / F64 are packed (one wt 2 key, the payload length, the values without keys);
+ * arrays of any other kind write one wt 2 field per element; an empty array writes nothing.
+ * Value issues (etl_bigquery_issues.value) do not fail the call: the first in (row, column) order over the emitted rows,
+ * the key cells of DELETE rows and COPY rows included.  ARRAY_NULL: an array with a NULL element (the conversion to
+ * CellNonOptional, checked first; element = the first NULL); NUMERIC_SCALE: a Numeric value, scalar or element, whose
+ * Display has more than 38 fractional digits; JSON_INTEGER: a Json document, scalar or element, holding an integer
+ * literal (no '.', 'e', 'E') outside i64 (starting with '-') or u64.  element is UINT32_MAX for a scalar.  Every row
+ * before the reported row is byte-exact; the reported row has consistent offsets (a NULL element writes nothing).
+ * to_host: also copy offsets, records and bytes to a pinned buffer (host = 1 accessors); else those return NULL.
+ * Scratch, beside the output: 4 B per (row, field) + 12 B per row + 28 B per record of the batch, and with Json columns
+ * 12 B per (record, Json column, image) + 17 B per input byte of Json text.  schema_index out of range, or non-zero
+ * for a COPY batch, is ETL_ERR_INVALID_ARG; a row of 4 GiB or more is ETL_ERR_INVALID_ARG; a Json value that does not
+ * parse again (the decode validated it) is ETL_ERR_INTERNAL. */
+enum { ETL_BQ_ISSUE_ARRAY_NULL = 1, ETL_BQ_ISSUE_NUMERIC_SCALE = 2, ETL_BQ_ISSUE_JSON_INTEGER = 3 };
+typedef struct etl_bq_issue {
+  uint64_t row;      /* emitted row; UINT64_MAX = none */
+  uint32_t column;   /* user column of the row (field column + 1) */
+  uint32_t element;  /* array element, UINT32_MAX for a scalar */
+  uint32_t kind;     /* ETL_BQ_ISSUE_* */
+  uint32_t _pad;
+} etl_bq_issue;
+typedef struct etl_bigquery_issues {
+  etl_bq_issue value;             /* first value issue in (row, column) order; row == UINT64_MAX: none */
+  uint64_t first_invalid_record;  /* smallest batch-local record that write_events rejects with InvalidState; UINT64_MAX: none */
+} etl_bigquery_issues;
+typedef struct etl_bigquery_batch etl_bigquery_batch;
+int etl_dec_bigquery_emit(const etl_dec_batch*, uint32_t schema_index, int to_host, etl_bigquery_batch** out);
+uint64_t etl_dec_bigquery_rows(const etl_bigquery_batch*);
+uint64_t etl_dec_bigquery_bytes(const etl_bigquery_batch*);
+const uint8_t* etl_dec_bigquery_data(const etl_bigquery_batch*, int host);
+const uint64_t* etl_dec_bigquery_row_offsets(const etl_bigquery_batch*, int host);  /* n_rows + 1 */
+/* record index of each row (a COPY batch: the row index); both rows of a primary-key change carry the same record */
+const uint64_t* etl_dec_bigquery_row_records(const etl_bigquery_batch*, int host);
+int etl_dec_bigquery_issues(const etl_bigquery_batch*, etl_bigquery_issues* out);
+void etl_dec_bigquery_free(etl_bigquery_batch*);
+
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
 const uint8_t* etl_dec_batch_device_stream(const etl_dec_batch*);
