@@ -973,6 +973,16 @@ static void fill_planes(etl_dec_planes& pl, uint8_t* bs, const PlaneLayout& L, u
   pl.cell_tag = bs + L.tag; pl.cell_val = (uint64_t*)(bs + L.val); pl.cell_aux = (uint32_t*)(bs + L.aux); pl.heap = bs + L.heap;
 }
 
+// The kernels bump-allocate the scalar heap without checking its end (the bound is sized so that they cannot pass it);
+// a heap_top above the bound means cells point past what was reserved: an error, never a truncated result.
+static int check_scalar_heap(etl_dec_ctx* ctx, uint64_t scalar_heap) {
+  const uint64_t top = ctx->h_scalars[5];
+  if (top <= scalar_heap) return ETL_OK;
+  ctx->last_error = "scalar heap bound exceeded: the kernels allocated " + std::to_string(top) + " bytes of a " +
+                    std::to_string(scalar_heap) + "-byte scalar heap";
+  return ETL_ERR_CUDA;
+}
+
 // ---------------------------------------------------------------- pass C into planes of capacity (cap_r, cap_c)
 // entries of the binned record order: the records plus at most 31 padding lanes per (tile, bin)
 static size_t perm_capacity(const DecodeParams& P) { return P.cap_records + 32ull * P.n_bin_tiles * P.n_bins + 256; }
@@ -981,9 +991,13 @@ static int launch_emit(etl_dec_ctx* ctx, etl_dec_batch* b, uint64_t cap_r, uint6
   cudaStream_t st = ctx->stream;
   bool any_heap = false, any_array = false;
   for (const RelVersion& v : b->schemas) for (uint8_t k : v.kind) { any_heap = any_heap || kind_has_heap(k); any_array = any_array || (k & ETL_K_ARRAY); }
-  // upper bound on Σ cell_heap_bound: numeric ≤ n/2+19, bytea ≤ n/2+7, uuid = 16 per decoded text cell.
+  // scalar heap: every byte bump-allocated from heap_top, per cell of length n (Σ n ≤ len, at most cap_c cells):
+  //   k_rows   uuid slot of a light-parsed uuid cell: 16, reserved before fast_uuid looks at the text
+  //   k_heavy  cell_heap_bound of a pending cell: numeric ≤ n/2 + 19, bytea ≤ n/2 + 6, uuid 16 — a uuid that
+  //            fast_uuid declined (any other spelling, or an invalid value) holds both slots: 32
+  // → ≤ len/2 + 32·cap_c.  The host fails the decode if heap_top ends above it.
   // Arrays reserve 16 + 44·n_elems + 1.5·len per cell: first guess 3·len, retried ×4 on overflow (≤ 48·len).
-  uint64_t nh = any_heap ? (P.len / 2 + 24 * cap_c + 256) : 0;
+  uint64_t nh = any_heap ? (P.len / 2 + 32 * cap_c + 256) : 0;
   nh = (nh + 15) & ~15ull;
   *scalar_heap_out = nh;
   if (any_array) nh += array_heap ? array_heap : 3 * P.len + 4096;
@@ -1189,6 +1203,8 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
       continue;
     }
     const Summ T = *ctx->h_total;
+    if (int rc = check_scalar_heap(ctx, scalar_heap)) return fail(rc);
+    // (the min only trims the 8-byte rounding of the last array reservation: the scalar region was checked above)
     heap_used = P.heap_cap;
     if (P.heap_cap) heap_used = std::min<uint64_t>(P.heap_cap, ctx->h_scalars[10] ? scalar_heap + ctx->h_scalars[10] : ctx->h_scalars[5]);
     if (ctx->h_scalars[9]) {                          // an array reservation did not fit: larger array region, pass C again
@@ -1394,8 +1410,15 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
     P.buf = ctx->d_stream.ptr(); h2d += in->len;
   }
   const uint64_t nr = in->n_rows, nc = nr * n_cols;
-  // planes: rec_off (row offsets) + cells + heap (unescaped text ≤ len, scalar payloads, arrays)
-  uint64_t nh = in->len + 64 + (any_heap ? in->len / 2 + 24 * nc + 256 : 0);
+  // planes: rec_off (row offsets) + cells + heap (scalar region, then arrays).  The scalar region holds every byte
+  // bump-allocated from heap_top, per emitted field of length flen (at most nc fields, Σ flen ≤ len) and unescaped
+  // length n ≤ flen; a row that ends in an error has its earlier fields decoded all the same:
+  //   k_copy_rows  unescaped copy of a field with a backslash: (flen + 7) & ~7 ≤ flen + 8
+  //                uuid slot of an unescaped uuid field: 16, reserved before fast_uuid looks at the text
+  //   k_heavy      cell_heap_bound of a pending cell, on its (unescaped) length: numeric ≤ n/2 + 19, bytea ≤ n/2 + 6,
+  //                uuid 16 — a uuid that fast_uuid declined holds both slots: 32
+  // → ≤ len + 8·nc without heap kinds, ≤ len + len/2 + (8 + 32)·nc with them.  Checked after the kernels.
+  uint64_t nh = in->len + 8 * nc + 64 + (any_heap ? in->len / 2 + 32 * nc + 256 : 0);
   nh = (nh + 15) & ~15ull;
   const uint64_t scalar_heap = nh;
   uint64_t array_heap = any_array ? 3 * in->len + 4096 : 0;
@@ -1444,10 +1467,12 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
     CKB(cudaEventRecord(ctx->ev[4], st));
     CKB(cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars.ptr(), kScalarWords * 8, cudaMemcpyDeviceToHost, st));
     CKB(cudaStreamSynchronize(st));
+    if (int rc = check_scalar_heap(ctx, scalar_heap)) return fail(rc);
     if (!ctx->h_scalars[9]) break;
     if (attempt >= 4) { ctx->last_error = "array heap reservation overflow after retries"; return fail(ETL_ERR_CUDA); }
     array_heap *= 4;
   }
+  // (the min only trims the 8-byte rounding of the last array reservation: the scalar region was checked above)
   const uint64_t heap_used = std::min<uint64_t>(P.heap_cap, ctx->h_scalars[10] ? scalar_heap + ctx->h_scalars[10] : ctx->h_scalars[5]);
   b->dev.heap_bytes = heap_used;
   uint64_t d2h = kScalarWords * 8;
