@@ -68,6 +68,15 @@ class BigQueryIssues(C.Structure):
     _fields_ = [("value", BqIssue), ("first_invalid_record", C.c_uint64)]
 
 
+class DuckLakeIssues(C.Structure):
+    _fields_ = [("first_rejected_record", C.c_uint64), ("rejected_reason", C.c_uint32), ("mixed_versions", C.c_uint32),
+                ("first_empty_partial_record", C.c_uint64)]
+
+
+class DlSubBatch(C.Structure):
+    _fields_ = [("first_mutation", C.c_uint64), ("n_mutations", C.c_uint32), ("_pad", C.c_uint32), ("fingerprint", C.c_uint64)]
+
+
 class Planes(C.Structure):
     _fields_ = [("n_records", C.c_uint64), ("n_cells", C.c_uint64), ("heap_bytes", C.c_uint64),
                 ("rec_off", C.c_void_p), ("rec_kind", C.c_void_p), ("rec_flags", C.c_void_p), ("rec_rel", C.c_void_p),
@@ -105,6 +114,9 @@ EXPORTS = [
     "etl_dec_rowbinary_data", "etl_dec_rowbinary_row_offsets", "etl_dec_rowbinary_row_records", "etl_dec_rowbinary_issues",
     "etl_dec_rowbinary_free", "etl_dec_bigquery_emit", "etl_dec_bigquery_rows", "etl_dec_bigquery_bytes", "etl_dec_bigquery_data",
     "etl_dec_bigquery_row_offsets", "etl_dec_bigquery_row_records", "etl_dec_bigquery_issues", "etl_dec_bigquery_free",
+    "etl_dec_ducklake_emit", "etl_dec_ducklake_mutations", "etl_dec_ducklake_kinds", "etl_dec_ducklake_records",
+    "etl_dec_ducklake_text", "etl_dec_ducklake_issues", "etl_dec_ducklake_sub_batches", "etl_dec_ducklake_copy_fingerprint",
+    "etl_dec_ducklake_free",
     "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
 ]
@@ -196,6 +208,19 @@ def load(build: bool = True):
     L.etl_dec_bigquery_issues.argtypes = [vp, C.POINTER(BigQueryIssues)]
     L.etl_dec_bigquery_free.argtypes = [vp]
     L.etl_dec_bigquery_free.restype = None
+    L.etl_dec_ducklake_emit.argtypes = [vp, C.c_uint32, C.POINTER(C.c_char_p), C.c_uint32, C.c_int, C.POINTER(vp)]
+    L.etl_dec_ducklake_mutations.argtypes = [vp]
+    L.etl_dec_ducklake_mutations.restype = C.c_uint64
+    for f in ("etl_dec_ducklake_kinds", "etl_dec_ducklake_records"):
+        getattr(L, f).argtypes = [vp, C.c_int]
+        getattr(L, f).restype = C.c_void_p
+    L.etl_dec_ducklake_text.argtypes = [vp, C.c_uint32, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_uint64)]
+    L.etl_dec_ducklake_issues.argtypes = [vp, C.POINTER(DuckLakeIssues)]
+    L.etl_dec_ducklake_sub_batches.argtypes = [vp, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint64), C.c_int, C.POINTER(vp),
+                                               C.POINTER(C.c_uint64)]
+    L.etl_dec_ducklake_copy_fingerprint.argtypes = [vp, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint64)]
+    L.etl_dec_ducklake_free.argtypes = [vp]
+    L.etl_dec_ducklake_free.restype = None
     L.etl_dec_batch_device_stream.argtypes = [vp]
     L.etl_dec_batch_device_stream.restype = C.c_void_p
     L.etl_shim_materialise.argtypes = [vp, vp, vp, C.POINTER(vp)]
@@ -225,6 +250,11 @@ ARROW_CDC_COLUMNS = 0x200
 BQ_ISSUE_ARRAY_NULL = 1
 BQ_ISSUE_NUMERIC_SCALE = 2
 BQ_ISSUE_JSON_INTEGER = 3
+
+# etl_dec_ducklake_* (ETL_DL_*)
+DL_INSERT, DL_UPDATE, DL_UPDATE_PARTIAL, DL_REPLACE, DL_DELETE, DL_MF_ARRAY = 1, 2, 3, 4, 5, 0x80
+DL_TEXT_ROW, DL_TEXT_PREDICATE, DL_TEXT_ASSIGNMENTS = 0, 1, 2
+DL_REJECT_UPDATE_NO_IDENTITY, DL_REJECT_DELETE_NO_IDENTITY, DL_REJECT_DELETE_NO_OLD_ROW, DL_REJECT_PARTIAL_KEY_MISSING = 1, 2, 3, 4
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

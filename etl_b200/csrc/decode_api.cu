@@ -204,6 +204,7 @@ struct etl_dec_batch {
   bool copy = false;                     // COPY rows: the table and column classes they were decoded with
   uint32_t copy_table = 0;
   std::vector<uint8_t> copy_kinds;
+  std::vector<uint8_t> copy_pk;          // 1 = the stored column has a primary_key_ordinal_position
 };
 
 struct etl_dec_ctx {
@@ -1519,6 +1520,7 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
   S.n_events = nr;
   b->dev_stream = P.buf;
   b->copy = true; b->copy_table = table_id; b->copy_kinds = std::move(kinds);
+  for (uint32_t i = 0; i < n_cols; i++) b->copy_pk.push_back(t.cols[i].pk != -1 ? 1 : 0);
   *out = b;
   return ETL_OK;
 #undef CKB
@@ -1558,6 +1560,11 @@ int etl_dec_mem_info(etl_dec_ctx* ctx, uint64_t* free_bytes, uint64_t* total_byt
 bool etl_schema_pk_columns(const etl_dec_batch* b, uint32_t index, const uint8_t** pk) {
   if (!b || index >= b->schemas.size()) return false;
   *pk = b->schemas[index].pk.data();
+  return true;
+}
+bool etl_copy_batch_pk_columns(const etl_dec_batch* b, const uint8_t** pk) {
+  if (!b || !b->copy) return false;
+  *pk = b->copy_pk.data();
   return true;
 }
 bool etl_copy_batch_columns(const etl_dec_batch* b, uint32_t* table_id, const uint8_t** col_kind, uint32_t* n_cols) {

@@ -6,6 +6,7 @@
 //   * lowercase hex (bytes_to_hex, encoding.rs:162-172);
 //   * the Date32 range check (date_to_date32_days, encoding.rs:131-148);
 //   * the UUID wire order (rb_encode_value, encoding.rs:230-237).
+// The DuckLake emitter's variants sit next to the functions they vary: the fixed 6-digit time fraction and uppercase hex.
 #pragma once
 #include <stdint.h>
 
@@ -52,6 +53,22 @@ __device__ __forceinline__ uint32_t time_write(uint64_t secs, uint32_t nanos, ui
   for (uint32_t k = d; k > 0; k--) { out[8 + k] = (uint8_t)('0' + f % 10u); f /= 10u; }
   return 9u + d;
 }
+// chrono's "%H:%M:%S%.6f" (the DuckLake TIME / TIMESTAMP literals): always 6 fraction digits, truncated; a leap second
+// is second 60 as above.  15 bytes
+constexpr uint32_t kTime6Len = 15;
+__device__ __forceinline__ uint32_t time6_write(uint64_t secs, uint32_t nanos, uint8_t* out) {
+  uint32_t sec = (uint32_t)(secs % 60u);
+  if (nanos >= kNanos) { sec += 1u; nanos -= kNanos; }
+  put2((uint32_t)(secs / 3600u), out);
+  out[2] = ':';
+  put2((uint32_t)(secs / 60u % 60u), out + 3);
+  out[5] = ':';
+  put2(sec, out + 6);
+  out[8] = '.';
+  uint32_t f = nanos / 1000u;
+  for (uint32_t k = 6; k > 0; k--) { out[8 + k] = (uint8_t)('0' + f % 10u); f /= 10u; }
+  return kTime6Len;
+}
 
 // lowercase hex, two characters per byte
 __device__ __forceinline__ void hex_byte(uint8_t b, uint8_t* out) {
@@ -61,6 +78,12 @@ __device__ __forceinline__ void hex_byte(uint8_t b, uint8_t* out) {
 }
 __device__ __forceinline__ void hex_write(const uint8_t* src, uint32_t n, uint8_t* out) {
   for (uint32_t i = 0; i < n; i++) hex_byte(src[i], out + 2 * i);
+}
+// uppercase hex (DuckLake's from_hex literal, encode_hex in crates/etl-destinations/src/ducklake/encoding.rs)
+__device__ __forceinline__ void hex_byte_upper(uint8_t b, uint8_t* out) {
+  const uint32_t hi = b >> 4, lo = b & 15u;
+  out[0] = (uint8_t)(hi < 10u ? '0' + hi : 'A' - 10u + hi);
+  out[1] = (uint8_t)(lo < 10u ? '0' + lo : 'A' - 10u + lo);
 }
 
 // Date32 holds 1900-01-01 ..= 2299-12-31: days -25567 ..= 120529 from 1970-01-01

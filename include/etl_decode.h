@@ -635,6 +635,103 @@ const uint64_t* etl_dec_bigquery_row_records(const etl_bigquery_batch*, int host
 int etl_dec_bigquery_issues(const etl_bigquery_batch*, etl_bigquery_issues* out);
 void etl_dec_bigquery_free(etl_bigquery_batch*);
 
+/* ---------------------------------------------------------------- DuckLake emitter
+ * The row mutations of ONE replicated-schema version of a decoded batch, with the SQL-literal texts the DuckLake
+ * destination builds for them, built on the device, and the fingerprints of its retry-safe batch identity.  Replaces
+ * the host work of crates/etl-destinations/src/ducklake: write_events_inner (core.rs:715-836) with
+ * validate_ducklake_replica_identity (:237-258) and key_row_from_updated_partial_row (:266-359);
+ * cell_to_sql_literal_ref / table_row_to_sql_literal_ref (encoding.rs:28-272) behind delete_predicate_from_row
+ * (batches.rs:1099-1186), update_assignments_from_partial_row (:1189-1269), delete_predicate_from_copy_row (:1338-1371)
+ * and prepare_rows (encoding.rs:13-26); build_mutation_batch_identity / build_copy_batch_identity (batches.rs:1272-1336)
+ * over the chunks of prepare_mutation_table_batches (:594-622) after retain_mutations_after_sequence_key (:806-820).
+ * quoted_names: the version's n_cols column names exactly as pg_escape::quote_identifier prints them, copied verbatim
+ * (any other n_names, or a NULL name, is ETL_ERR_INVALID_ARG).
+ * Mutations, in record order, come from the records of the version in the valid prefix that carry ETL_RF_EVENT:
+ *   Insert → INSERT (row: the new image);
+ *   Update with an old image (Full or Key), Full new image → UPDATE (predicate: the old image; row: the new image);
+ *   Update with an old image, ETL_RF_NEW_PARTIAL → UPDATE_PARTIAL (predicate: the old image; assignments);
+ *   Update without an old image, Full new image → REPLACE (predicate: from the new row; row);
+ *   Update without an old image, partial → UPDATE_PARTIAL (predicate: the identity cells of the partial row; assignments);
+ *   Delete with an old image → DELETE (predicate).
+ * No mutation, and the record counts for first_rejected_record with its reason: an Update / Delete when the version has
+ * no identity columns (UPDATE_NO_IDENTITY / DELETE_NO_IDENTITY), a Delete without an old image (DELETE_NO_OLD_ROW), a
+ * partial Update without an old image that lacks an identity column (PARTIAL_KEY_MISSING).  A partial Update without
+ * any present column is still a mutation, reported in first_empty_partial_record (batches.rs:1207-1216 raises it when
+ * the batch is prepared).  mixed_versions: a truncate-free run of the batch holds DML of this version's table under
+ * another version; the reference then builds that table's run with the last version's schema (core.rs:737-740), so the
+ * sub-batches here are not the reference's.
+ * A COPY batch (rec_kind == NULL): schema_index must be 0, every row of the valid prefix is an INSERT, its predicate is
+ * delete_predicate_from_copy_row: the stored TableSchema's primary-key columns (empty when there are none), and
+ * etl_dec_ducklake_records gives the row index.
+ * Texts (etl_dec_ducklake_text; which = ETL_DL_TEXT_*, n_mutations + 1 u64 offsets; a kind without the text has an
+ * empty one):
+ *   row: "(" values joined by ", " ")";
+ *   predicate: the identity columns in schema order (a Full image's identity cells, a key image's cells in order),
+ *              "name = lit" or "name IS NULL", joined by " AND ";
+ *   assignments: the present columns ascending, "name = lit" (NULL: "name = NULL"), joined by ", ".
+ * Literals: NULL; TRUE / FALSE; I16 / I32 / U32 / I64 in decimal; String quote_literal(text); Numeric
+ * quote_literal(PgNumeric's Display); Uuid CAST('<lowercase hyphenated>' AS UUID); Json CAST(quote_literal(the
+ * ETL_ARROW_ALL_COLUMNS text) AS JSON); Bytes from_hex('<UPPERCASE hex>'); Date DATE 'Y-m-d' (chrono's signed years);
+ * Time TIME 'HH:MM:SS.ffffff' (always 6 digits, truncated; a leap second is second 60); Timestamp TIMESTAMP
+ * 'Y-m-d HH:MM:SS.ffffff'; TimestampTz TIMESTAMPTZ '…ffffff+00:00'; F64 Rust's Display (the shortest round-trip
+ * digits, positional, no ".0", "-0"), F32 the same of `f as f64`, NaN / ±Infinity CAST('NaN' | 'Infinity' |
+ * '-Infinity' AS DOUBLE) (F32: AS FLOAT); arrays "[" elements joined by ", " "]", NULL for a NULL element.
+ * quote_literal is pg_escape 0.1.1's (third-party, its source is not in the reference: parity unpinned): wrap in ',
+ * double every ' and \, prefix E when the text holds a \.  Rust's shortest float digits are taken to be those of
+ * Python's repr; no Rust toolchain checked that.
+ * kinds: ETL_DL_* | ETL_DL_MF_ARRAY when the mutation's row image holds an array cell (prepare_rows then takes the row
+ * texts as SqlLiterals instead of the appender).  The appender values are the ETL_ARROW_ALL_COLUMNS output of
+ * etl_dec_arrow_emit with row_kinds = inserts | updates.
+ * etl_dec_ducklake_sub_batches: with last_key = {commit_lsn, tx_ordinal}, the mutations whose (rec_commit_lsn,
+ * rec_tx_ordinal) is greater (a suffix); within each truncate-free run (a Truncate event record of any table starts a
+ * new one) they are cut into consecutive chunks of 16, and each chunk's fingerprint is FNV-1a 64 over what Rust's Hash
+ * feeds BatchIdHasher: "mutation", the table name (a str is its bytes then 0xff), then per mutation start_lsn and
+ * commit_lsn (u64, 8 bytes little-endian), the kind word ("insert", "delete", "update" for both UPDATE kinds, "replace")
+ * and INSERT: row; DELETE: predicate; UPDATE / REPLACE: predicate, row; UPDATE_PARTIAL: predicate, n_cols (usize),
+ * then per present column its index (usize) and its literal.  batch_id = "mutation:{first start_lsn:016x}:{last
+ * commit_lsn:016x}:{fingerprint:016x}".  The result lives in the batch until the next call or etl_dec_ducklake_free;
+ * ETL_ERR_INVALID_ARG for a COPY batch.
+ * etl_dec_ducklake_copy_fingerprint: "copy", the table name, then per row its predicate and its row text — one serial
+ * chain, computed on the host over the pinned copy: the batch must have been emitted with to_host (else, or for a
+ * streaming batch, ETL_ERR_INVALID_ARG).
+ * to_host: also copy records, kinds, text offsets and texts to a pinned buffer (host = 1 accessors); else those return
+ * NULL (etl_dec_ducklake_text: ETL_ERR_INVALID_ARG).  Scratch, beside the output: 4 B per (text, mutation, column + 1)
+ * + 4 B per mutation + 29 B per record of the batch, and with Json columns 12 B per (mutation, Json column, image) +
+ * 17 B per input byte of Json text.  schema_index out of range, or non-zero for a COPY batch, is ETL_ERR_INVALID_ARG; a
+ * single text of 4 GiB or more is ETL_ERR_INVALID_ARG; a Json value that does not parse again (the decode validated it)
+ * is ETL_ERR_INTERNAL. */
+enum { ETL_DL_INSERT = 1, ETL_DL_UPDATE = 2, ETL_DL_UPDATE_PARTIAL = 3, ETL_DL_REPLACE = 4, ETL_DL_DELETE = 5,
+       ETL_DL_MF_ARRAY = 0x80 /* the mutation's row image holds a Cell::Array: prepare_rows takes SqlLiterals */ };
+enum { ETL_DL_TEXT_ROW = 0, ETL_DL_TEXT_PREDICATE = 1, ETL_DL_TEXT_ASSIGNMENTS = 2 };
+enum { ETL_DL_REJECT_UPDATE_NO_IDENTITY = 1, ETL_DL_REJECT_DELETE_NO_IDENTITY = 2, ETL_DL_REJECT_DELETE_NO_OLD_ROW = 3,
+       ETL_DL_REJECT_PARTIAL_KEY_MISSING = 4 };
+typedef struct etl_ducklake_issues {
+  uint64_t first_rejected_record;      /* smallest batch-local record write_events_inner rejects; UINT64_MAX: none */
+  uint32_t rejected_reason;            /* ETL_DL_REJECT_* of that record (0: none) */
+  uint32_t mixed_versions;             /* non-zero: a truncate-free run holds this table's DML under another version */
+  uint64_t first_empty_partial_record; /* partial update with no present column; UINT64_MAX: none */
+} etl_ducklake_issues;
+typedef struct etl_dl_sub_batch {
+  uint64_t first_mutation;
+  uint32_t n_mutations;
+  uint32_t _pad;
+  uint64_t fingerprint;
+} etl_dl_sub_batch;
+typedef struct etl_ducklake_batch etl_ducklake_batch;
+int etl_dec_ducklake_emit(const etl_dec_batch*, uint32_t schema_index, const char* const* quoted_names, uint32_t n_names,
+                          int to_host, etl_ducklake_batch** out);
+uint64_t etl_dec_ducklake_mutations(const etl_ducklake_batch*);
+const uint8_t* etl_dec_ducklake_kinds(const etl_ducklake_batch*, int host);    /* ETL_DL_* | ETL_DL_MF_ARRAY */
+const uint64_t* etl_dec_ducklake_records(const etl_ducklake_batch*, int host); /* record (COPY: row) of each mutation */
+int etl_dec_ducklake_text(const etl_ducklake_batch*, uint32_t which, int host,
+                          const uint8_t** data, const uint64_t** offsets /* n_mutations + 1 */, uint64_t* bytes);
+int etl_dec_ducklake_issues(const etl_ducklake_batch*, etl_ducklake_issues* out);
+int etl_dec_ducklake_sub_batches(etl_ducklake_batch*, const uint8_t* table_name, uint32_t name_len,
+                                 const uint64_t* last_key /* NULL, or {commit_lsn, tx_ordinal} */, int host,
+                                 const etl_dl_sub_batch** out, uint64_t* n);
+int etl_dec_ducklake_copy_fingerprint(const etl_ducklake_batch*, const uint8_t* table_name, uint32_t name_len, uint64_t* out);
+void etl_dec_ducklake_free(etl_ducklake_batch*);
+
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
 const uint8_t* etl_dec_batch_device_stream(const etl_dec_batch*);
