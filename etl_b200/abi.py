@@ -77,6 +77,17 @@ class DlSubBatch(C.Structure):
     _fields_ = [("first_mutation", C.c_uint64), ("n_mutations", C.c_uint32), ("_pad", C.c_uint32), ("fingerprint", C.c_uint64)]
 
 
+class ParquetField(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("field_id", C.c_int32), ("element_field_id", C.c_int32), ("required", C.c_uint32),
+                ("_pad", C.c_uint32)]
+
+
+class ParquetMetrics(C.Structure):
+    _fields_ = [("field_id", C.c_int32), ("flags", C.c_uint32), ("num_values", C.c_uint64), ("null_count", C.c_uint64),
+                ("nan_count", C.c_uint64), ("compressed_bytes", C.c_uint64), ("uncompressed_bytes", C.c_uint64),
+                ("min", C.c_void_p), ("min_len", C.c_uint32), ("max", C.c_void_p), ("max_len", C.c_uint32)]
+
+
 class Planes(C.Structure):
     _fields_ = [("n_records", C.c_uint64), ("n_cells", C.c_uint64), ("heap_bytes", C.c_uint64),
                 ("rec_off", C.c_void_p), ("rec_kind", C.c_void_p), ("rec_flags", C.c_void_p), ("rec_rel", C.c_void_p),
@@ -116,7 +127,8 @@ EXPORTS = [
     "etl_dec_bigquery_row_offsets", "etl_dec_bigquery_row_records", "etl_dec_bigquery_issues", "etl_dec_bigquery_free",
     "etl_dec_ducklake_emit", "etl_dec_ducklake_mutations", "etl_dec_ducklake_kinds", "etl_dec_ducklake_records",
     "etl_dec_ducklake_text", "etl_dec_ducklake_issues", "etl_dec_ducklake_sub_batches", "etl_dec_ducklake_copy_fingerprint",
-    "etl_dec_ducklake_free",
+    "etl_dec_ducklake_free", "etl_dec_parquet_write", "etl_dec_parquet_size", "etl_dec_parquet_bytes", "etl_dec_parquet_metrics",
+    "etl_dec_parquet_required_null", "etl_dec_parquet_free",
     "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
 ]
@@ -221,6 +233,16 @@ def load(build: bool = True):
     L.etl_dec_ducklake_copy_fingerprint.argtypes = [vp, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint64)]
     L.etl_dec_ducklake_free.argtypes = [vp]
     L.etl_dec_ducklake_free.restype = None
+    L.etl_dec_parquet_write.argtypes = [vp, C.POINTER(ParquetField), C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int,
+                                        C.POINTER(vp)]
+    L.etl_dec_parquet_size.argtypes = [vp]
+    L.etl_dec_parquet_size.restype = C.c_uint64
+    L.etl_dec_parquet_bytes.argtypes = [vp, C.c_int]
+    L.etl_dec_parquet_bytes.restype = C.c_void_p
+    L.etl_dec_parquet_metrics.argtypes = [vp, C.c_uint32, C.POINTER(ParquetMetrics)]
+    L.etl_dec_parquet_required_null.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
+    L.etl_dec_parquet_free.argtypes = [vp]
+    L.etl_dec_parquet_free.restype = None
     L.etl_dec_batch_device_stream.argtypes = [vp]
     L.etl_dec_batch_device_stream.restype = C.c_void_p
     L.etl_shim_materialise.argtypes = [vp, vp, vp, C.POINTER(vp)]
@@ -255,6 +277,10 @@ BQ_ISSUE_JSON_INTEGER = 3
 DL_INSERT, DL_UPDATE, DL_UPDATE_PARTIAL, DL_REPLACE, DL_DELETE, DL_MF_ARRAY = 1, 2, 3, 4, 5, 0x80
 DL_TEXT_ROW, DL_TEXT_PREDICATE, DL_TEXT_ASSIGNMENTS = 0, 1, 2
 DL_REJECT_UPDATE_NO_IDENTITY, DL_REJECT_DELETE_NO_IDENTITY, DL_REJECT_DELETE_NO_OLD_ROW, DL_REJECT_PARTIAL_KEY_MISSING = 1, 2, 3, 4
+
+# etl_dec_parquet_write codecs (ETL_PQ_*) and etl_parquet_metrics.flags
+PQ_UNCOMPRESSED, PQ_SNAPPY = 0, 1
+PQ_HAS_MIN_MAX = 1
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

@@ -1,0 +1,334 @@
+// parquet_format.cuh — the byte-level pieces of the Parquet writer (parquet_write.cu) that a host harness can compile too
+// (tests/emul/host_parquet.cpp builds this same file with g++, so the CPU suite checks it against tests/parquet_ref.py):
+//   * a Thrift compact-protocol writer (Parquet's footer and page headers): fields in ascending id order, i32 / i64 as
+//     zigzag varints, binary as varint length + bytes, lists with the size in the header nibble below 15;
+//   * the data page header (PageHeader {type DATA_PAGE, uncompressed_page_size, compressed_page_size, data_page_header
+//     {num_values, encoding PLAIN, definition / repetition level encoding RLE}});
+//   * the RLE / bit-packed hybrid level encoder with the deterministic run rule of include/etl_decode.h: entries cut into
+//     groups of 8, a group is uniform when its present entries are equal, consecutive uniform groups of one value are one
+//     RLE run of their exact entry count, every other stretch is bit-packed runs of at most 63 groups;
+//   * the Snappy compressor of one fragment of at most 64 KiB: 4-byte hash match finder over a 4096-entry table,
+//     literal / copy-1 / copy-2 elements; copies never reach outside the fragment, so fragments compress independently
+//     and their element streams concatenate into one valid stream;
+//   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders.
+#pragma once
+#include <stdint.h>
+#include <string.h>
+
+#include <string>
+#include <vector>
+
+namespace etl_pq {
+
+// Parquet physical types / converted types / repetition / codecs / encodings (parquet.thrift)
+enum { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
+enum { CT_UTF8 = 0, CT_LIST = 3, CT_DATE = 6, CT_TIMESTAMP_MICROS = 10, CT_NONE = -1 };
+enum { REP_REQUIRED = 0, REP_OPTIONAL = 1, REP_REPEATED = 2 };
+enum { ENC_PLAIN = 0, ENC_RLE = 3 };
+constexpr uint32_t kPageRows = 20000;                 // a page ends after the row that brings it to this many rows
+constexpr uint64_t kPageBytes = 1ull << 20;           // … or to this many PLAIN value bytes
+constexpr uint64_t kRowGroupRows = 1ull << 20;
+constexpr uint32_t kFragment = 65536;                 // Snappy fragment
+constexpr uint32_t kSnappyHashBits = 12;
+constexpr uint32_t kStatMax = 64;                     // a longer byte-array min / max is not written
+constexpr uint32_t kPageHeaderMax = 48;               // 4 fields + a 4-field struct of i32 varints: at most 41 bytes
+
+__host__ __device__ inline uint32_t snappy_bound(uint32_t n) { return 32u + n + n / 6u; }
+// level section bound (4-byte length prefix, runs): every group costs at most w bytes + 1 header byte of its bit-packed
+// run, or 2 bytes as (part of) an RLE run; the constant covers one RLE header of up to 5 bytes
+__host__ __device__ inline uint64_t levels_bound(uint64_t n, uint32_t w) { return 14u + ((n + 7u) / 8u) * (w + 2u); }
+__host__ __device__ inline uint32_t bit_width(uint32_t max_level) { uint32_t w = 0; while (max_level >> w) w++; return w; }
+
+// ------------------------------------------------------------------------------------------------ Thrift compact
+__host__ __device__ inline uint32_t varint(uint64_t v, uint8_t* out) {
+  uint32_t n = 0;
+  while (v >= 0x80u) { if (out) out[n] = (uint8_t)(v | 0x80u); n++; v >>= 7; }
+  if (out) out[n] = (uint8_t)v;
+  return n + 1;
+}
+__host__ __device__ inline uint64_t zigzag(int64_t v) { return ((uint64_t)v << 1) ^ (uint64_t)(v >> 63); }
+
+enum { TT_TRUE = 1, TT_FALSE = 2, TT_I16 = 4, TT_I32 = 5, TT_I64 = 6, TT_BINARY = 8, TT_LIST = 9, TT_STRUCT = 12 };
+// out == nullptr counts only
+struct TWriter {
+  uint8_t* out; uint64_t n; int16_t last[8]; int depth;
+  __host__ __device__ explicit TWriter(uint8_t* o) : out(o), n(0), depth(0) { last[0] = 0; }
+  __host__ __device__ void byte(uint8_t b) { if (out) out[n] = b; n++; }
+  __host__ __device__ void var(uint64_t v) { n += varint(v, out ? out + n : nullptr); }
+  __host__ __device__ void field(int16_t id, uint8_t type) {
+    const int16_t d = id - last[depth];
+    if (d > 0 && d <= 15) byte((uint8_t)((d << 4) | type));
+    else { byte(type); var(zigzag(id)); }
+    last[depth] = id;
+  }
+  __host__ __device__ void i32(int16_t id, int32_t v) { field(id, TT_I32); var(zigzag(v)); }
+  __host__ __device__ void i64(int16_t id, int64_t v) { field(id, TT_I64); var(zigzag(v)); }
+  __host__ __device__ void boolean(int16_t id, bool v) { field(id, v ? TT_TRUE : TT_FALSE); }
+  __host__ __device__ void bin(int16_t id, const uint8_t* p, uint32_t len) {
+    field(id, TT_BINARY); var(len);
+    if (out && len) memcpy(out + n, p, len);
+    n += len;
+  }
+  __host__ __device__ void begin(int16_t id) { field(id, TT_STRUCT); last[++depth] = 0; }   // nested struct
+  __host__ __device__ void end() { byte(0); if (depth) depth--; }
+  __host__ __device__ void list(int16_t id, uint8_t elem_type, uint32_t size) {
+    field(id, TT_LIST);
+    if (size < 15) byte((uint8_t)((size << 4) | elem_type));
+    else { byte((uint8_t)(0xF0 | elem_type)); var(size); }
+  }
+  __host__ __device__ void list_struct_begin() { last[++depth] = 0; }   // one struct element of a list
+};
+
+// DATA_PAGE header; returns its length (at most kPageHeaderMax)
+__host__ __device__ inline uint32_t page_header(uint8_t* out, uint32_t usize, uint32_t csize, uint32_t num_values) {
+  TWriter w(out);
+  w.i32(1, 0);               // type DATA_PAGE
+  w.i32(2, (int32_t)usize);
+  w.i32(3, (int32_t)csize);
+  w.begin(5);                // data_page_header
+  w.i32(1, (int32_t)num_values);
+  w.i32(2, ENC_PLAIN);
+  w.i32(3, ENC_RLE);
+  w.i32(4, ENC_RLE);
+  w.end();
+  w.end();
+  return (uint32_t)w.n;
+}
+
+// ------------------------------------------------------------------------------------------------ levels
+// RLE / bit-packed hybrid of n level bytes (values < 2^w, w in 1..2), without the length prefix; returns the bytes
+// written.  PRECONDITION: lv is 8-byte aligned and 8 bytes past n are readable (whole groups are loaded at once).
+__host__ __device__ inline uint64_t levels_encode(const uint8_t* lv, uint64_t n, uint32_t w, uint8_t* out) {
+  const uint64_t ng = (n + 7) / 8;
+  uint64_t o = 0, g = 0;
+  // uniform value of group g, or -1
+  auto cls = [&](uint64_t k) -> int {
+    const uint32_t m = (uint32_t)(n - k * 8 < 8 ? n - k * 8 : 8);
+    const uint64_t x = reinterpret_cast<const uint64_t*>(lv)[k];
+    const uint64_t mask = m == 8 ? ~0ull : ((1ull << (8 * m)) - 1);
+    const uint64_t v = x & 0xFFu;
+    return ((x ^ (v * 0x0101010101010101ull)) & mask) == 0 ? (int)v : -1;
+  };
+  while (g < ng) {
+    const int c = cls(g);
+    if (c >= 0) {                                       // RLE run: every following uniform group of the same value
+      uint64_t h = g + 1;
+      while (h < ng && cls(h) == c) h++;
+      const uint64_t cnt = (h == ng ? n : h * 8) - g * 8;
+      o += varint(cnt << 1, out + o);
+      out[o++] = (uint8_t)c;
+      g = h;
+    } else {                                            // bit-packed: the stretch of non-uniform groups, 63 at most
+      uint64_t h = g + 1;
+      while (h < ng && h - g < 63 && cls(h) < 0) h++;
+      out[o++] = (uint8_t)(((h - g) << 1) | 1u);
+      for (uint64_t k = g; k < h; k++) {                // 8 entries → w bytes, LSB first
+        uint32_t acc = 0;
+        for (uint32_t j = 0; j < 8; j++) {
+          const uint64_t e = k * 8 + j;
+          acc |= (e < n ? (uint32_t)lv[e] : 0u) << (j * w);
+        }
+        for (uint32_t b = 0; b < w; b++) out[o++] = (uint8_t)(acc >> (8 * b));
+      }
+      g = h;
+    }
+  }
+  return o;
+}
+
+// ------------------------------------------------------------------------------------------------ Snappy
+__host__ __device__ inline uint32_t load32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
+__host__ __device__ inline uint32_t snappy_hash(uint32_t v) { return (v * 0x1e35a7bdu) >> (32 - kSnappyHashBits); }
+__host__ __device__ inline uint32_t snappy_literal(const uint8_t* src, uint32_t len, uint8_t* out) {
+  uint32_t o = 0;
+  const uint32_t l = len - 1;
+  if (l < 60) out[o++] = (uint8_t)(l << 2);
+  else {
+    const uint32_t nb = l < 0x100u ? 1 : l < 0x10000u ? 2 : l < 0x1000000u ? 3 : 4;
+    out[o++] = (uint8_t)((59 + nb) << 2);
+    for (uint32_t b = 0; b < nb; b++) out[o++] = (uint8_t)(l >> (8 * b));
+  }
+  memcpy(out + o, src, len);
+  return o + len;
+}
+__host__ __device__ inline uint32_t snappy_copy(uint32_t off, uint32_t len, uint8_t* out) {
+  uint32_t o = 0;
+  while (len > 0) {
+    // split as the reference compressor does: 64-byte copies, 60 when that would leave fewer than 4
+    const uint32_t take = len >= 68 ? 64 : len > 64 ? 60 : len;
+    if (take >= 4 && take <= 11 && off < 2048) {
+      out[o++] = (uint8_t)(1u | ((take - 4) << 2) | ((off >> 8) << 5));
+      out[o++] = (uint8_t)off;
+    } else {
+      out[o++] = (uint8_t)(2u | ((take - 1) << 2));
+      out[o++] = (uint8_t)off;
+      out[o++] = (uint8_t)(off >> 8);
+    }
+    len -= take;
+  }
+  return o;
+}
+// the elements of one fragment (n <= kFragment; no length preamble) into out (snappy_bound(n) bytes); table has
+// 1 << kSnappyHashBits entries of scratch.  Returns the bytes written.
+__host__ __device__ inline uint32_t snappy_fragment(const uint8_t* in, uint32_t n, uint8_t* out, uint16_t* table) {
+  uint32_t o = 0, lit = 0, ip = 0;
+  if (n >= 15) {
+    for (uint32_t k = 0; k < (1u << kSnappyHashBits); k++) table[k] = 0;
+    const uint32_t limit = n - 4;                        // a 4-byte load at ip stays inside the fragment
+    uint32_t skip = 32;
+    ip = 1;
+    while (ip <= limit) {
+      const uint32_t cur = load32(in + ip);
+      const uint32_t h = snappy_hash(cur);
+      const uint32_t cand = table[h];
+      table[h] = (uint16_t)ip;
+      if (cand < ip && load32(in + cand) == cur) {
+        uint32_t len = 4;
+        while (ip + len < n && in[cand + len] == in[ip + len]) len++;
+        if (ip > lit) o += snappy_literal(in + lit, ip - lit, out + o);
+        o += snappy_copy(ip - cand, len, out + o);
+        ip += len;
+        lit = ip;
+        skip = 32;
+        if (ip - 1 <= limit) table[snappy_hash(load32(in + ip - 1))] = (uint16_t)(ip - 1);
+      } else {
+        ip += skip >> 5;                                 // incompressible stretches are skipped faster and faster
+        skip++;
+      }
+    }
+  }
+  if (n > lit) o += snappy_literal(in + lit, n - lit, out + o);
+  return o;
+}
+
+// ------------------------------------------------------------------------------------------------ footer (host)
+struct Leaf {                       // one column of the file: a flat leaf, or a list and its element
+  std::string name;
+  int32_t field_id, element_field_id;
+  uint32_t ptype;                   // PT_*
+  int32_t converted;                // CT_* of the leaf (CT_NONE)
+  uint32_t logical;                 // 0 none, 1 STRING, 6 DATE, 7 TIME(µs, utc=false), 8 TIMESTAMP(µs), 14 UUID
+  bool utc;                         // TIMESTAMP: isAdjustedToUTC
+  bool required, is_list;
+};
+struct Chunk {
+  uint64_t offset, num_values, usize, csize, null_count;
+  bool has_minmax;
+  std::string min, max;
+};
+
+inline void schema_element(TWriter& w, const Leaf& L, bool element) {
+  w.list_struct_begin();
+  w.i32(1, (int32_t)L.ptype);
+  if (L.ptype == PT_FLBA) w.i32(2, 16);
+  w.i32(3, element ? REP_OPTIONAL : L.required ? REP_REQUIRED : REP_OPTIONAL);
+  const std::string& nm = element ? std::string("element") : L.name;
+  w.bin(4, (const uint8_t*)nm.data(), (uint32_t)nm.size());
+  if (L.converted != CT_NONE) w.i32(6, L.converted);
+  w.i32(9, element ? L.element_field_id : L.field_id);
+  if (L.logical) {
+    w.begin(10);
+    w.begin((int16_t)L.logical);
+    if (L.logical == 7 || L.logical == 8) {
+      w.boolean(1, L.logical == 8 && L.utc);
+      w.begin(2); w.begin(2); w.end(); w.end();    // unit: MICROS
+    }
+    w.end();
+    w.end();
+  }
+  w.end();
+}
+
+// FileMetaData {1 version, 2 schema, 3 num_rows, 4 row_groups, 6 created_by, 7 column_orders}; chunks row-group major
+inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::vector<uint64_t>& rg_rows,
+                                   const std::vector<Chunk>& chunks, uint32_t codec, const char* created_by) {
+  std::vector<uint8_t> buf;
+  for (int pass = 0; pass < 2; pass++) {
+    TWriter w(pass ? buf.data() : nullptr);
+    uint32_t n_elems = 1;
+    for (const Leaf& L : leaves) n_elems += L.is_list ? 3 : 1;
+    uint64_t num_rows = 0;
+    for (uint64_t r : rg_rows) num_rows += r;
+    w.i32(1, 1);
+    w.list(2, TT_STRUCT, n_elems);
+    w.list_struct_begin();
+    w.bin(4, (const uint8_t*)"schema", 6);
+    w.i32(5, (int32_t)leaves.size());
+    w.end();
+    for (const Leaf& L : leaves) {
+      if (!L.is_list) { schema_element(w, L, false); continue; }
+      w.list_struct_begin();                           // <rep> group name (LIST)
+      w.i32(3, L.required ? REP_REQUIRED : REP_OPTIONAL);
+      w.bin(4, (const uint8_t*)L.name.data(), (uint32_t)L.name.size());
+      w.i32(5, 1);
+      w.i32(6, CT_LIST);
+      w.i32(9, L.field_id);
+      w.begin(10); w.begin(3); w.end(); w.end();
+      w.end();
+      w.list_struct_begin();                           // repeated group list
+      w.i32(3, REP_REPEATED);
+      w.bin(4, (const uint8_t*)"list", 4);
+      w.i32(5, 1);
+      w.end();
+      schema_element(w, L, true);
+    }
+    w.i64(3, (int64_t)num_rows);
+    w.list(4, TT_STRUCT, (uint32_t)rg_rows.size());
+    for (size_t g = 0; g < rg_rows.size(); g++) {
+      w.list_struct_begin();
+      uint64_t tu = 0, tc = 0;
+      for (size_t l = 0; l < leaves.size(); l++) { tu += chunks[g * leaves.size() + l].usize; tc += chunks[g * leaves.size() + l].csize; }
+      w.list(1, TT_STRUCT, (uint32_t)leaves.size());
+      for (size_t l = 0; l < leaves.size(); l++) {
+        const Leaf& L = leaves[l];
+        const Chunk& C = chunks[g * leaves.size() + l];
+        w.list_struct_begin();
+        w.i64(2, (int64_t)C.offset);
+        w.begin(3);
+        w.i32(1, (int32_t)L.ptype);
+        const bool levels = L.is_list || !L.required;
+        w.list(2, TT_I32, levels ? 2 : 1);
+        w.var(zigzag(ENC_PLAIN));
+        if (levels) w.var(zigzag(ENC_RLE));
+        const std::string& leaf_name = L.name;
+        w.list(3, TT_BINARY, L.is_list ? 3 : 1);
+        w.var(leaf_name.size());
+        for (char ch : leaf_name) w.byte((uint8_t)ch);
+        if (L.is_list) { w.var(4); for (char ch : std::string("list")) w.byte((uint8_t)ch); w.var(7); for (char ch : std::string("element")) w.byte((uint8_t)ch); }
+        w.i32(4, (int32_t)codec);
+        w.i64(5, (int64_t)C.num_values);
+        w.i64(6, (int64_t)C.usize);
+        w.i64(7, (int64_t)C.csize);
+        w.i64(9, (int64_t)C.offset);
+        w.begin(12);
+        w.i64(3, (int64_t)C.null_count);
+        if (C.has_minmax) {
+          w.bin(5, (const uint8_t*)C.max.data(), (uint32_t)C.max.size());
+          w.bin(6, (const uint8_t*)C.min.data(), (uint32_t)C.min.size());
+        }
+        w.end();
+        w.end();
+        w.end();
+      }
+      w.i64(2, (int64_t)tu);
+      w.i64(3, (int64_t)rg_rows[g]);
+      w.i64(5, (int64_t)chunks[g * leaves.size()].offset);
+      w.i64(6, (int64_t)tc);
+      w.field(7, TT_I16); w.var(zigzag((int64_t)g));
+      w.end();
+    }
+    const uint32_t cb = (uint32_t)strlen(created_by);
+    w.bin(6, (const uint8_t*)created_by, cb);
+    w.list(7, TT_STRUCT, (uint32_t)leaves.size());
+    for (size_t l = 0; l < leaves.size(); l++) {       // ColumnOrder { 1: TypeDefinedOrder {} }
+      w.list_struct_begin();
+      w.begin(1); w.end();
+      w.end();
+    }
+    w.end();
+    if (!pass) buf.resize(w.n);
+  }
+  return buf;
+}
+
+}  // namespace etl_pq

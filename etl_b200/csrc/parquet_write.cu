@@ -1,0 +1,716 @@
+// parquet_write.cu — the Iceberg destination's Parquet data file, written on the device from an Arrow emit
+// (etl_dec_arrow_emit with ETL_ARROW_ALL_COLUMNS [| ETL_ARROW_CDC_COLUMNS]).  Replaces what iceberg-rust's ParquetWriter
+// does on the host for IcebergClient::write_record_batch (crates/etl-destinations/src/iceberg/client.rs:324-379):
+// encode every value again, build the levels, Snappy-compress the pages and compute the column statistics behind the
+// DataFile metrics.  The format rules are in include/etl_decode.h; the byte-level pieces are in parquet_format.cuh.
+//
+// Stages (one leaf per column: a flat column, or the element of a List column):
+//   1. Plan.  k_plan, a thread per (row, leaf): level entries (1, or max(1, list length)), non-null values and PLAIN
+//      value bytes (Boolean: bits) of the row, and a required column's first null row (atomicMin).  Three scans per leaf
+//      (emit_scan.cuh) give their prefix sums.  k_cut, a thread per (leaf, row group), walks the greedy page rule with a
+//      binary search over the value prefix sums; it runs twice, counting and then writing the pages.  SYNC 1 (the page
+//      counts, the totals and the required-null rows) sizes every buffer from bounds, so no later step waits for sizes.
+//   2. Encode.  k_encode, a CTA per page: the page's level bytes into scratch (thread per row), the RLE hybrid by one
+//      thread per section over whole 8-entry groups (one u64 load per group), then the non-null values compacted with a
+//      block scan over the validity: fixed width at rank * width, Booleans by atomicOr into a zeroed bit scratch, byte
+//      arrays as length + bytes with every value copied by the whole warp.  The same pass reduces the page's statistics
+//      (min / max as item indices, NaN count).  The payload goes to a slot sized by the bound of the page.
+//   3. Compress (ETL_PQ_SNAPPY).  k_snappy, a CTA per 64 KiB fragment slot of every page, runs the fragment compressor
+//      of parquet_format.cuh on one thread, its hash table in shared memory, into a slot of snappy_bound bytes; k_page writes the length preamble and the page header
+//      (its varint widths depend on the sizes) and the page's file bytes; a scan gives the file offsets; k_gather, a CTA
+//      per page, copies header + payload (+ fragments) into the file buffer, whose size is the sum of the bounds.
+//   4. Statistics.  k_chunk, a thread per (leaf, row group), folds the page candidates and sizes of its chunk, k_leaf the
+//      chunks of a leaf; both write the PLAIN bytes of min / max (−0.0 / +0.0 for a zero float, none above 64 bytes).
+//      SYNC 2 copies the chunk and leaf records back.
+//   5. Footer, on the host from those records (parquet_format.cuh), copied behind the pages with its length and "PAR1".
+//      SYNC 3 ends the call (and the copy to pinned host memory with to_host).
+// Scratch: per (row, leaf) 3 × 4 B lengths + 3 × 8 B prefix sums; per level entry 2 B (+ 64 B per page of the leaf);
+// Boolean leaves 1 bit per item (+ 4 B per page of the leaf); per page a bounded payload slot (the PLAIN value bytes + levels_bound per section) and,
+// with Snappy, a compressed slot of snappy_bound per fragment.
+// ptxas -v (sm_90a, CUDA 12.9): see the comment at the end of this file.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "etl_decode.h"
+#include "emit_scan.cuh"
+#include "parquet_format.cuh"
+
+namespace {
+
+using namespace etl_pq;
+
+struct LeafDev {
+  uint32_t atype;            // ETL_ARROW_* of the values (a List: of its child)
+  uint32_t is_list, required, max_def, max_rep, w;   // w: bit width of the definition level
+  uint32_t fixed;            // PLAIN width of a fixed-width value (Boolean: 0)
+  uint32_t off64;            // LargeBinary offsets
+  uint64_t bscr;             // Boolean: first word of the leaf's bit scratch
+  const uint8_t* lvalid;     // List: validity of the lists
+  const int32_t* loffs;      // List: offsets of the lists
+  const uint8_t* valid;      // validity of the values (the column, or the List's child)
+  const uint8_t* values;     // fixed width / Boolean bits
+  const void* offs;          // byte arrays
+  const uint8_t* data;
+};
+struct Page {
+  uint32_t leaf, chunk;
+  uint64_t lp;               // index of the page among the pages of its leaf (places its level and bit scratch)
+  uint64_t row0, row1;       // local rows [row0, row1)
+  uint64_t e0, e1;           // level entries (prefix of the leaf)
+  uint64_t it0, it1;         // items of the value column
+  uint64_t nn, vbytes, ubound, lscr;   // non-null values, PLAIN value bytes, payload bound, level scratch offset
+  uint64_t usize, csize;
+  uint32_t hlen, plen;       // page header / Snappy preamble bytes
+  uint64_t min_it, max_it, nan;
+  uint8_t hdr[kPageHeaderMax];
+  uint8_t pre[8];
+};
+struct ChunkOut {
+  uint64_t offset, num_values, usize, csize, null_count, nan_count;
+  uint32_t has, min_len, max_len, _pad;
+  uint8_t min[kStatMax], max[kStatMax];
+};
+constexpr uint64_t kNone = ~0ull;
+
+__device__ __forceinline__ bool bit(const uint8_t* v, uint64_t i) { return (v[i >> 3] >> (i & 7)) & 1u; }
+__device__ __forceinline__ uint64_t byte_off(const LeafDev& L, uint64_t i) {
+  return L.off64 ? (uint64_t)((const int64_t*)L.offs)[i] : (uint64_t)(uint32_t)((const int32_t*)L.offs)[i];
+}
+__device__ __forceinline__ bool is_bytes(const LeafDev& L) { return L.atype == ETL_ARROW_UTF8 || L.atype == ETL_ARROW_LARGE_BINARY; }
+__device__ __forceinline__ bool is_float(const LeafDev& L) { return L.atype == ETL_ARROW_FLOAT32 || L.atype == ETL_ARROW_FLOAT64; }
+__device__ __forceinline__ bool is_nan(const LeafDev& L, uint64_t i) {
+  if (L.atype == ETL_ARROW_FLOAT32) { const float f = ((const float*)L.values)[i]; return f != f; }
+  if (L.atype == ETL_ARROW_FLOAT64) { const double d = ((const double*)L.values)[i]; return d != d; }
+  return false;
+}
+// the type-defined order of two present, non-NaN items: < 0, 0, > 0
+__device__ int cmp_items(const LeafDev& L, uint64_t a, uint64_t b) {
+  switch (L.atype) {
+    case ETL_ARROW_BOOLEAN: return (int)bit(L.values, a) - (int)bit(L.values, b);
+    case ETL_ARROW_INT32: case ETL_ARROW_DATE32: { const int32_t x = ((const int32_t*)L.values)[a], y = ((const int32_t*)L.values)[b]; return x < y ? -1 : x > y; }
+    case ETL_ARROW_FLOAT32: { const float x = ((const float*)L.values)[a], y = ((const float*)L.values)[b]; return x < y ? -1 : x > y; }
+    case ETL_ARROW_FLOAT64: { const double x = ((const double*)L.values)[a], y = ((const double*)L.values)[b]; return x < y ? -1 : x > y; }
+    case ETL_ARROW_UUID: {
+      const uint8_t* x = L.values + a * 16; const uint8_t* y = L.values + b * 16;
+      for (int k = 0; k < 16; k++) if (x[k] != y[k]) return x[k] < y[k] ? -1 : 1;
+      return 0;
+    }
+    case ETL_ARROW_UTF8: case ETL_ARROW_LARGE_BINARY: {
+      const uint64_t a0 = byte_off(L, a), al = byte_off(L, a + 1) - a0, b0 = byte_off(L, b), bl = byte_off(L, b + 1) - b0;
+      const uint64_t m = al < bl ? al : bl;
+      for (uint64_t k = 0; k < m; k++) if (L.data[a0 + k] != L.data[b0 + k]) return L.data[a0 + k] < L.data[b0 + k] ? -1 : 1;
+      return al < bl ? -1 : al > bl;
+    }
+    default: { const int64_t x = ((const int64_t*)L.values)[a], y = ((const int64_t*)L.values)[b]; return x < y ? -1 : x > y; }
+  }
+}
+// fold candidate c into (mn, mx); kNone = no candidate
+__device__ __forceinline__ void fold(const LeafDev& L, uint64_t c_min, uint64_t c_max, uint64_t& mn, uint64_t& mx) {
+  if (c_min != kNone && (mn == kNone || cmp_items(L, c_min, mn) < 0)) mn = c_min;
+  if (c_max != kNone && (mx == kNone || cmp_items(L, c_max, mx) > 0)) mx = c_max;
+}
+
+// 1. per (row, leaf): entries, non-null values, PLAIN value bytes (Boolean: bits); a required column's first null
+__global__ void __launch_bounds__(256) k_plan(const LeafDev* leaves, uint64_t rb, uint64_t n, uint32_t* ent, uint32_t* nn,
+                                              uint32_t* vb, unsigned long long* req_null) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const LeafDev L = leaves[blockIdx.y];
+  const uint64_t r = rb + i, at = (uint64_t)blockIdx.y * (n + 1) + i;
+  uint64_t it0 = r, it1 = r + 1;
+  uint32_t e = 1;
+  if (L.is_list) {
+    const bool present = bit(L.lvalid, r);
+    if (!present && L.required) atomicMin(req_null + blockIdx.y, (unsigned long long)r);
+    it0 = present ? (uint64_t)L.loffs[r] : 0; it1 = present ? (uint64_t)L.loffs[r + 1] : 0;
+    e = it1 > it0 ? (uint32_t)(it1 - it0) : 1u;
+  } else if (L.required && !bit(L.valid, r)) atomicMin(req_null + blockIdx.y, (unsigned long long)r);
+  uint32_t c = 0;
+  uint64_t b = 0;
+  for (uint64_t k = it0; k < it1; k++) {
+    if (!bit(L.valid, k)) continue;
+    c++;
+    b += is_bytes(L) ? 4 + byte_off(L, k + 1) - byte_off(L, k) : L.fixed;
+  }
+  ent[at] = e; nn[at] = c; vb[at] = (uint32_t)(L.atype == ETL_ARROW_BOOLEAN ? c : b);
+}
+
+// 1b. a thread per (leaf, row group): greedy page cuts.  pages == nullptr: count into n_pages[chunk]
+__global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, uint64_t rb, uint64_t n, const uint64_t* E,
+                      const uint64_t* NN, const uint64_t* V, uint32_t* n_pages, const uint64_t* page_base, const uint64_t* leaf_page_base,
+                      const uint64_t* lscr_base,
+                      Page* pages) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_leaves * n_rg) return;
+  const uint32_t g = t / n_leaves, l = t % n_leaves;
+  const LeafDev L = leaves[l];
+  const uint64_t* e = E + (uint64_t)l * (n + 1); const uint64_t* nv = NN + (uint64_t)l * (n + 1); const uint64_t* v = V + (uint64_t)l * (n + 1);
+  const uint64_t g0 = (uint64_t)g * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
+  const bool boolean = L.atype == ETL_ARROW_BOOLEAN;
+  const uint64_t thresh = boolean ? 8 * kPageBytes - 7 : kPageBytes;   // ceil(bits / 8) >= 1 MiB
+  uint32_t np = 0;
+  for (uint64_t s = g0; s < g1; np++) {
+    uint64_t hi = min(g1 - 1, s + kPageRows - 1);
+    if (v[hi + 1] - v[s] >= thresh) {                    // the first row that brings the page to the byte limit
+      uint64_t lo = s;
+      while (lo < hi) { const uint64_t m = (lo + hi) / 2; if (v[m + 1] - v[s] >= thresh) hi = m; else lo = m + 1; }
+    }
+    const uint64_t end = hi + 1;
+    if (pages) {
+      Page& P = pages[page_base[t] + np];
+      P.leaf = l; P.chunk = t; P.lp = leaf_page_base[t] + np; P.row0 = s; P.row1 = end; P.e0 = e[s]; P.e1 = e[end];
+      P.it0 = L.is_list ? (uint64_t)L.loffs[rb + s] : rb + s;
+      P.it1 = L.is_list ? (uint64_t)L.loffs[rb + end] : rb + end;
+      P.nn = nv[end] - nv[s];
+      P.vbytes = boolean ? (P.nn + 7) / 8 : v[end] - v[s];
+      const uint64_t ne = P.e1 - P.e0;
+      P.ubound = P.vbytes + (L.max_def ? levels_bound(ne, L.w) : 0) + (L.max_rep ? levels_bound(ne, 1) : 0);
+      // level scratch: 8-aligned per page, two sections (rep | def)
+      P.lscr = lscr_base[l] + 2 * ((P.e0 + 7) & ~7ull) + 64ull * P.lp;
+      P.usize = P.csize = 0; P.hlen = P.plen = 0; P.min_it = P.max_it = kNone; P.nan = 0;
+    }
+    s = end;
+  }
+  if (!pages) n_pages[t] = np;
+}
+
+// 2. a CTA per page: levels, PLAIN values, statistics
+constexpr int kEncThreads = 256;
+__global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, Page* pages, uint64_t rb, const uint64_t* E,
+                                                        uint64_t n, uint8_t* lscr, uint8_t* uslot_base, const uint64_t* uslot,
+                                                        uint32_t* bool_scr) {
+  __shared__ uint64_t s_lv, s_warp[kEncThreads / 32], s_min[kEncThreads], s_max[kEncThreads];
+  __shared__ unsigned long long s_nan;
+  const uint32_t p = blockIdx.x;
+  Page& P = pages[p];
+  const LeafDev L = leaves[P.leaf];
+  const uint64_t ne = P.e1 - P.e0;
+  uint8_t* rep = lscr + P.lscr;
+  uint8_t* def = rep + ((ne + 15) & ~7ull);
+  const uint64_t* e = E + (uint64_t)P.leaf * (n + 1);
+  // levels of each row's entries
+  if (L.max_def) {
+    for (uint64_t i = P.row0 + threadIdx.x; i < P.row1; i += blockDim.x) {
+      const uint64_t r = rb + i, at = e[i] - P.e0;
+      if (!L.is_list) { def[at] = bit(L.valid, r); continue; }
+      if (!bit(L.lvalid, r)) { def[at] = 0; rep[at] = 0; continue; }
+      const uint64_t a = (uint64_t)L.loffs[r], b = (uint64_t)L.loffs[r + 1];
+      if (a == b) { def[at] = (uint8_t)(L.max_def - 2); rep[at] = 0; continue; }
+      for (uint64_t k = a; k < b; k++) {
+        def[at + k - a] = (uint8_t)(bit(L.valid, k) ? L.max_def : L.max_def - 1);
+        rep[at + k - a] = k == a ? 0 : 1;
+      }
+    }
+  }
+  __syncthreads();
+  uint8_t* out = uslot_base + uslot[p];
+  if (threadIdx.x == 0) {
+    uint64_t o = 0;
+    for (int s = 0; s < 2; s++) {
+      const bool is_rep = s == 0;
+      if (is_rep ? !L.max_rep : !L.max_def) continue;
+      const uint64_t len = levels_encode(is_rep ? rep : def, ne, is_rep ? 1u : L.w, out + o + 4);
+      for (int b = 0; b < 4; b++) out[o + b] = (uint8_t)(len >> (8 * b));
+      o += 4 + len;
+    }
+    s_lv = o;
+    s_nan = 0;
+  }
+  __syncthreads();
+  uint8_t* val = out + s_lv;
+  // values: compact the non-null items of [it0, it1) in order, tile by tile
+  uint64_t base = 0;          // values (Boolean / fixed) or bytes (byte arrays) before this tile
+  uint64_t mn = kNone, mx = kNone, nan = 0;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint64_t bw = L.bscr + (P.it0 >> 5) + P.lp;    // Boolean scratch: first word of this page
+  for (uint64_t t0 = P.it0; t0 < P.it1; t0 += blockDim.x) {
+    const uint64_t it = t0 + threadIdx.x;
+    const bool v = it < P.it1 && bit(L.valid, it);
+    uint64_t sz = 0, boff = 0, blen = 0;
+    if (v && is_bytes(L)) { boff = byte_off(L, it); blen = byte_off(L, it + 1) - boff; sz = 4 + blen; }
+    else if (v) sz = 1;
+    // block exclusive scan of sz
+    uint64_t x = sz;
+    for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += y; }
+    if (lane == 31) s_warp[wid] = x;
+    __syncthreads();
+    uint64_t before = 0, tile = 0;
+    for (int k = 0; k < kEncThreads / 32; k++) { if (k < wid) before += s_warp[k]; tile += s_warp[k]; }
+    const uint64_t rank = base + before + x - sz;
+    if (v) {
+      if (L.atype == ETL_ARROW_BOOLEAN) {
+        if (bit(L.values, it)) atomicOr(bool_scr + bw + (rank >> 5), 1u << (rank & 31));
+      } else if (!is_bytes(L)) {
+        for (uint32_t k = 0; k < L.fixed; k++) val[rank * L.fixed + k] = L.values[it * L.fixed + k];
+      } else {
+        for (int b = 0; b < 4; b++) val[rank + b] = (uint8_t)(blen >> (8 * b));
+      }
+      if (is_nan(L, it)) nan++;
+      else fold(L, it, it, mn, mx);
+    }
+    if (is_bytes(L)) {                                  // every value of the warp copied by the whole warp
+      unsigned todo = __ballot_sync(0xffffffffu, v && blen);
+      while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const uint64_t so = __shfl_sync(0xffffffffu, boff, src), sl = __shfl_sync(0xffffffffu, blen, src);
+        const uint64_t dst = __shfl_sync(0xffffffffu, rank, src) + 4;
+        for (uint64_t k = lane; k < sl; k += 32) val[dst + k] = L.data[so + k];
+      }
+    }
+    base += tile;
+    __syncthreads();
+  }
+  // statistics: block reduction of the candidates
+  s_min[threadIdx.x] = mn; s_max[threadIdx.x] = mx;
+  if (nan) atomicAdd(&s_nan, (unsigned long long)nan);
+  __syncthreads();
+  for (int d = kEncThreads / 2; d > 0; d >>= 1) {
+    if ((int)threadIdx.x < d) {
+      uint64_t a = s_min[threadIdx.x], b = s_max[threadIdx.x];
+      fold(L, s_min[threadIdx.x + d], s_max[threadIdx.x + d], a, b);
+      s_min[threadIdx.x] = a; s_max[threadIdx.x] = b;
+    }
+    __syncthreads();
+  }
+  if (L.atype == ETL_ARROW_BOOLEAN) {                   // the page's bits, from the word-aligned scratch
+    for (uint64_t k = threadIdx.x; k < P.vbytes; k += blockDim.x) val[k] = (uint8_t)(bool_scr[bw + (k >> 2)] >> (8 * (k & 3)));
+  }
+  if (threadIdx.x == 0) {
+    P.usize = s_lv + P.vbytes;
+    P.min_it = s_min[0]; P.max_it = s_max[0]; P.nan = s_nan;
+  }
+}
+
+// 3. a CTA per fragment slot of every page (fbase: exclusive scan of the slots per page); one thread compresses, with the
+// hash table in shared memory: the match finder is a chain of dependent table lookups, so their latency is the cost
+__global__ void __launch_bounds__(32) k_snappy(const Page* pages, uint32_t n_pages, const uint64_t* fbase, const uint8_t* uslot_base,
+                                               const uint64_t* uslot, uint8_t* cslot_base, const uint64_t* cslot, uint32_t* fsize) {
+  __shared__ uint16_t table[1u << kSnappyHashBits];
+  const uint64_t f = blockIdx.x;
+  if (threadIdx.x) return;
+  uint32_t lo = 0, hi = n_pages - 1;                      // the page: last fbase <= f
+  while (lo < hi) { const uint32_t m = (lo + hi + 1) / 2; if (fbase[m] <= f) lo = m; else hi = m - 1; }
+  const Page& P = pages[lo];
+  const uint64_t k = f - fbase[lo], off = k * kFragment;
+  if (off >= P.usize) { fsize[f] = 0; return; }
+  const uint32_t len = (uint32_t)(P.usize - off < kFragment ? P.usize - off : kFragment);
+  fsize[f] = snappy_fragment(uslot_base + uslot[lo] + off, len, cslot_base + cslot[lo] + 8 + k * snappy_bound(kFragment), table);
+}
+
+// a thread per page + 1: what the slot scans add up (0 payload bound, 1 compressed slot, 2 fragment slots); entry
+// n_pages is 0, so that the exclusive scan leaves the total there
+__global__ void k_fill(const Page* pages, uint32_t n_pages, int which, uint64_t* dst) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > n_pages) return;
+  if (p == n_pages) { dst[p] = 0; return; }
+  const uint64_t nf = pages[p].ubound ? (pages[p].ubound + kFragment - 1) / kFragment : 1;
+  dst[p] = which == 0 ? pages[p].ubound : which == 1 ? 8 + nf * snappy_bound(kFragment) : nf;
+}
+
+// a thread per page: compressed size, preamble, header, file bytes of the page
+__global__ void k_page(Page* pages, uint32_t n_pages, int snappy, const uint64_t* fbase, const uint32_t* fsize, uint64_t* fbytes) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_pages) return;
+  Page& P = pages[p];
+  if (snappy) {
+    P.plen = varint(P.usize, P.pre);
+    uint64_t c = P.plen;
+    for (uint64_t f = fbase[p]; f < fbase[p + 1]; f++) c += fsize[f];
+    P.csize = c;
+  } else P.csize = P.usize;
+  P.hlen = page_header(P.hdr, (uint32_t)P.usize, (uint32_t)P.csize, (uint32_t)(P.e1 - P.e0));
+  fbytes[p] = P.hlen + P.csize;
+}
+
+// a CTA per page: header, preamble and payload (or its fragments) at the page's file offset
+__global__ void __launch_bounds__(256) k_gather(const Page* pages, int snappy, const uint64_t* foff, const uint8_t* uslot_base,
+                                                const uint64_t* uslot, const uint8_t* cslot_base, const uint64_t* cslot,
+                                                const uint64_t* fbase, const uint32_t* fsize, uint8_t* file) {
+  const uint32_t p = blockIdx.x;
+  const Page& P = pages[p];
+  uint8_t* dst = file + 4 + foff[p];
+  for (uint32_t k = threadIdx.x; k < P.hlen; k += blockDim.x) dst[k] = P.hdr[k];
+  dst += P.hlen;
+  if (!snappy) {
+    const uint8_t* src = uslot_base + uslot[p];
+    for (uint64_t k = threadIdx.x; k < P.usize; k += blockDim.x) dst[k] = src[k];
+    return;
+  }
+  for (uint32_t k = threadIdx.x; k < P.plen; k += blockDim.x) dst[k] = P.pre[k];
+  dst += P.plen;
+  for (uint64_t f = fbase[p]; f < fbase[p + 1]; f++) {
+    const uint8_t* src = cslot_base + cslot[p] + 8 + (f - fbase[p]) * snappy_bound(kFragment);
+    for (uint32_t k = threadIdx.x; k < fsize[f]; k += blockDim.x) dst[k] = src[k];
+    dst += fsize[f];
+  }
+}
+
+// PLAIN statistic bytes of item it (a zero float minimum as −0.0, maximum as +0.0); false when longer than kStatMax
+__device__ bool stat_bytes(const LeafDev& L, uint64_t it, bool is_max, uint8_t* out, uint32_t* len) {
+  if (is_bytes(L)) {
+    const uint64_t a = byte_off(L, it), l = byte_off(L, it + 1) - a;
+    if (l > kStatMax) return false;
+    for (uint64_t k = 0; k < l; k++) out[k] = L.data[a + k];
+    *len = (uint32_t)l;
+    return true;
+  }
+  if (L.atype == ETL_ARROW_BOOLEAN) { out[0] = bit(L.values, it); *len = 1; return true; }
+  const uint32_t w = L.fixed;
+  for (uint32_t k = 0; k < w; k++) out[k] = L.values[it * w + k];
+  if (is_float(L)) {
+    const bool zero = w == 4 ? ((const float*)L.values)[it] == 0.0f : ((const double*)L.values)[it] == 0.0;
+    if (zero) out[w - 1] = is_max ? 0x00 : 0x80;        // the sign bit is the top bit of the last byte
+  }
+  *len = w;
+  return true;
+}
+__device__ void write_stats(const LeafDev& L, uint64_t mn, uint64_t mx, ChunkOut& C) {
+  C.has = 0; C.min_len = C.max_len = 0;
+  if (mn == kNone) return;
+  if (stat_bytes(L, mn, false, C.min, &C.min_len) && stat_bytes(L, mx, true, C.max, &C.max_len)) C.has = 1;
+  else C.min_len = C.max_len = 0;
+}
+
+// 4. a thread per chunk (row-group major): sizes, counts, statistics of its pages
+__global__ void k_chunk(const LeafDev* leaves, const Page* pages, const uint64_t* page_base, uint32_t n_chunks, const uint64_t* foff,
+                        ChunkOut* out) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  const Page& P0 = pages[page_base[c]];
+  const LeafDev L = leaves[P0.leaf];
+  ChunkOut C{};
+  C.offset = 4 + foff[page_base[c]];
+  uint64_t mn = kNone, mx = kNone;
+  for (uint64_t p = page_base[c]; p < page_base[c + 1]; p++) {
+    const Page& P = pages[p];
+    C.num_values += P.e1 - P.e0; C.null_count += (P.e1 - P.e0) - P.nn; C.nan_count += P.nan;
+    C.usize += P.hlen + P.usize; C.csize += P.hlen + P.csize;
+    fold(L, P.min_it, P.max_it, mn, mx);
+  }
+  write_stats(L, mn, mx, C);
+  out[c] = C;
+  // the candidates themselves, for the file-level fold
+  reinterpret_cast<uint64_t*>(out + n_chunks)[2 * c] = mn;
+  reinterpret_cast<uint64_t*>(out + n_chunks)[2 * c + 1] = mx;
+}
+// a thread per leaf: the file's statistics over its chunks
+__global__ void k_leaf(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, ChunkOut* chunks, ChunkOut* out) {
+  const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
+  if (l >= n_leaves) return;
+  const LeafDev L = leaves[l];
+  const uint32_t n_chunks = n_leaves * n_rg;
+  const uint64_t* cand = reinterpret_cast<const uint64_t*>(chunks + n_chunks);
+  ChunkOut C{};
+  uint64_t mn = kNone, mx = kNone;
+  for (uint32_t g = 0; g < n_rg; g++) {
+    const ChunkOut& K = chunks[g * n_leaves + l];
+    C.num_values += K.num_values; C.null_count += K.null_count; C.nan_count += K.nan_count;
+    C.usize += K.usize; C.csize += K.csize;
+    fold(L, cand[2 * (g * n_leaves + l)], cand[2 * (g * n_leaves + l) + 1], mn, mx);
+  }
+  write_stats(L, mn, mx, C);
+  out[l] = C;
+}
+
+uint32_t parquet_type(uint32_t at) {
+  switch (at) {
+    case ETL_ARROW_BOOLEAN: return PT_BOOLEAN;
+    case ETL_ARROW_INT32: case ETL_ARROW_DATE32: return PT_INT32;
+    case ETL_ARROW_FLOAT32: return PT_FLOAT;
+    case ETL_ARROW_FLOAT64: return PT_DOUBLE;
+    case ETL_ARROW_UTF8: case ETL_ARROW_LARGE_BINARY: return PT_BYTE_ARRAY;
+    case ETL_ARROW_UUID: return PT_FLBA;
+    default: return PT_INT64;
+  }
+}
+uint32_t plain_width(uint32_t at) {
+  switch (at) {
+    case ETL_ARROW_INT32: case ETL_ARROW_DATE32: case ETL_ARROW_FLOAT32: return 4;
+    case ETL_ARROW_INT64: case ETL_ARROW_FLOAT64: case ETL_ARROW_TIME64_US: case ETL_ARROW_TIMESTAMP_US: case ETL_ARROW_TIMESTAMPTZ_US: return 8;
+    case ETL_ARROW_UUID: return 16;
+    default: return 0;
+  }
+}
+
+}  // namespace
+
+struct etl_parquet_file {
+  uint8_t* dev = nullptr;
+  uint8_t* host = nullptr;
+  uint64_t size = 0;
+  std::vector<etl_parquet_metrics> metrics;
+  std::vector<std::string> stats;                   // min / max bytes of the metrics
+  uint32_t null_column = UINT32_MAX;
+  uint64_t null_row = UINT64_MAX;
+};
+
+extern "C" {
+
+int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fields, uint32_t n_fields, uint64_t row_begin,
+                          uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out) {
+  // a file needs at least one column (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS has none)
+  if (!a || !out || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
+  if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) || (codec != ETL_PQ_UNCOMPRESSED && codec != ETL_PQ_SNAPPY)) return ETL_ERR_INVALID_ARG;
+  std::vector<LeafDev> hl(n_fields);
+  std::vector<Leaf> meta(n_fields);
+  for (uint32_t c = 0; c < n_fields; c++) {
+    const etl_parquet_field& F = fields[c];
+    if (!F.name) return ETL_ERR_INVALID_ARG;
+    const size_t nl = strnlen(F.name, 1025);
+    if (nl == 0 || nl > 1024) return ETL_ERR_INVALID_ARG;
+    etl_arrow_column col;
+    if (etl_dec_arrow_column(a, c, 0, &col) != ETL_OK || col.arrow_type == ETL_ARROW_UNSUPPORTED) return ETL_ERR_INVALID_ARG;
+    LeafDev& L = hl[c];
+    memset(&L, 0, sizeof L);
+    L.is_list = col.arrow_type == ETL_ARROW_LIST;
+    L.required = F.required != 0;
+    if (L.is_list) {
+      etl_arrow_column kid;
+      uint64_t ne = 0;
+      if (etl_dec_arrow_list_child(a, c, 0, &kid, &ne) != ETL_OK) return ETL_ERR_INVALID_ARG;
+      L.lvalid = col.validity; L.loffs = (const int32_t*)col.offsets;
+      col = kid;
+    }
+    L.atype = col.arrow_type;
+    L.max_def = L.is_list ? (L.required ? 2 : 3) : (L.required ? 0 : 1);
+    L.max_rep = L.is_list ? 1 : 0;
+    L.w = bit_width(L.max_def);
+    L.fixed = plain_width(L.atype);
+    L.off64 = L.atype == ETL_ARROW_LARGE_BINARY;
+    L.valid = col.validity; L.values = (const uint8_t*)col.values; L.offs = col.offsets; L.data = col.data;
+    Leaf& M = meta[c];
+    M.name.assign(F.name, nl);
+    M.field_id = F.field_id; M.element_field_id = F.element_field_id;
+    M.ptype = parquet_type(L.atype);
+    M.required = L.required; M.is_list = L.is_list;
+    M.converted = CT_NONE; M.logical = 0; M.utc = false;
+    switch (L.atype) {
+      case ETL_ARROW_UTF8: M.converted = CT_UTF8; M.logical = 1; break;
+      case ETL_ARROW_DATE32: M.converted = CT_DATE; M.logical = 6; break;
+      case ETL_ARROW_TIME64_US: M.logical = 7; break;
+      case ETL_ARROW_TIMESTAMP_US: M.logical = 8; break;
+      case ETL_ARROW_TIMESTAMPTZ_US: M.logical = 8; M.utc = true; M.converted = CT_TIMESTAMP_MICROS; break;
+      case ETL_ARROW_UUID: M.logical = 14; break;
+      default: break;
+    }
+  }
+  const uint64_t n = row_end - row_begin;
+  const uint32_t nL = n_fields;
+  const uint32_t n_rg = (uint32_t)((n + kRowGroupRows - 1) / kRowGroupRows);
+  const uint32_t n_chunks = n_rg * nL;
+  const int snappy = codec == ETL_PQ_SNAPPY;
+  cudaStream_t st = cudaStreamPerThread;
+  etl_parquet_file* Fo = new etl_parquet_file();
+  std::vector<void*> pool;
+  auto dalloc = [&](uint64_t bytes) -> void* { void* p = nullptr; if (cudaMalloc(&p, bytes + 64) != cudaSuccess) return nullptr; pool.push_back(p); return p; };
+  auto fail = [&](int rc) { cudaGetLastError(); for (void* p : pool) cudaFree(p); if (Fo->dev) cudaFree(Fo->dev); if (Fo->host) cudaFreeHost(Fo->host); delete Fo; return rc; };
+#define CK(call) do { if ((call) != cudaSuccess) return fail(ETL_ERR_CUDA); } while (0)
+  // 1. plan
+  LeafDev* d_leaves = (LeafDev*)dalloc(sizeof(LeafDev) * (nL + 1));
+  const uint64_t nr1 = (uint64_t)nL * (n + 1);
+  uint32_t* d_len = (uint32_t*)dalloc(3 * nr1 * 4);
+  uint64_t* d_pre = (uint64_t*)dalloc(3 * nr1 * 8);
+  const uint32_t lb = (uint32_t)((n + 1023) / 1024);
+  unsigned long long* d_blk = (unsigned long long*)dalloc(3ull * nL * (lb + 1) * 8);
+  unsigned long long* d_tot = (unsigned long long*)dalloc(3ull * nL * 8);
+  unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull);
+  uint32_t* d_np = (uint32_t*)dalloc(n_chunks * 4ull);
+  if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np) return fail(ETL_ERR_ALLOC);
+  CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(d_req, 0xff, nL * 8ull, st));
+  CK(cudaMemsetAsync(d_tot, 0, 3ull * nL * 8, st));
+  CK(cudaMemsetAsync(d_pre, 0, 3 * nr1 * 8, st));
+  uint32_t* ent = d_len; uint32_t* nn = d_len + nr1; uint32_t* vb = d_len + 2 * nr1;
+  uint64_t* E = d_pre; uint64_t* NN = d_pre + nr1; uint64_t* V = d_pre + 2 * nr1;
+  if (n && nL) {
+    k_plan<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, row_begin, n, ent, nn, vb, d_req);
+    for (uint32_t s = 0; s < 3; s++)
+      for (uint32_t l = 0; l < nL; l++) {
+        const uint64_t at = (uint64_t)(s * nL + l);
+        uint32_t* lens = d_len + s * nr1 + (uint64_t)l * (n + 1);
+        unsigned long long* blk = d_blk + at * (lb + 1);
+        k_len_blocks<<<lb, 1024, 0, st>>>(lens, n, blk);
+        k_blk_scan64<<<1, 1024, 0, st>>>(blk, lb, d_tot + at);
+        k_offsets<uint64_t><<<lb, 1024, 0, st>>>(lens, n, blk, d_pre + s * nr1 + (uint64_t)l * (n + 1));
+      }
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr);
+  }
+  // SYNC 1: page counts, totals, required-column nulls
+  std::vector<uint32_t> np(n_chunks);
+  std::vector<unsigned long long> tot(3ull * nL), req(nL);
+  if (n_chunks) CK(cudaMemcpyAsync(np.data(), d_np, n_chunks * 4ull, cudaMemcpyDeviceToHost, st));
+  if (nL) {
+    CK(cudaMemcpyAsync(tot.data(), d_tot, 3ull * nL * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(req.data(), d_req, nL * 8ull, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  for (uint32_t l = 0; l < nL; l++)
+    if (req[l] != kNone) {                            // RecordBatch::try_new fails before anything is written
+      Fo->null_column = l; Fo->null_row = req[l];
+      for (void* p : pool) cudaFree(p);
+      *out = Fo;
+      return ETL_OK;
+    }
+  std::vector<uint64_t> page_base(n_chunks + 1, 0);
+  for (uint32_t c = 0; c < n_chunks; c++) page_base[c + 1] = page_base[c] + np[c];
+  const uint64_t P = page_base[n_chunks];
+  // bounds of every buffer from the totals
+  std::vector<uint64_t> pages_of(nL, 0), lscr_base(nL + 1, 0);
+  for (uint32_t c = 0; c < n_chunks; c++) pages_of[c % nL] += np[c];
+  uint64_t U = 0;
+  for (uint32_t l = 0; l < nL; l++) {
+    const uint64_t El = tot[l], NNl = tot[nL + l], Vl = tot[2 * nL + l], Pl = pages_of[l];
+    const uint64_t lev = 14 * Pl + (El / 8 + Pl) * (hl[l].w + 2);
+    U += (hl[l].atype == ETL_ARROW_BOOLEAN ? NNl / 8 + Pl : Vl) + (hl[l].max_def ? lev : 0) + (hl[l].max_rep ? 14 * Pl + (El / 8 + Pl) * 3 : 0);
+    (void)NNl;
+  }
+  // level scratch: per leaf 2 × (entries + 16 per page (alignment) + slack); page_base enters the per-page offset
+  // level scratch of a leaf: rep | def of each page, 8-aligned, at 2 * align8(e0) + 64 * (page index within the leaf)
+  for (uint32_t l = 0; l < nL; l++) lscr_base[l + 1] = lscr_base[l] + 2 * ((tot[l] + 7) & ~7ull) + 64 * (pages_of[l] + 1) + 64;
+  std::vector<uint64_t> leaf_page_base(n_chunks + 1, 0);   // pages of the chunk's leaf in the row groups before it
+  for (uint32_t c = nL; c < n_chunks; c++) leaf_page_base[c] = leaf_page_base[c - nL] + np[c - nL];
+  const uint64_t n_frag_bound = snappy ? U / kFragment + P + 1 : 0;
+  const uint64_t C_bound = snappy ? 8 * P + n_frag_bound * snappy_bound(kFragment) : 0;
+  // bit scratch: page lp of a Boolean leaf starts at word bscr + it0 / 32 + lp
+  uint64_t bool_words = 0;
+  for (uint32_t l = 0; l < nL; l++)
+    if (hl[l].atype == ETL_ARROW_BOOLEAN) {
+      etl_arrow_column col; uint64_t ne = 0;
+      if (hl[l].is_list) etl_dec_arrow_list_child(a, l, 0, &col, &ne); else ne = etl_dec_arrow_rows(a);
+      hl[l].bscr = bool_words;
+      bool_words += ne / 32 + pages_of[l] + 2;
+    }
+  // footer bound: every size at its widest varint, every statistic at its longest
+  std::vector<uint64_t> rg_rows(n_rg);
+  for (uint32_t g = 0; g < n_rg; g++) rg_rows[g] = std::min<uint64_t>(kRowGroupRows, n - (uint64_t)g * kRowGroupRows);
+  std::vector<Chunk> wide(n_chunks);
+  for (Chunk& k : wide) { k.offset = k.num_values = k.usize = k.csize = k.null_count = 1ull << 62; k.has_minmax = true; k.min.assign(kStatMax, 'x'); k.max.assign(kStatMax, 'x'); }
+  const char* created_by = "etl-b200 parquet writer";
+  const uint64_t footer_bound = footer(meta, rg_rows, wide, codec, created_by).size() + 8;
+  const uint64_t data_bound = 4 + P * kPageHeaderMax + (snappy ? C_bound : U);
+  Page* d_pages = (Page*)dalloc(sizeof(Page) * (P + 1));
+  uint64_t* d_pbase = (uint64_t*)dalloc(16 * (n_chunks + 1ull));   // page_base | leaf_page_base
+  uint64_t* d_lbase = (uint64_t*)dalloc(8 * (nL + 1ull));
+  uint8_t* d_lscr = (uint8_t*)dalloc(lscr_base[nL] + 16);
+  uint64_t* d_scan = (uint64_t*)dalloc(8 * 4 * (P + 1));   // uslot | cslot | fbase | file offsets, P + 1 each
+  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 4);
+  uint8_t* d_u = (uint8_t*)dalloc(U + 16);
+  uint32_t* d_bool = (uint32_t*)dalloc(bool_words * 4 + 8);
+  uint8_t* d_c = snappy ? (uint8_t*)dalloc(C_bound + 16) : nullptr;
+  uint32_t* d_fsz = snappy ? (uint32_t*)dalloc(n_frag_bound * 4 + 4) : nullptr;
+  ChunkOut* d_cout = (ChunkOut*)dalloc(sizeof(ChunkOut) * (n_chunks + nL) + 16ull * n_chunks);
+  ChunkOut* d_lout = d_cout ? (ChunkOut*)((uint8_t*)d_cout + sizeof(ChunkOut) * n_chunks + 16ull * n_chunks) : nullptr;
+  if (!d_pages || !d_pbase || !d_lbase || !d_lscr || !d_scan || !d_stot || !d_u || !d_bool || !d_cout || (snappy && (!d_c || !d_fsz)))
+    return fail(ETL_ERR_ALLOC);
+  if (cudaMalloc(&Fo->dev, data_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
+  uint64_t* uslot = d_scan; uint64_t* cslot = d_scan + (P + 1); uint64_t* fbase = d_scan + 2 * (P + 1); uint64_t* foff = d_scan + 3 * (P + 1);
+  CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_pbase, page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_pbase + n_chunks + 1, leaf_page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_lbase, lscr_base.data(), 8 * (nL + 1ull), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(Fo->dev, "PAR1", 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(d_bool, 0, bool_words * 4 + 8, st));
+  CK(cudaMemsetAsync(d_lscr, 0, lscr_base[nL] + 16, st));
+  if (P) {
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages);
+    // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
+    auto fill_scan = [&](int which, uint64_t* dst) {
+      k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, dst);
+      k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)dst, (uint32_t)(P + 1), d_stot + which);
+    };
+    fill_scan(0, uslot);
+    k_encode<<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, E, n, d_lscr, d_u, uslot, d_bool);
+    if (snappy) {
+      fill_scan(1, cslot);
+      fill_scan(2, fbase);
+      k_snappy<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz);
+    }
+    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, snappy, fbase, d_fsz, foff);
+    CK(cudaMemsetAsync(foff + P, 0, 8, st));
+    k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
+    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, snappy, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
+    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout);
+  }
+  if (nL) k_leaf<<<(nL + 63) / 64, 64, 0, st>>>(d_leaves, nL, P ? n_rg : 0, d_cout, d_lout);
+  // SYNC 2: chunk and leaf records
+  std::vector<ChunkOut> hc(n_chunks), hlo(nL);
+  unsigned long long data_end = 0;
+  if (P) {
+    CK(cudaMemcpyAsync(hc.data(), d_cout, sizeof(ChunkOut) * n_chunks, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&data_end, d_stot + 3, 8, cudaMemcpyDeviceToHost, st));
+  }
+  if (nL) CK(cudaMemcpyAsync(hlo.data(), d_lout, sizeof(ChunkOut) * nL, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
+  // 5. footer
+  std::vector<Chunk> chunks(n_chunks);
+  for (uint32_t c = 0; c < n_chunks; c++) {
+    const ChunkOut& K = hc[c];
+    chunks[c] = Chunk{K.offset, K.num_values, K.usize, K.csize, K.null_count, K.has != 0,
+                      std::string((const char*)K.min, K.min_len), std::string((const char*)K.max, K.max_len)};
+  }
+  std::vector<uint8_t> foot = footer(meta, rg_rows, chunks, codec, created_by);
+  const uint32_t flen = (uint32_t)foot.size();
+  for (int b = 0; b < 4; b++) foot.push_back((uint8_t)(flen >> (8 * b)));
+  for (char ch : std::string("PAR1")) foot.push_back((uint8_t)ch);
+  Fo->size = 4 + data_end + foot.size();
+  CK(cudaMemcpyAsync(Fo->dev + 4 + data_end, foot.data(), foot.size(), cudaMemcpyHostToDevice, st));
+  if (to_host) {
+    if (cudaHostAlloc((void**)&Fo->host, Fo->size, cudaHostAllocDefault) != cudaSuccess) { Fo->host = nullptr; return fail(ETL_ERR_ALLOC); }
+    CK(cudaMemcpyAsync(Fo->host, Fo->dev, Fo->size, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));                      // SYNC 3 (the footer's host buffer is read by the copy)
+  Fo->metrics.resize(nL);
+  Fo->stats.resize(2 * nL);
+  for (uint32_t l = 0; l < nL; l++) {
+    const ChunkOut& K = hlo[l];
+    etl_parquet_metrics& M = Fo->metrics[l];
+    memset(&M, 0, sizeof M);
+    M.field_id = hl[l].is_list ? fields[l].element_field_id : fields[l].field_id;
+    M.flags = K.has ? ETL_PQ_HAS_MIN_MAX : 0;
+    M.num_values = K.num_values; M.null_count = K.null_count; M.nan_count = K.nan_count;
+    M.compressed_bytes = K.csize; M.uncompressed_bytes = K.usize;
+    if (K.has) {
+      Fo->stats[2 * l].assign((const char*)K.min, K.min_len);
+      Fo->stats[2 * l + 1].assign((const char*)K.max, K.max_len);
+      M.min = (const uint8_t*)Fo->stats[2 * l].data(); M.min_len = K.min_len;
+      M.max = (const uint8_t*)Fo->stats[2 * l + 1].data(); M.max_len = K.max_len;
+    }
+  }
+  for (void* p : pool) cudaFree(p);
+  *out = Fo;
+  return ETL_OK;
+#undef CK
+}
+uint64_t etl_dec_parquet_size(const etl_parquet_file* f) { return f ? f->size : 0; }
+const uint8_t* etl_dec_parquet_bytes(const etl_parquet_file* f, int host) { return f ? (host ? f->host : f->dev) : nullptr; }
+int etl_dec_parquet_metrics(const etl_parquet_file* f, uint32_t leaf, etl_parquet_metrics* out) {
+  if (!f || !out || leaf >= f->metrics.size()) return ETL_ERR_INVALID_ARG;
+  *out = f->metrics[leaf];
+  return ETL_OK;
+}
+int etl_dec_parquet_required_null(const etl_parquet_file* f, uint32_t* column, uint64_t* row) {
+  if (!f) return ETL_ERR_INVALID_ARG;
+  if (column) *column = f->null_column;
+  if (row) *row = f->null_row;
+  return ETL_OK;
+}
+void etl_dec_parquet_free(etl_parquet_file* f) {
+  if (!f) return;
+  if (f->dev) cudaFree(f->dev);
+  if (f->host) cudaFreeHost(f->host);
+  delete f;
+}
+
+}  // extern "C"
+
+// ptxas -v, sm_90a, CUDA 12.9 (registers / shared memory / stack):
+//   k_plan 32 / 0 / 0      k_cut 54 / 0 / 0       k_encode 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 12 / 0 / 0
+//   k_snappy 50 / 8192 B / 0                      k_page 30 / 0 / 40 B (the header bytes)   k_gather 23 / 0 / 0
+//   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)
+//   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan64 32 / 8192 B, k_offsets<uint64_t> 18 / 8192 B

@@ -732,6 +732,90 @@ int etl_dec_ducklake_sub_batches(etl_ducklake_batch*, const uint8_t* table_name,
 int etl_dec_ducklake_copy_fingerprint(const etl_ducklake_batch*, const uint8_t* table_name, uint32_t name_len, uint64_t* out);
 void etl_dec_ducklake_free(etl_ducklake_batch*);
 
+/* ---------------------------------------------------------------- Iceberg Parquet writer
+ * Rows [row_begin, row_end) of an Arrow emit (etl_dec_arrow_emit with ETL_ARROW_ALL_COLUMNS, usually with
+ * ETL_ARROW_CDC_COLUMNS) as one complete Parquet data file built on the device, plus the per-column metrics of the
+ * Iceberg DataFile.  Replaces what iceberg-rust's ParquetWriter does on the host in IcebergClient::write_record_batch
+ * (crates/etl-destinations/src/iceberg/client.rs:324-379, WriterProperties with Compression::SNAPPY): encode the values,
+ * build the levels, compress the pages, compute the column statistics behind column_sizes, value_counts,
+ * null_value_counts, nan_value_counts and lower_bounds / upper_bounds.  The shim keeps the control path: the table's
+ * FileIO, the catalog transaction, file naming and the metrics mode (truncate(16) by default).
+ * fields: one per emitted column, in order (n_fields == etl_dec_arrow_cols).  ETL_ERR_INVALID_ARG, before any launch:
+ * another n_fields or none (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS), an ETL_ARROW_UNSUPPORTED
+ * column (the emit lacked ETL_ARROW_ALL_COLUMNS), row_begin > row_end or row_end > etl_dec_arrow_rows, an unknown
+ * codec, a NULL or empty name or one longer than 1 KiB.
+ * A null in a required column (a null list of a required List column, or a null value) is data: ETL_OK with size 0 and
+ * no bytes, and etl_dec_parquet_required_null gives the smallest such column and its first null row (emit row numbers)
+ * — RecordBatch::try_new in rows_to_record_batch fails there before anything is written (a ConversionError in the shim).
+ * The file (parity with arrow-rs bytes and defaults is not a goal: its writer adds a dictionary, a page index and an
+ * ARROW:schema key; Iceberg readers resolve columns by field id and Parquet type):
+ *   layout: "PAR1", the column chunks (row-group major, column minor, pages in row order), the footer, its 4-byte LE
+ *           length, "PAR1".  Row groups of at most 1 048 576 rows in row order; zero rows: no row group.
+ *   pages: data page V1, no dictionary, no CRC, no page statistics; whole rows; a page ends after the first row that
+ *          brings it to 20 000 rows or to >= 1 MiB of PLAIN value bytes (Boolean: ceil(values / 8)), and at the row
+ *          group's end.
+ *   values: PLAIN, non-null only: Boolean bit-packed LSB first, INT32 / INT64 / FLOAT / DOUBLE little-endian,
+ *           BYTE_ARRAY 4-byte LE length + bytes, FIXED_LEN_BYTE_ARRAY(16) raw.
+ *   levels: only when the max level > 0, each section with a 4-byte LE length, repetition before definition; RLE /
+ *           bit-packed hybrid of bit width = bits of the max level, runs cut deterministically: entries in groups of 8,
+ *           a group is uniform when its (present) entries are equal; consecutive uniform groups of one value are one
+ *           RLE run of their exact entry count; each maximal stretch of other groups is bit-packed runs of at most 63
+ *           groups, the last group zero-padded.
+ *   types: Bool BOOLEAN, Int32 INT32, Int64 INT64, Float32 FLOAT, Float64 DOUBLE, Utf8 BYTE_ARRAY STRING (UTF8),
+ *          LargeBinary BYTE_ARRAY, Date32 INT32 DATE (DATE), Time64 µs INT64 TIME(MICROS, utc=false), Timestamp µs
+ *          INT64 TIMESTAMP(MICROS, utc=false), Timestamptz µs INT64 TIMESTAMP(MICROS, utc=true) (TIMESTAMP_MICROS),
+ *          Uuid FIXED_LEN_BYTE_ARRAY(16) UUID.  Every element carries its field id.
+ *   lists: <rep> group name (LIST) { repeated group list { optional <leaf> element } }, field_id on the outer group,
+ *          element_field_id on element (always optional: NestedField::list_element(…, false), iceberg/schema.rs:67-75);
+ *          max definition level 3 (optional list) or 2 (required), max repetition level 1.
+ *   codec: ETL_PQ_SNAPPY compresses each page's levels + values as one Snappy stream: the varint length, then the
+ *          elements of independent 64 KiB fragments (no copy crosses a fragment).  Page headers are not compressed.
+ *   statistics: per column chunk null_count, max_value, min_value in the type's order (signed ints / dates / times,
+ *          unsigned bytewise BYTE_ARRAY / UUID, false < true), NaN excluded, a zero minimum written as -0.0 and a zero
+ *          maximum as +0.0; none when the chunk has no non-NaN value or a byte-array min / max is longer than 64 bytes.
+ *          column_orders: TypeDefinedOrder for every leaf.
+ *   footer: Thrift compact, ascending field ids: FileMetaData {version 1, schema, num_rows, row_groups, created_by,
+ *          column_orders}, SchemaElement {type, type_length, repetition_type, name, num_children, converted_type,
+ *          field_id, logicalType}, RowGroup {columns, total_byte_size, num_rows, file_offset, total_compressed_size,
+ *          ordinal}, ColumnChunk {file_offset, meta_data}, ColumnMetaData {type, encodings (PLAIN, + RLE with levels),
+ *          path_in_schema, codec, num_values, total_uncompressed_size, total_compressed_size, data_page_offset,
+ *          statistics}.
+ * Metrics: one record per leaf (a List column's leaf is its element), over every row group of the file; min / max are
+ * the PLAIN statistic bytes, which equal Iceberg's single-value serialization of these types (before truncation).
+ * to_host: also copy the file to pinned host memory (etl_dec_parquet_bytes(f, 1); else NULL).  Scratch, beside the
+ * file: 36 B per (row, column), 2 B per level entry + 64 B per page, 1 bit per Boolean value, a payload slot per page (values +
+ * level bound) and with Snappy a compressed slot per 64 KiB of payload. */
+enum { ETL_PQ_UNCOMPRESSED = 0, ETL_PQ_SNAPPY = 1 };
+#define ETL_PQ_HAS_MIN_MAX 1u   /* etl_parquet_metrics.flags: min / max are set */
+typedef struct etl_parquet_field {
+  const char* name;           /* UTF-8 column name, written verbatim into the Parquet schema */
+  int32_t field_id;           /* Iceberg field id of the column */
+  int32_t element_field_id;   /* ETL_ARROW_LIST columns: Iceberg field id of the list element; ignored otherwise */
+  uint32_t required;          /* 1: REQUIRED (ColumnSchema nullable == false; both CDC columns), 0: OPTIONAL */
+  uint32_t _pad;
+} etl_parquet_field;
+typedef struct etl_parquet_metrics {   /* one per leaf (= per column; a List column's leaf is its element) */
+  int32_t field_id;           /* the leaf's id: field_id, or element_field_id for a List */
+  uint32_t flags;             /* ETL_PQ_HAS_MIN_MAX */
+  uint64_t num_values;        /* level entries (Parquet num_values), summed over row groups */
+  uint64_t null_count;        /* entries whose definition level < max */
+  uint64_t nan_count;         /* Float / Double leaves only */
+  uint64_t compressed_bytes;  /* column-chunk bytes including page headers, summed over row groups */
+  uint64_t uncompressed_bytes;
+  const uint8_t* min; uint32_t min_len;   /* host memory, PLAIN-encoded statistic bytes, valid until free */
+  const uint8_t* max; uint32_t max_len;
+} etl_parquet_metrics;
+typedef struct etl_parquet_file etl_parquet_file;
+int etl_dec_parquet_write(const etl_arrow_batch*, const etl_parquet_field* fields, uint32_t n_fields,
+                          uint64_t row_begin, uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out);
+uint64_t etl_dec_parquet_size(const etl_parquet_file*);
+const uint8_t* etl_dec_parquet_bytes(const etl_parquet_file*, int host);   /* the whole file, "PAR1" … "PAR1" */
+int etl_dec_parquet_metrics(const etl_parquet_file*, uint32_t leaf, etl_parquet_metrics* out);
+/* arrow-rs rejects a RecordBatch with a null in a non-nullable field: the smallest such column and its first null row
+ * (UINT32_MAX / UINT64_MAX when there is none); no file */
+int etl_dec_parquet_required_null(const etl_parquet_file*, uint32_t* column, uint64_t* row);
+void etl_dec_parquet_free(etl_parquet_file*);
+
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
 const uint8_t* etl_dec_batch_device_stream(const etl_dec_batch*);

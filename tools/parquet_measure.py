@@ -1,0 +1,169 @@
+#!/usr/bin/env python
+"""Time the Iceberg Parquet writer (etl_dec_parquet_write) on resident Arrow emits, against pyarrow's CPU writer.
+
+  python tools/parquet_measure.py [--copy-rows 1000000] [--c3-scale 1] [--c4-scale 0.1] [--reps 7] [--warmup 2]
+
+Workloads: bench.py's 10-column COPY table, C3 (one schema version) and C4 (every schema version: times and sizes are
+sums over the versions), each emitted once with 7 | ETL_ARROW_ALL_COLUMNS | ETL_ARROW_CDC_COLUMNS and kept in HBM.
+Every time is median / min / max over the repetitions of wall time around the call (the call syncs before it returns),
+to_host 0:
+  * write_ms_uncompressed / write_ms_snappy: the whole call, file in HBM;
+  * snappy_GBps: page payload bytes before compression / the median Snappy call;
+  * file_bytes_* and the pyarrow baseline: pyarrow.parquet.write_table(compression="snappy") with its defaults
+    (dictionary encoding on) over the same columns on the host, into memory — its time and file size show what the
+    device writer's missing dictionary costs in bytes.
+Prints the card name and power limit in the same run.
+"""
+import argparse
+import ctypes as C
+import io
+import json
+import os
+import sys
+import time
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+sys.path.insert(0, ROOT)
+sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import numpy as np  # noqa: E402
+import pyarrow as pa  # noqa: E402
+import pyarrow.parquet as pq  # noqa: E402
+import torch  # noqa: E402
+
+import parquet_ref as R  # noqa: E402
+from arrow_emit_measure import bench_copy_table, card, timed  # noqa: E402
+from etl_b200 import abi, decoder, workloads as wl  # noqa: E402
+from rowbinary_measure import sum_stats  # noqa: E402
+from parquet_io import emit_columns, fields_for, pq_write  # noqa: E402
+
+KINDS = 7 | abi.ARROW_ALL_COLUMNS | abi.ARROW_CDC_COLUMNS
+PA_TYPE = {R.BOOLEAN: pa.bool_(), R.INT32: pa.int32(), R.INT64: pa.int64(), R.FLOAT32: pa.float32(), R.FLOAT64: pa.float64(),
+           R.DATE32: pa.date32(), R.TIME64_US: pa.time64("us"), R.TIMESTAMP_US: pa.timestamp("us"),
+           R.TIMESTAMPTZ_US: pa.timestamp("us", tz="UTC")}
+
+
+def to_arrow(col):
+    """a parquet_ref column as a pyarrow array (host copy of the emit)"""
+    t, valid = col["type"], col["valid"]
+    mask = pa.py_buffer(np.packbits(valid, bitorder="little").tobytes())
+    n = len(valid)
+    if t == R.LIST:
+        kid = to_arrow(col["child"])
+        return pa.Array.from_buffers(pa.list_(kid.type), n, [mask, pa.py_buffer(col["offsets"].astype(np.int32).tobytes())],
+                                     children=[kid])
+    if t in (R.UTF8, R.LARGE_BINARY):
+        ty, ow = (pa.string(), np.int32) if t == R.UTF8 else (pa.large_binary(), np.int64)
+        return pa.Array.from_buffers(ty, n, [mask, pa.py_buffer(col["offsets"].astype(ow).tobytes()), pa.py_buffer(col["data"])])
+    if t == R.UUID:
+        return pa.Array.from_buffers(pa.binary(16), n, [mask, pa.py_buffer(col["values"].tobytes())])
+    if t == R.BOOLEAN:
+        return pa.Array.from_buffers(pa.bool_(), n, [mask, pa.py_buffer(np.packbits(col["values"], bitorder="little").tobytes())])
+    return pa.Array.from_buffers(PA_TYPE[t], n, [mask, pa.py_buffer(np.ascontiguousarray(col["values"]).tobytes())])
+
+
+def measure_emits(lib, emits, reps, warmup):
+    """emits: Arrow batch handles of one workload; sums over them"""
+    t0, t1, tp, sizes, payload, rows = [], [], [], [0, 0, 0], 0, 0
+    for a in emits:
+        cols = emit_columns(lib, a)
+        fields = fields_for(cols)
+        n = lib.etl_dec_arrow_rows(a)
+        rows += n
+        for codec, acc in ((abi.PQ_UNCOMPRESSED, t0), (abi.PQ_SNAPPY, t1)):
+            acc.append(timed(lambda: lib.etl_dec_parquet_free(pq_write(lib, a, fields, 0, n, codec, 0)[1]), reps, warmup))
+            rc, h = pq_write(lib, a, fields, 0, n, codec, 0)
+            assert rc == 0
+            sizes[codec] += lib.etl_dec_parquet_size(h)
+            if codec == abi.PQ_UNCOMPRESSED:
+                for l in range(len(fields)):
+                    m = abi.ParquetMetrics()
+                    lib.etl_dec_parquet_metrics(h, l, C.byref(m))
+                    payload += m.uncompressed_bytes
+            lib.etl_dec_parquet_free(h)
+        table = pa.table({f[0]: to_arrow(c) for c, f in zip(cols, fields)})
+        sink = io.BytesIO()
+        pq.write_table(table, sink, compression="snappy")
+        sizes[2] += len(sink.getvalue())
+
+        def cpu():
+            pq.write_table(table, io.BytesIO(), compression="snappy")
+        tp.append(timed(cpu, max(3, reps // 2), 1))
+    s1 = sum_stats(t1)
+    return dict(rows=int(rows), write_ms_uncompressed=sum_stats(t0), write_ms_snappy=s1,
+                snappy_GBps=round(payload / (s1["median"] * 1e-3) / 1e9, 2) if s1["median"] else None,
+                file_bytes_uncompressed=int(sizes[0]), file_bytes_snappy=int(sizes[1]),
+                pyarrow_snappy_ms=sum_stats(tp), pyarrow_file_bytes=int(sizes[2]))
+
+
+def copy_table(n_rows, reps, warmup):
+    oids, rows = bench_copy_table(n_rows)
+    lib = abi.load()
+    blob = b"".join(rows)
+    offs = np.zeros(len(rows) + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum([len(r) for r in rows])
+    d_buf = torch.zeros(len(blob) + 64, dtype=torch.uint8, device="cuda")
+    d_buf[:len(blob)].copy_(torch.from_numpy(np.frombuffer(blob, dtype=np.uint8).copy()))
+    d_off = torch.from_numpy(offs.view(np.int64).copy()).cuda()
+    torch.cuda.synchronize()
+    dec = decoder.Decoder(0)
+    dec.put_table_schema(9, [dict(name=f"c{i}", type_oid=o, pk=1 if i == 0 else None, nullable=i != 0) for i, o in enumerate(oids)])
+    inp = abi.CopyInput()
+    inp.dev_buf, inp.dev_row_offsets, inp.len, inp.n_rows, inp.row_offsets = d_buf.data_ptr(), d_off.data_ptr(), len(blob), len(rows), offs.ctypes.data
+    h = C.c_void_p()
+    assert lib.etl_dec_copy_decode(dec._ctx, 9, C.byref(inp), 0, C.byref(h)) == 0, lib.etl_dec_last_error(dec._ctx)
+    with decoder.BatchHandle(dec, h) as bh:
+        a = C.c_void_p()
+        assert lib.etl_dec_arrow_emit(bh._h, 0, KINDS, 1, C.byref(a)) == 0
+        res = dict(workload="bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
+        res.update(measure_emits(lib, [a], reps, warmup))
+        lib.etl_dec_arrow_free(a)
+        print(json.dumps(res), flush=True)
+    dec.close()
+
+
+def streaming(name, scale, reps, warmup):
+    w = wl.make(name, scale, n_segments=1)
+    stream, stats = w.generate()
+    st = decoder.Stager(stream.nbytes, 2048)
+    st.append_framed(stream)
+    dec = decoder.Decoder(0)
+    for tid, cols in w.table_schemas().items():
+        dec.put_table_schema(tid, cols)
+    lib = abi.load()
+    res = dict(workload=name, scale=scale, stream_bytes=int(stream.nbytes))
+    with dec.decode_input(st.view(), to_host=False) as bh:
+        emits = []
+        for si in range(bh.summary().n_schemas):
+            a = C.c_void_p()
+            assert lib.etl_dec_arrow_emit(bh._h, si, KINDS, 1, C.byref(a)) == 0
+            emits.append(a)
+        res.update(measure_emits(lib, emits, reps, warmup), versions=len(emits))
+        for a in emits:
+            lib.etl_dec_arrow_free(a)
+    st.close()
+    dec.close()
+    print(json.dumps(res), flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--copy-rows", type=int, default=1_000_000)
+    ap.add_argument("--c3-scale", type=float, default=1.0)
+    ap.add_argument("--c4-scale", type=float, default=0.1)
+    ap.add_argument("--reps", type=int, default=7)
+    ap.add_argument("--warmup", type=int, default=2)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("parquet_measure needs a CUDA device")
+    t = time.time()
+    print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
+    copy_table(a.copy_rows, a.reps, a.warmup)
+    for name, scale in (("c3", a.c3_scale), ("c4", a.c4_scale)):
+        streaming(name, scale, a.reps, a.warmup)
+    print(json.dumps(dict(wall_s=round(time.time() - t, 1))), flush=True)
+
+
+if __name__ == "__main__":
+    main()
