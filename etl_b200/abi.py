@@ -281,6 +281,8 @@ DL_REJECT_UPDATE_NO_IDENTITY, DL_REJECT_DELETE_NO_IDENTITY, DL_REJECT_DELETE_NO_
 # etl_dec_parquet_write codecs (ETL_PQ_*) and etl_parquet_metrics.flags
 PQ_UNCOMPRESSED, PQ_SNAPPY = 0, 1
 PQ_HAS_MIN_MAX = 1
+# codec bit: dictionary-encode the eligible column chunks (ETL_PQ_DICTIONARY)
+PQ_DICTIONARY = 0x100
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

@@ -1,5 +1,6 @@
 // parquet_format.cuh — the byte-level pieces of the Parquet writer (parquet_write.cu) that a host harness can compile too
-// (tests/emul/host_parquet.cpp builds this same file with g++, so the CPU suite checks it against tests/parquet_ref.py):
+// (tests/emul/host_parquet.cpp and host_parquet_dict.cpp build this same file with g++, so the CPU suite checks it against
+// tests/parquet_ref.py and tests/parquet_dict_ref.py):
 //   * a Thrift compact-protocol writer (Parquet's footer and page headers): fields in ascending id order, i32 / i64 as
 //     zigzag varints, binary as varint length + bytes, lists with the size in the header nibble below 15;
 //   * the data page header (PageHeader {type DATA_PAGE, uncompressed_page_size, compressed_page_size, data_page_header
@@ -10,7 +11,12 @@
 //   * the Snappy compressor of one fragment of at most 64 KiB: 4-byte hash match finder over a 4096-entry table,
 //     literal / copy-1 / copy-2 elements; copies never reach outside the fragment, so fragments compress independently
 //     and their element streams concatenate into one valid stream;
-//   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders.
+//   * the dictionary pieces (ETL_PQ_DICTIONARY): the DICTIONARY_PAGE header, the RLE_DICTIONARY data page header, and
+//     the RLE / bit-packed hybrid of dictionary indices (bit width 1..18) under the same run rule as the levels, split
+//     into the run classification and the writing of one run, so that the CTA-parallel encoder of parquet_write.cu and
+//     the serial indices_encode below share them;
+//   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders, and
+//     for a dictionary chunk its dictionary_page_offset and encoding_stats.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -24,7 +30,8 @@ namespace etl_pq {
 enum { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
 enum { CT_UTF8 = 0, CT_LIST = 3, CT_DATE = 6, CT_TIMESTAMP_MICROS = 10, CT_NONE = -1 };
 enum { REP_REQUIRED = 0, REP_OPTIONAL = 1, REP_REPEATED = 2 };
-enum { ENC_PLAIN = 0, ENC_RLE = 3 };
+enum { ENC_PLAIN = 0, ENC_RLE = 3, ENC_RLE_DICTIONARY = 8 };
+enum { PAGE_DATA = 0, PAGE_DICTIONARY = 2 };
 constexpr uint32_t kPageRows = 20000;                 // a page ends after the row that brings it to this many rows
 constexpr uint64_t kPageBytes = 1ull << 20;           // … or to this many PLAIN value bytes
 constexpr uint64_t kRowGroupRows = 1ull << 20;
@@ -32,6 +39,7 @@ constexpr uint32_t kFragment = 65536;                 // Snappy fragment
 constexpr uint32_t kSnappyHashBits = 12;
 constexpr uint32_t kStatMax = 64;                     // a longer byte-array min / max is not written
 constexpr uint32_t kPageHeaderMax = 48;               // 4 fields + a 4-field struct of i32 varints: at most 41 bytes
+constexpr uint64_t kDictBytes = 1ull << 20;           // a chunk is dictionary-encoded while its entries' PLAIN size fits
 
 __host__ __device__ inline uint32_t snappy_bound(uint32_t n) { return 32u + n + n / 6u; }
 // level section bound (4-byte length prefix, runs): every group costs at most w bytes + 1 header byte of its bit-packed
@@ -79,17 +87,32 @@ struct TWriter {
   __host__ __device__ void list_struct_begin() { last[++depth] = 0; }   // one struct element of a list
 };
 
-// DATA_PAGE header; returns its length (at most kPageHeaderMax)
-__host__ __device__ inline uint32_t page_header(uint8_t* out, uint32_t usize, uint32_t csize, uint32_t num_values) {
+// DATA_PAGE header (values PLAIN, or RLE_DICTIONARY indices); returns its length (at most kPageHeaderMax)
+__host__ __device__ inline uint32_t page_header(uint8_t* out, uint32_t usize, uint32_t csize, uint32_t num_values,
+                                                uint32_t encoding = ENC_PLAIN) {
   TWriter w(out);
-  w.i32(1, 0);               // type DATA_PAGE
+  w.i32(1, PAGE_DATA);
   w.i32(2, (int32_t)usize);
   w.i32(3, (int32_t)csize);
   w.begin(5);                // data_page_header
   w.i32(1, (int32_t)num_values);
-  w.i32(2, ENC_PLAIN);
+  w.i32(2, (int32_t)encoding);
   w.i32(3, ENC_RLE);
   w.i32(4, ENC_RLE);
+  w.end();
+  w.end();
+  return (uint32_t)w.n;
+}
+
+// DICTIONARY_PAGE header {type, sizes, dictionary_page_header {num_values, encoding PLAIN}}; at most 25 bytes
+__host__ __device__ inline uint32_t dict_page_header(uint8_t* out, uint32_t usize, uint32_t csize, uint32_t entries) {
+  TWriter w(out);
+  w.i32(1, PAGE_DICTIONARY);
+  w.i32(2, (int32_t)usize);
+  w.i32(3, (int32_t)csize);
+  w.begin(7);                // dictionary_page_header
+  w.i32(1, (int32_t)entries);
+  w.i32(2, ENC_PLAIN);
   w.end();
   w.end();
   return (uint32_t)w.n;
@@ -135,6 +158,59 @@ __host__ __device__ inline uint64_t levels_encode(const uint8_t* lv, uint64_t n,
   }
   return o;
 }
+
+// ------------------------------------------------------------------------------------------------ dictionary indices
+// The hybrid of n indices x (bit width w = max(1, bits(entries - 1)) <= 18), without the bit-width byte or a length
+// prefix, under the run rule of the levels: groups of 8; the uniform value of a group (its present entries equal) or -1.
+__host__ __device__ inline int64_t idx_cls(const uint32_t* x, uint64_t n, uint64_t g) {
+  const uint64_t a = g * 8, m = n - a < 8 ? n - a : 8;
+  const uint32_t v = x[a];
+  for (uint64_t j = 1; j < m; j++) if (x[a + j] != v) return -1;
+  return v;
+}
+// run of groups [g, h): an RLE run when group g is uniform (then every group of the run is), else bit-packed (h - g <= 63)
+__host__ __device__ inline uint64_t idx_run_bytes(const uint32_t* x, uint64_t n, uint32_t w, uint64_t g, uint64_t h) {
+  if (idx_cls(x, n, g) >= 0) {
+    const uint64_t cnt = ((h * 8 < n ? h * 8 : n)) - g * 8;
+    return varint(cnt << 1, nullptr) + (w + 7) / 8;
+  }
+  return 1 + (h - g) * w;
+}
+__host__ __device__ inline void idx_write_run(const uint32_t* x, uint64_t n, uint32_t w, uint64_t g, uint64_t h, uint8_t* out) {
+  const int64_t c = idx_cls(x, n, g);
+  if (c >= 0) {
+    const uint64_t cnt = ((h * 8 < n ? h * 8 : n)) - g * 8;
+    const uint32_t o = varint(cnt << 1, out);
+    for (uint32_t b = 0; b < (w + 7) / 8; b++) out[o + b] = (uint8_t)((uint64_t)c >> (8 * b));
+    return;
+  }
+  out[0] = (uint8_t)(((h - g) << 1) | 1u);
+  uint64_t o = 1, acc = 0;
+  uint32_t bits = 0;
+  for (uint64_t e = g * 8; e < h * 8; e++) {          // LSB first, the last group zero-padded
+    acc |= (uint64_t)(e < n ? x[e] : 0u) << bits;
+    bits += w;
+    while (bits >= 8) { out[o++] = (uint8_t)acc; acc >>= 8; bits -= 8; }
+  }
+}
+// serial encoder (the host harness; the device encodes the same runs in parallel); returns the bytes written
+__host__ __device__ inline uint64_t indices_encode(const uint32_t* x, uint64_t n, uint32_t w, uint8_t* out) {
+  const uint64_t ng = (n + 7) / 8;
+  uint64_t o = 0, g = 0;
+  while (g < ng) {
+    const int64_t c = idx_cls(x, n, g);
+    uint64_t h = g + 1;
+    if (c >= 0) while (h < ng && idx_cls(x, n, h) == c) h++;
+    else while (h < ng && h - g < 63 && idx_cls(x, n, h) < 0) h++;
+    idx_write_run(x, n, w, g, h, out + o);
+    o += idx_run_bytes(x, n, w, g, h);
+    g = h;
+  }
+  return o;
+}
+// bound of an RLE_DICTIONARY payload's index part (bit-width byte + runs): a group costs at most w + 1 bytes bit-packed
+// or 4 as (part of) an RLE run
+__host__ __device__ inline uint64_t indices_bound(uint64_t n) { return 1 + ((n + 7) / 8) * 19; }
 
 // ------------------------------------------------------------------------------------------------ Snappy
 __host__ __device__ inline uint32_t load32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
@@ -212,9 +288,12 @@ struct Leaf {                       // one column of the file: a flat leaf, or a
   bool required, is_list;
 };
 struct Chunk {
-  uint64_t offset, num_values, usize, csize, null_count;
+  uint64_t offset, num_values, usize, csize, null_count;   // offset: the chunk's first page (a dictionary chunk: its dictionary page)
   bool has_minmax;
   std::string min, max;
+  bool dict = false;                // dictionary chunk: its data pages are RLE_DICTIONARY
+  uint64_t data_offset = 0;         // dictionary chunk: the first data page
+  uint64_t data_pages = 0;          // dictionary chunk: its data pages
 };
 
 inline void schema_element(TWriter& w, const Leaf& L, bool element) {
@@ -287,19 +366,21 @@ inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::v
         w.begin(3);
         w.i32(1, (int32_t)L.ptype);
         const bool levels = L.is_list || !L.required;
-        w.list(2, TT_I32, levels ? 2 : 1);
+        w.list(2, TT_I32, (levels ? 2 : 1) + (C.dict ? 1 : 0));
         w.var(zigzag(ENC_PLAIN));
         if (levels) w.var(zigzag(ENC_RLE));
+        if (C.dict) w.var(zigzag(ENC_RLE_DICTIONARY));
         const std::string& leaf_name = L.name;
         w.list(3, TT_BINARY, L.is_list ? 3 : 1);
         w.var(leaf_name.size());
         for (char ch : leaf_name) w.byte((uint8_t)ch);
         if (L.is_list) { w.var(4); for (char ch : std::string("list")) w.byte((uint8_t)ch); w.var(7); for (char ch : std::string("element")) w.byte((uint8_t)ch); }
-        w.i32(4, (int32_t)codec);
+        w.i32(4, (int32_t)(codec & 0xFFu));        // the compression codec, without the ETL_PQ_DICTIONARY bit
         w.i64(5, (int64_t)C.num_values);
         w.i64(6, (int64_t)C.usize);
         w.i64(7, (int64_t)C.csize);
-        w.i64(9, (int64_t)C.offset);
+        w.i64(9, (int64_t)(C.dict ? C.data_offset : C.offset));
+        if (C.dict) w.i64(11, (int64_t)C.offset);
         w.begin(12);
         w.i64(3, (int64_t)C.null_count);
         if (C.has_minmax) {
@@ -307,6 +388,11 @@ inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::v
           w.bin(6, (const uint8_t*)C.min.data(), (uint32_t)C.min.size());
         }
         w.end();
+        if (C.dict) {                                  // PageEncodingStats {page_type, encoding, count}
+          w.list(13, TT_STRUCT, 2);
+          w.list_struct_begin(); w.i32(1, PAGE_DICTIONARY); w.i32(2, ENC_PLAIN); w.i32(3, 1); w.end();
+          w.list_struct_begin(); w.i32(1, PAGE_DATA); w.i32(2, ENC_RLE_DICTIONARY); w.i32(3, (int32_t)C.data_pages); w.end();
+        }
         w.end();
         w.end();
       }

@@ -10,6 +10,16 @@
 //      (emit_scan.cuh) give their prefix sums.  k_cut, a thread per (leaf, row group), walks the greedy page rule with a
 //      binary search over the value prefix sums; it runs twice, counting and then writing the pages.  SYNC 1 (the page
 //      counts, the totals and the required-null rows) sizes every buffer from bounds, so no later step waits for sizes.
+//   1'. Dictionaries (ETL_PQ_DICTIONARY).  k_cut puts a dictionary slot (a Page of kind 1) in front of the data pages of
+//      every chunk of a non-Boolean leaf.  k_dict_setup sizes each chunk's open-addressing table from its non-null count
+//      (the NN prefix sums), a scan places the tables; k_dict_insert (per leaf, grid-stride) inserts every non-null item,
+//      a slot keeping the smallest chunk-relative item of its value by atomicMin, and adds each new entry's PLAIN size to
+//      its chunk, marking it for fallback past 1 MiB (exact whatever the order: the entries are a set); k_dict_mark flags
+//      the first occurrences (an item equal to its slot's value) and the scans of emit_scan.cuh turn the flags into
+//      entry ids in item order and, for byte arrays, the entry sizes into PLAIN offsets; k_dict_finish decides each chunk
+//      and its bit width; k_dict_page writes the entries into the dictionary slot.  k_encode<true> writes a dictionary
+//      chunk's compacted entry ids and encodes their runs with the whole CTA (encode_indices); k_page gives a slot the
+//      DICTIONARY_PAGE header, or no bytes when its chunk is PLAIN, so a fallen-back chunk is the PLAIN chunk.
 //   2. Encode.  k_encode, a CTA per page: the page's level bytes into scratch (thread per row), the RLE hybrid by one
 //      thread per section over whole 8-entry groups (one u64 load per group), then the non-null values compacted with a
 //      block scan over the validity: fixed width at rank * width, Booleans by atomicOr into a zeroed bit scratch, byte
@@ -26,7 +36,10 @@
 //      SYNC 3 ends the call (and the copy to pinned host memory with to_host).
 // Scratch: per (row, leaf) 3 × 4 B lengths + 3 × 8 B prefix sums; per level entry 2 B (+ 64 B per page of the leaf);
 // Boolean leaves 1 bit per item (+ 4 B per page of the leaf); per page a bounded payload slot (the PLAIN value bytes + levels_bound per section) and,
-// with Snappy, a compressed slot of snappy_bound per fragment.
+// with Snappy, a compressed slot of snappy_bound per fragment.  ETL_PQ_DICTIONARY adds, per item of an eligible leaf
+// (bounded by its level entries), 4 B slot + 4 B flag + 4 B entry size / index + 2 × 8 B prefix sums and 0.5 B of run
+// heads (+ 12 B per page), the chunks' tables (4 B × pow2 >= 2 × non-null values: at most 16 B per value), a dictionary
+// slot per chunk (at most 1 MiB, at most the chunk's PLAIN bytes) and 32 B more per data page slot.
 // ptxas -v (sm_90a, CUDA 12.9): see the comment at the end of this file.
 #include <cuda_runtime.h>
 
@@ -55,6 +68,7 @@ struct LeafDev {
   const uint8_t* values;     // fixed width / Boolean bits
   const void* offs;          // byte arrays
   const uint8_t* data;
+  uint64_t dscr, hscr;       // ETL_PQ_DICTIONARY: first item slot of the leaf's dictionary scratch / of its run heads
 };
 struct Page {
   uint32_t leaf, chunk;
@@ -66,15 +80,34 @@ struct Page {
   uint64_t usize, csize;
   uint32_t hlen, plen;       // page header / Snappy preamble bytes
   uint64_t min_it, max_it, nan;
+  uint32_t kind, _pad;       // 0 data page; 1 the dictionary slot in front of a chunk's data pages (ETL_PQ_DICTIONARY)
   uint8_t hdr[kPageHeaderMax];
   uint8_t pre[8];
 };
 struct ChunkOut {
   uint64_t offset, num_values, usize, csize, null_count, nan_count;
-  uint32_t has, min_len, max_len, _pad;
+  uint64_t data_offset, data_pages;   // the first data page and the data pages (they differ from offset with a dictionary)
+  uint32_t has, min_len, max_len, dict;
   uint8_t min[kStatMax], max[kStatMax];
 };
 constexpr uint64_t kNone = ~0ull;
+// ETL_PQ_DICTIONARY: one record per chunk (Boolean chunks have none: dict stays 0)
+struct DictChunk {
+  unsigned long long bytes;  // PLAIN size of the entries claimed so far
+  uint64_t it0, it1;         // the chunk's items
+  uint64_t tab;              // its table's first slot
+  uint64_t page;             // its dictionary slot
+  uint64_t entries;
+  uint32_t mask;             // table slots - 1
+  uint32_t fallback;         // the entries passed kDictBytes (or filled the table, which implies it): PLAIN chunk
+  uint32_t dict, width;      // k_dict_finish: dictionary-encoded, index bit width
+};
+constexpr uint32_t kEmpty = 0xffffffffu;
+constexpr uint32_t kInsBlocks = 1024, kInsThreads = 256;   // k_dict_insert's grid-stride launch
+// entries a table must hold: every entry up to the first past kDictBytes (each entry is >= 4 PLAIN bytes), plus one
+// insert in flight per thread of k_dict_insert when the fallback mark is set; a table that fills anyway also proves it
+constexpr uint64_t kDictCap = kDictBytes / 4 + 1 + (uint64_t)kInsBlocks * kInsThreads;
+constexpr uint32_t kLongBytes = 32;   // longer byte arrays are hashed and compared by the whole warp
 
 __device__ __forceinline__ bool bit(const uint8_t* v, uint64_t i) { return (v[i >> 3] >> (i & 7)) & 1u; }
 __device__ __forceinline__ uint64_t byte_off(const LeafDev& L, uint64_t i) {
@@ -143,7 +176,7 @@ __global__ void __launch_bounds__(256) k_plan(const LeafDev* leaves, uint64_t rb
 __global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, uint64_t rb, uint64_t n, const uint64_t* E,
                       const uint64_t* NN, const uint64_t* V, uint32_t* n_pages, const uint64_t* page_base, const uint64_t* leaf_page_base,
                       const uint64_t* lscr_base,
-                      Page* pages) {
+                      Page* pages, int dict) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n_leaves * n_rg) return;
   const uint32_t g = t / n_leaves, l = t % n_leaves;
@@ -152,6 +185,16 @@ __global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, u
   const uint64_t g0 = (uint64_t)g * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
   const bool boolean = L.atype == ETL_ARROW_BOOLEAN;
   const uint64_t thresh = boolean ? 8 * kPageBytes - 7 : kPageBytes;   // ceil(bits / 8) >= 1 MiB
+  const uint32_t slot = dict && !boolean ? 1 : 0;          // the dictionary slot in front of the data pages
+  if (pages && slot) {
+    Page& P = pages[page_base[t]];
+    memset(&P, 0, sizeof P);
+    P.leaf = l; P.chunk = t; P.kind = 1; P.row0 = P.row1 = g0; P.e0 = P.e1 = e[g0];
+    P.it0 = L.is_list ? (uint64_t)L.loffs[rb + g0] : rb + g0;
+    P.it1 = L.is_list ? (uint64_t)L.loffs[rb + g1] : rb + g1;
+    P.ubound = min(v[g1] - v[g0], kDictBytes);           // the entries are distinct values of the chunk
+    P.min_it = P.max_it = kNone;
+  }
   uint32_t np = 0;
   for (uint64_t s = g0; s < g1; np++) {
     uint64_t hi = min(g1 - 1, s + kPageRows - 1);
@@ -161,7 +204,7 @@ __global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, u
     }
     const uint64_t end = hi + 1;
     if (pages) {
-      Page& P = pages[page_base[t] + np];
+      Page& P = pages[page_base[t] + slot + np];
       P.leaf = l; P.chunk = t; P.lp = leaf_page_base[t] + np; P.row0 = s; P.row1 = end; P.e0 = e[s]; P.e1 = e[end];
       P.it0 = L.is_list ? (uint64_t)L.loffs[rb + s] : rb + s;
       P.it1 = L.is_list ? (uint64_t)L.loffs[rb + end] : rb + end;
@@ -169,25 +212,119 @@ __global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, u
       P.vbytes = boolean ? (P.nn + 7) / 8 : v[end] - v[s];
       const uint64_t ne = P.e1 - P.e0;
       P.ubound = P.vbytes + (L.max_def ? levels_bound(ne, L.w) : 0) + (L.max_rep ? levels_bound(ne, 1) : 0);
+      if (slot) P.ubound += 32;                          // bit-width byte + index runs <= PLAIN values + 20 (indices_bound)
       // level scratch: 8-aligned per page, two sections (rep | def)
       P.lscr = lscr_base[l] + 2 * ((P.e0 + 7) & ~7ull) + 64ull * P.lp;
-      P.usize = P.csize = 0; P.hlen = P.plen = 0; P.min_it = P.max_it = kNone; P.nan = 0;
+      P.usize = P.csize = 0; P.hlen = P.plen = 0; P.min_it = P.max_it = kNone; P.nan = 0; P.kind = 0;
     }
     s = end;
   }
   if (!pages) n_pages[t] = np;
 }
 
-// 2. a CTA per page: levels, PLAIN values, statistics
+// block-wide scans of kEncThreads threads (every thread calls them): inclusive sum, inclusive max
+__device__ uint64_t block_sum(uint64_t x, uint64_t* s_warp, uint64_t* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += y; }
+  if (lane == 31) s_warp[wid] = x;
+  __syncthreads();
+  uint64_t before = 0, t = 0;
+  for (int k = 0; k < (int)(blockDim.x / 32); k++) { if (k < wid) before += s_warp[k]; t += s_warp[k]; }
+  __syncthreads();
+  *total = t;
+  return before + x;
+}
+__device__ int64_t block_max(int64_t x, int64_t* s_warp, int64_t* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d && y > x) x = y; }
+  if (lane == 31) s_warp[wid] = x;
+  __syncthreads();
+  int64_t before = -1, t = -1;
+  for (int k = 0; k < (int)(blockDim.x / 32); k++) { if (k < wid && s_warp[k] > before) before = s_warp[k]; if (s_warp[k] > t) t = s_warp[k]; }
+  __syncthreads();
+  *total = t;
+  return before > x ? before : x;
+}
+
+// the index hybrid of a page by the whole CTA (idx_cls / idx_run_bytes / idx_write_run of parquet_format.cuh, so the
+// runs are those of the serial indices_encode): 1. classify the groups of 8 tile by tile and keep the run heads (a
+// uniform group whose predecessor is not the same uniform value; a non-uniform group 63k groups after the start of its
+// stretch, found by a max scan of the last uniform group); 2. the heads' byte sizes, their scan, and one thread per run
+// writes it.  x: the page's nn indices; heads: room for ng + 1; returns the bytes written to out
+__device__ uint64_t encode_indices(const uint32_t* x, uint64_t nn, uint32_t w, uint32_t* heads, uint8_t* out, uint64_t* s_warp,
+                                   int64_t* s_cls) {
+  __shared__ uint64_t s_carry[3];                         // runs so far, last uniform group, class of the tile's last group
+  const uint64_t ng = (nn + 7) / 8;
+  if (threadIdx.x == 0) { s_carry[0] = 0; s_carry[1] = (uint64_t)-1; s_carry[2] = (uint64_t)-2; }
+  __syncthreads();
+  for (uint64_t t0 = 0; t0 < ng; t0 += blockDim.x) {
+    const uint64_t g = t0 + threadIdx.x;
+    const int64_t c = g < ng ? idx_cls(x, nn, g) : -2;
+    s_cls[threadIdx.x] = c;
+    const int64_t prev_tile_cls = (int64_t)s_carry[2], last_u = (int64_t)s_carry[1];
+    __syncthreads();
+    const int64_t prev = threadIdx.x ? s_cls[threadIdx.x - 1] : prev_tile_cls;
+    int64_t tmax;
+    int64_t u = block_max(c >= 0 ? (int64_t)g : -1, (int64_t*)s_warp, &tmax);
+    if (last_u > u) u = last_u;
+    const bool head = g < ng && (c >= 0 ? (g == 0 || prev != c) : (g - (uint64_t)(u + 1)) % 63 == 0);
+    uint64_t cnt;
+    const uint64_t incl = block_sum(head, s_warp, &cnt);
+    const uint64_t base = s_carry[0];
+    if (head) heads[base + incl - 1] = (uint32_t)g;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      s_carry[0] = base + cnt;
+      if (tmax > last_u) s_carry[1] = (uint64_t)tmax;
+      const uint64_t last = min((uint64_t)blockDim.x, ng - t0) - 1;
+      s_carry[2] = (uint64_t)s_cls[last];
+    }
+    __syncthreads();
+  }
+  const uint64_t R = s_carry[0];
+  if (threadIdx.x == 0) heads[R] = (uint32_t)ng;
+  __syncthreads();
+  uint64_t o = 0;
+  for (uint64_t r0 = 0; r0 < R; r0 += blockDim.x) {
+    const uint64_t r = r0 + threadIdx.x;
+    const uint64_t g = r < R ? heads[r] : 0, h = r < R ? heads[r + 1] : 0;
+    const uint64_t b = r < R ? idx_run_bytes(x, nn, w, g, h) : 0;
+    uint64_t tot;
+    const uint64_t incl = block_sum(b, s_warp, &tot);
+    if (r < R) idx_write_run(x, nn, w, g, h, out + o + incl - b);
+    o += tot;
+  }
+  return o;
+}
+
+// dictionary state handed to k_encode<true> (ETL_PQ_DICTIONARY)
+struct DictArgs {
+  const DictChunk* chunks;
+  const uint32_t* tab;       // the chunks' tables: chunk-relative item of each entry's first occurrence
+  const uint32_t* pos;       // per item: its slot
+  const uint64_t* first;     // per item: exclusive scan of the first-occurrence flags (the entry ids)
+  uint32_t* idx;             // per item: the pages' compacted indices
+  uint32_t* heads;           // run heads
+};
+
+// 2. a CTA per page: levels, PLAIN values (kDict: the dictionary indices of a dictionary chunk), statistics
 constexpr int kEncThreads = 256;
+template <bool kDict>
 __global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, Page* pages, uint64_t rb, const uint64_t* E,
                                                         uint64_t n, uint8_t* lscr, uint8_t* uslot_base, const uint64_t* uslot,
-                                                        uint32_t* bool_scr) {
+                                                        uint32_t* bool_scr, DictArgs D) {
   __shared__ uint64_t s_lv, s_warp[kEncThreads / 32], s_min[kEncThreads], s_max[kEncThreads];
   __shared__ unsigned long long s_nan;
   const uint32_t p = blockIdx.x;
   Page& P = pages[p];
+  if (kDict && P.kind) return;                          // a dictionary slot: k_dict_page
   const LeafDev L = leaves[P.leaf];
+  const bool dict = kDict && D.chunks[P.chunk].dict;
+  uint64_t i0 = 0, c0 = 0;                              // the leaf's first item, the chunk's first entry id
+  if (dict) {
+    i0 = L.is_list ? (uint64_t)L.loffs[rb] : rb;
+    c0 = D.first[L.dscr + D.chunks[P.chunk].it0 - i0];
+  }
   const uint64_t ne = P.e1 - P.e0;
   uint8_t* rep = lscr + P.lscr;
   uint8_t* def = rep + ((ne + 15) & ~7ull);
@@ -231,7 +368,7 @@ __global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, P
     const uint64_t it = t0 + threadIdx.x;
     const bool v = it < P.it1 && bit(L.valid, it);
     uint64_t sz = 0, boff = 0, blen = 0;
-    if (v && is_bytes(L)) { boff = byte_off(L, it); blen = byte_off(L, it + 1) - boff; sz = 4 + blen; }
+    if (v && is_bytes(L) && !dict) { boff = byte_off(L, it); blen = byte_off(L, it + 1) - boff; sz = 4 + blen; }
     else if (v) sz = 1;
     // block exclusive scan of sz
     uint64_t x = sz;
@@ -242,7 +379,12 @@ __global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, P
     for (int k = 0; k < kEncThreads / 32; k++) { if (k < wid) before += s_warp[k]; tile += s_warp[k]; }
     const uint64_t rank = base + before + x - sz;
     if (v) {
-      if (L.atype == ETL_ARROW_BOOLEAN) {
+      if (dict) {                                       // the entry id of the item's value
+        const DictChunk& K = D.chunks[P.chunk];
+        const uint64_t j = L.dscr + it - i0;
+        const uint64_t fo = D.tab[K.tab + D.pos[j]];    // chunk-relative first occurrence
+        D.idx[L.dscr + P.it0 - i0 + rank] = (uint32_t)(D.first[L.dscr + K.it0 + fo - i0] - c0);
+      } else if (L.atype == ETL_ARROW_BOOLEAN) {
         if (bit(L.values, it)) atomicOr(bool_scr + bw + (rank >> 5), 1u << (rank & 31));
       } else if (!is_bytes(L)) {
         for (uint32_t k = 0; k < L.fixed; k++) val[rank * L.fixed + k] = L.values[it * L.fixed + k];
@@ -252,7 +394,7 @@ __global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, P
       if (is_nan(L, it)) nan++;
       else fold(L, it, it, mn, mx);
     }
-    if (is_bytes(L)) {                                  // every value of the warp copied by the whole warp
+    if (is_bytes(L) && !dict) {                         // every value of the warp copied by the whole warp
       unsigned todo = __ballot_sync(0xffffffffu, v && blen);
       while (todo) {
         const int src = __ffs(todo) - 1;
@@ -280,9 +422,246 @@ __global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, P
   if (L.atype == ETL_ARROW_BOOLEAN) {                   // the page's bits, from the word-aligned scratch
     for (uint64_t k = threadIdx.x; k < P.vbytes; k += blockDim.x) val[k] = (uint8_t)(bool_scr[bw + (k >> 2)] >> (8 * (k & 3)));
   }
+  if (dict) {                                           // bit width, then the index runs
+    const uint64_t mn0 = s_min[0], mx0 = s_max[0];
+    const unsigned long long nan0 = s_nan;
+    const uint32_t w = D.chunks[P.chunk].width;
+    if (threadIdx.x == 0) val[0] = (uint8_t)w;
+    const uint64_t len = encode_indices(D.idx + L.dscr + P.it0 - i0, P.nn, w, D.heads + L.hscr + (P.it0 - i0) / 8 + 3 * P.lp,
+                                        val + 1, s_warp, (int64_t*)s_min);
+    if (threadIdx.x == 0) {
+      P.usize = s_lv + 1 + len;
+      P.min_it = mn0; P.max_it = mx0; P.nan = nan0;
+    }
+    return;
+  }
   if (threadIdx.x == 0) {
     P.usize = s_lv + P.vbytes;
     P.min_it = s_min[0]; P.max_it = s_max[0]; P.nan = s_nan;
+  }
+}
+
+// 1c. ETL_PQ_DICTIONARY, a thread per chunk: its items, and its table sized from its non-null values (pow2 >= 2 ×
+// min(nn, kDictCap); Boolean chunks none) into tab_n, whose exclusive scan places the tables
+__global__ void k_dict_setup(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_chunks, uint64_t rb, uint64_t n, const uint64_t* NN,
+                             const uint64_t* page_base, DictChunk* D, unsigned long long* tab_n) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t > n_chunks) return;
+  if (t == n_chunks) { tab_n[t] = 0; return; }
+  const uint32_t g = t / n_leaves, l = t % n_leaves;
+  const LeafDev L = leaves[l];
+  const uint64_t g0 = (uint64_t)g * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
+  DictChunk K;
+  memset(&K, 0, sizeof K);
+  K.it0 = L.is_list ? (uint64_t)L.loffs[rb + g0] : rb + g0;
+  K.it1 = L.is_list ? (uint64_t)L.loffs[rb + g1] : rb + g1;
+  K.page = page_base[t];
+  uint64_t slots = 0;
+  if (L.atype != ETL_ARROW_BOOLEAN) {
+    const uint64_t* nv = NN + (uint64_t)l * (n + 1);
+    const uint64_t m = min(nv[g1] - nv[g0], kDictCap);
+    slots = 1;
+    while (slots < 2 * m) slots <<= 1;
+  }
+  K.mask = (uint32_t)(slots - 1);
+  D[t] = K;
+  tab_n[t] = slots;
+}
+
+__device__ __forceinline__ uint64_t mix64(uint64_t h) {
+  h ^= h >> 33; h *= 0xff51afd7ed558ccdull; h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 33;
+  return h;
+}
+// hash of bytes [k, len) step 32 of p (a lane's share of a long value, or k = 0 step 1 for a short one)
+__device__ __forceinline__ uint64_t hash_bytes(const uint8_t* p, uint64_t len, uint64_t k, uint64_t step) {
+  uint64_t h = 0x9e3779b97f4a7c15ull;
+  for (; k < len; k += step) h = (h ^ p[k]) * 0x100000001b3ull;
+  return h;
+}
+// the PLAIN bytes of present items a and b are equal (byte arrays of at most kLongBytes, or fixed width)
+__device__ bool same_value(const LeafDev& L, uint64_t a, uint64_t b) {
+  if (is_bytes(L)) {
+    const uint64_t a0 = byte_off(L, a), al = byte_off(L, a + 1) - a0, b0 = byte_off(L, b), bl = byte_off(L, b + 1) - b0;
+    if (al != bl) return false;
+    for (uint64_t k = 0; k < al; k++) if (L.data[a0 + k] != L.data[b0 + k]) return false;
+    return true;
+  }
+  switch (L.fixed) {
+    case 4: return ((const uint32_t*)L.values)[a] == ((const uint32_t*)L.values)[b];
+    case 8: return ((const uint64_t*)L.values)[a] == ((const uint64_t*)L.values)[b];
+    default: return ((const uint64_t*)L.values)[2 * a] == ((const uint64_t*)L.values)[2 * b] &&
+                    ((const uint64_t*)L.values)[2 * a + 1] == ((const uint64_t*)L.values)[2 * b + 1];
+  }
+}
+__device__ __forceinline__ uint64_t plain_size(const LeafDev& L, uint64_t it) {
+  return is_bytes(L) ? 4 + byte_off(L, it + 1) - byte_off(L, it) : L.fixed;
+}
+__device__ __forceinline__ uint32_t chunk_of(const DictChunk* D, uint32_t l, uint32_t n_leaves, uint32_t n_rg, uint64_t it) {
+  uint32_t g = 0;
+  while (g + 1 < n_rg && it >= D[(g + 1) * n_leaves + l].it0) g++;
+  return g * n_leaves + l;
+}
+// a slot claimed for a new entry: its PLAIN size joins the chunk's total; past kDictBytes the chunk falls back
+__device__ __forceinline__ void claimed(DictChunk& K, uint64_t sz) {
+  if (atomicAdd(&K.bytes, (unsigned long long)sz) + sz > kDictBytes) atomicExch(&K.fallback, 1u);
+}
+
+// a thread per chunk: its table's first slot, from the exclusive scan of the table sizes
+__global__ void k_dict_place(uint32_t n_chunks, const unsigned long long* tab_off, DictChunk* D) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < n_chunks) D[c].tab = tab_off[c];
+}
+
+// 1d. ETL_PQ_DICTIONARY, one leaf, grid-stride over its items (warp-uniform): each non-null item of a chunk that has
+// not fallen back goes into the chunk's open-addressing table (linear probing).  A slot keeps the smallest
+// chunk-relative item of its value (atomicMin), so after the pass an item is a first occurrence iff it is its slot's
+// value, whatever the order of the inserts.  Byte arrays longer than kLongBytes are hashed and compared by the warp.
+__global__ void __launch_bounds__(kInsThreads) k_dict_insert(const LeafDev* leaves, uint32_t l, uint32_t n_leaves, uint32_t n_rg,
+                                                             uint64_t rb, DictChunk* D, uint32_t* tab, uint32_t* pos) {
+  const LeafDev L = leaves[l];
+  const uint64_t i0 = L.is_list ? (uint64_t)L.loffs[rb] : rb, i1 = D[(n_rg - 1) * n_leaves + l].it1;
+  const int lane = threadIdx.x & 31;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t base = i0 + (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < i1; base += stride) {
+    const uint64_t it = base + lane;
+    bool v = it < i1 && bit(L.valid, it);
+    uint32_t c = 0;
+    if (v) {
+      c = chunk_of(D, l, n_leaves, n_rg, it);
+      v = !*(volatile uint32_t*)&D[c].fallback;          // inserts into a marked chunk stop
+    }
+    uint64_t len = 0;
+    if (v && is_bytes(L)) len = byte_off(L, it + 1) - byte_off(L, it);
+    const bool lng = v && len > kLongBytes;
+    uint64_t h = 0;
+    if (v && !lng) h = is_bytes(L) ? hash_bytes(L.data + byte_off(L, it), len, 0, 1) ^ len
+                                   : mix64(L.fixed == 16 ? ((const uint64_t*)L.values)[2 * it] ^ mix64(((const uint64_t*)L.values)[2 * it + 1])
+                                                         : L.fixed == 8 ? ((const uint64_t*)L.values)[it] : ((const uint32_t*)L.values)[it]);
+    if (v && !lng) {
+      DictChunk& K = D[c];
+      const uint32_t rel = (uint32_t)(it - K.it0);
+      uint32_t* T = tab + K.tab;
+      uint32_t s = (uint32_t)h & K.mask;
+      for (uint64_t probe = 0;; probe++, s = (s + 1) & K.mask) {
+        if (probe > K.mask) { atomicExch(&K.fallback, 1u); break; }   // full: more than kDictCap entries
+        uint32_t cur = *(volatile uint32_t*)&T[s];
+        if (cur == kEmpty) {
+          cur = atomicCAS(&T[s], kEmpty, rel);
+          if (cur == kEmpty) { pos[L.dscr + it - i0] = s; claimed(K, plain_size(L, it)); break; }
+        }
+        if (same_value(L, K.it0 + cur, it)) { atomicMin(&T[s], rel); pos[L.dscr + it - i0] = s; break; }
+      }
+    }
+    unsigned todo = __ballot_sync(0xffffffffu, lng);
+    while (todo) {                                       // one long value at a time, by the whole warp
+      const int src = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const uint64_t sit = __shfl_sync(0xffffffffu, it, src), slen = __shfl_sync(0xffffffffu, len, src);
+      const uint32_t sc = __shfl_sync(0xffffffffu, c, src);
+      const uint8_t* sp = L.data + byte_off(L, sit);
+      uint64_t hh = mix64(hash_bytes(sp, slen, lane, 32) + lane);
+      for (int d = 16; d > 0; d >>= 1) hh ^= __shfl_xor_sync(0xffffffffu, hh, d);
+      DictChunk& K = D[sc];
+      const uint32_t rel = (uint32_t)(sit - K.it0);
+      uint32_t* T = tab + K.tab;
+      uint32_t s = (uint32_t)(hh ^ slen) & K.mask;
+      for (uint64_t probe = 0;; probe++, s = (s + 1) & K.mask) {
+        if (probe > K.mask) { if (lane == 0) atomicExch(&K.fallback, 1u); break; }
+        uint32_t cur = 0;
+        int won = 0;
+        if (lane == 0) {
+          cur = *(volatile uint32_t*)&T[s];
+          if (cur == kEmpty) { cur = atomicCAS(&T[s], kEmpty, rel); won = cur == kEmpty; }
+        }
+        cur = __shfl_sync(0xffffffffu, cur, 0);
+        if (__shfl_sync(0xffffffffu, won, 0)) {
+          if (lane == 0) { pos[L.dscr + sit - i0] = s; claimed(K, 4 + slen); }
+          break;
+        }
+        const uint64_t o = K.it0 + cur, o0 = byte_off(L, o);   // a slot lost to another insert holds its claimant
+        bool eq = byte_off(L, o + 1) - o0 == slen;
+        if (eq) {
+          bool mine = true;
+          for (uint64_t k = lane; k < slen; k += 32) if (L.data[o0 + k] != sp[k]) { mine = false; break; }
+          eq = __all_sync(0xffffffffu, mine);
+        }
+        if (eq) {
+          if (lane == 0) { atomicMin(&T[s], rel); pos[L.dscr + sit - i0] = s; }
+          break;
+        }
+      }
+    }
+  }
+}
+
+// 1e. ETL_PQ_DICTIONARY, one leaf, a thread per item bound: first-occurrence flags (and, byte arrays, entry sizes) of
+// the items of chunks that have not fallen back, 0 elsewhere; their scans give entry ids and PLAIN offsets
+__global__ void __launch_bounds__(256) k_dict_mark(const LeafDev* leaves, uint32_t l, uint32_t n_leaves, uint32_t n_rg, uint64_t rb,
+                                                   uint64_t bound, const DictChunk* D, const uint32_t* tab, const uint32_t* pos,
+                                                   uint32_t* flag, uint32_t* esize) {
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= bound) return;
+  const LeafDev L = leaves[l];
+  const uint64_t i0 = L.is_list ? (uint64_t)L.loffs[rb] : rb, it = i0 + j;
+  uint32_t f = 0, sz = 0;
+  if (it < D[(n_rg - 1) * n_leaves + l].it1 && bit(L.valid, it)) {
+    const DictChunk& K = D[chunk_of(D, l, n_leaves, n_rg, it)];
+    if (!K.fallback && tab[K.tab + pos[L.dscr + j]] == (uint32_t)(it - K.it0)) { f = 1; sz = (uint32_t)plain_size(L, it); }
+  }
+  flag[L.dscr + j] = f;
+  if (esize) esize[L.dscr + j] = sz;
+}
+
+// 1f. ETL_PQ_DICTIONARY, a thread per chunk: entries, PLAIN size, decision, bit width; the dictionary slot's payload size
+__global__ void k_dict_finish(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_chunks, uint64_t rb, const uint64_t* first,
+                              const uint64_t* esum, DictChunk* D, Page* pages) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  const LeafDev L = leaves[c % n_leaves];
+  DictChunk& K = D[c];
+  if (L.atype == ETL_ARROW_BOOLEAN) return;
+  const uint64_t i0 = L.is_list ? (uint64_t)L.loffs[rb] : rb, a = L.dscr + K.it0 - i0, b = L.dscr + K.it1 - i0;
+  K.entries = K.fallback ? 0 : first[b] - first[a];
+  K.dict = K.entries > 0;                                 // no fallback: every entry is in, and their total <= kDictBytes
+  uint32_t w = 1;
+  while (K.entries > 1 && (K.entries - 1) >> w) w++;
+  K.width = w;
+  if (K.dict) pages[K.page].usize = is_bytes(L) ? esum[b] - esum[a] : K.entries * L.fixed;
+}
+
+// 1g. ETL_PQ_DICTIONARY, one leaf, a thread per item bound: each first occurrence of a dictionary chunk writes its
+// entry, PLAIN, at its offset in the chunk's dictionary slot (byte arrays: the bytes copied by the whole warp)
+__global__ void __launch_bounds__(256) k_dict_page(const LeafDev* leaves, uint32_t l, uint32_t n_leaves, uint32_t n_rg, uint64_t rb,
+                                                   uint64_t bound, const DictChunk* D, const uint64_t* first, const uint64_t* esum,
+                                                   uint8_t* uslot_base, const uint64_t* uslot) {
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const LeafDev L = leaves[l];
+  const uint64_t i0 = L.is_list ? (uint64_t)L.loffs[rb] : rb, it = i0 + j;
+  const int lane = threadIdx.x & 31;
+  bool v = j < bound && first[L.dscr + j + 1] != first[L.dscr + j];   // a first occurrence (only of non-fallback chunks)
+  uint64_t dst = 0, boff = 0, blen = 0;
+  if (v) {
+    const DictChunk& K = D[chunk_of(D, l, n_leaves, n_rg, it)];
+    v = K.dict;
+    const uint64_t a = L.dscr + K.it0 - i0;
+    uint8_t* out = uslot_base + uslot[K.page];
+    if (v && is_bytes(L)) {
+      dst = uslot[K.page] + esum[L.dscr + j] - esum[a];
+      boff = byte_off(L, it); blen = byte_off(L, it + 1) - boff;
+      for (int b = 0; b < 4; b++) out[dst - uslot[K.page] + b] = (uint8_t)(blen >> (8 * b));
+      dst += 4;
+    } else if (v) {
+      const uint64_t o = (first[L.dscr + j] - first[a]) * L.fixed;
+      for (uint32_t k = 0; k < L.fixed; k++) out[o + k] = L.values[it * L.fixed + k];
+    }
+  }
+  if (!is_bytes(L)) return;
+  unsigned todo = __ballot_sync(0xffffffffu, v && blen);
+  while (todo) {
+    const int src = __ffs(todo) - 1;
+    todo &= todo - 1;
+    const uint64_t so = __shfl_sync(0xffffffffu, boff, src), sl = __shfl_sync(0xffffffffu, blen, src), d = __shfl_sync(0xffffffffu, dst, src);
+    for (uint64_t k = lane; k < sl; k += 32) uslot_base[d + k] = L.data[so + k];
   }
 }
 
@@ -312,18 +691,23 @@ __global__ void k_fill(const Page* pages, uint32_t n_pages, int which, uint64_t*
   dst[p] = which == 0 ? pages[p].ubound : which == 1 ? 8 + nf * snappy_bound(kFragment) : nf;
 }
 
-// a thread per page: compressed size, preamble, header, file bytes of the page
-__global__ void k_page(Page* pages, uint32_t n_pages, int snappy, const uint64_t* fbase, const uint32_t* fsize, uint64_t* fbytes) {
+// a thread per page: compressed size, preamble, header, file bytes of the page (D: ETL_PQ_DICTIONARY; the dictionary
+// slot of a chunk that is not dictionary-encoded has no bytes)
+__global__ void k_page(Page* pages, uint32_t n_pages, int snappy, const uint64_t* fbase, const uint32_t* fsize, uint64_t* fbytes,
+                       const DictChunk* D) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n_pages) return;
   Page& P = pages[p];
+  const bool dict = D && D[P.chunk].dict;
+  if (P.kind && !dict) { P.hlen = P.plen = 0; P.csize = 0; fbytes[p] = 0; return; }
   if (snappy) {
     P.plen = varint(P.usize, P.pre);
     uint64_t c = P.plen;
     for (uint64_t f = fbase[p]; f < fbase[p + 1]; f++) c += fsize[f];
     P.csize = c;
   } else P.csize = P.usize;
-  P.hlen = page_header(P.hdr, (uint32_t)P.usize, (uint32_t)P.csize, (uint32_t)(P.e1 - P.e0));
+  if (P.kind) P.hlen = dict_page_header(P.hdr, (uint32_t)P.usize, (uint32_t)P.csize, (uint32_t)D[P.chunk].entries);
+  else P.hlen = page_header(P.hdr, (uint32_t)P.usize, (uint32_t)P.csize, (uint32_t)(P.e1 - P.e0), dict ? ENC_RLE_DICTIONARY : ENC_PLAIN);
   fbytes[p] = P.hlen + P.csize;
 }
 
@@ -378,13 +762,16 @@ __device__ void write_stats(const LeafDev& L, uint64_t mn, uint64_t mx, ChunkOut
 
 // 4. a thread per chunk (row-group major): sizes, counts, statistics of its pages
 __global__ void k_chunk(const LeafDev* leaves, const Page* pages, const uint64_t* page_base, uint32_t n_chunks, const uint64_t* foff,
-                        ChunkOut* out) {
+                        ChunkOut* out, const DictChunk* D) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= n_chunks) return;
   const Page& P0 = pages[page_base[c]];
   const LeafDev L = leaves[P0.leaf];
   ChunkOut C{};
   C.offset = 4 + foff[page_base[c]];
+  const uint64_t p0 = page_base[c] + P0.kind;          // the first data page
+  C.data_offset = 4 + foff[p0]; C.data_pages = page_base[c + 1] - p0;
+  C.dict = D ? D[c].dict : 0;
   uint64_t mn = kNone, mx = kNone;
   for (uint64_t p = page_base[c]; p < page_base[c + 1]; p++) {
     const Page& P = pages[p];
@@ -455,7 +842,10 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
                           uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out) {
   // a file needs at least one column (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS has none)
   if (!a || !out || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
-  if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) || (codec != ETL_PQ_UNCOMPRESSED && codec != ETL_PQ_SNAPPY)) return ETL_ERR_INVALID_ARG;
+  const uint32_t cc = codec & 0xFFu;                  // the compression codec; ETL_PQ_DICTIONARY is the only flag bit
+  if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) || (codec & ~(0xFFu | ETL_PQ_DICTIONARY)) ||
+      (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY)) return ETL_ERR_INVALID_ARG;
+  const int dict = (codec & ETL_PQ_DICTIONARY) != 0;
   std::vector<LeafDev> hl(n_fields);
   std::vector<Leaf> meta(n_fields);
   for (uint32_t c = 0; c < n_fields; c++) {
@@ -503,7 +893,7 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   const uint32_t nL = n_fields;
   const uint32_t n_rg = (uint32_t)((n + kRowGroupRows - 1) / kRowGroupRows);
   const uint32_t n_chunks = n_rg * nL;
-  const int snappy = codec == ETL_PQ_SNAPPY;
+  const int snappy = cc == ETL_PQ_SNAPPY;
   cudaStream_t st = cudaStreamPerThread;
   etl_parquet_file* Fo = new etl_parquet_file();
   std::vector<void*> pool;
@@ -538,7 +928,7 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
         k_blk_scan64<<<1, 1024, 0, st>>>(blk, lb, d_tot + at);
         k_offsets<uint64_t><<<lb, 1024, 0, st>>>(lens, n, blk, d_pre + s * nr1 + (uint64_t)l * (n + 1));
       }
-    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr);
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
   }
   // SYNC 1: page counts, totals, required-column nulls
   std::vector<uint32_t> np(n_chunks);
@@ -556,8 +946,10 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
       *out = Fo;
       return ETL_OK;
     }
+  // ETL_PQ_DICTIONARY: every chunk of a non-Boolean leaf has a dictionary slot in front of its data pages
+  auto has_dict = [&](uint32_t l) { return dict && hl[l].atype != ETL_ARROW_BOOLEAN; };
   std::vector<uint64_t> page_base(n_chunks + 1, 0);
-  for (uint32_t c = 0; c < n_chunks; c++) page_base[c + 1] = page_base[c] + np[c];
+  for (uint32_t c = 0; c < n_chunks; c++) page_base[c + 1] = page_base[c] + np[c] + (has_dict(c % nL) ? 1 : 0);
   const uint64_t P = page_base[n_chunks];
   // bounds of every buffer from the totals
   std::vector<uint64_t> pages_of(nL, 0), lscr_base(nL + 1, 0);
@@ -567,7 +959,18 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     const uint64_t El = tot[l], NNl = tot[nL + l], Vl = tot[2 * nL + l], Pl = pages_of[l];
     const uint64_t lev = 14 * Pl + (El / 8 + Pl) * (hl[l].w + 2);
     U += (hl[l].atype == ETL_ARROW_BOOLEAN ? NNl / 8 + Pl : Vl) + (hl[l].max_def ? lev : 0) + (hl[l].max_rep ? 14 * Pl + (El / 8 + Pl) * 3 : 0);
-    (void)NNl;
+    if (has_dict(l)) U += std::min<uint64_t>(Vl, n_rg * kDictBytes) + 32 * Pl;   // the dictionary slots, the index runs
+  }
+  // dictionary scratch: per item bound (a leaf's level entries) slot, flag, entry size / index, two prefix sums; run
+  // heads per 8 items + 3 per page; the chunks' tables of at most 4 × non-null values (+ 1) slots
+  uint64_t d_items = 0, d_heads = 0, d_slots = 0, d_maxI = 0;
+  for (uint32_t l = 0; l < nL; l++) {
+    if (!has_dict(l)) continue;
+    hl[l].dscr = d_items; hl[l].hscr = d_heads;
+    d_items += tot[l] + 1;
+    d_heads += tot[l] / 8 + 3 * (pages_of[l] + 1) + 8;
+    d_slots += 4 * tot[nL + l] + n_rg;
+    d_maxI = std::max<uint64_t>(d_maxI, tot[l]);
   }
   // level scratch: per leaf 2 × (entries + 16 per page (alignment) + slack); page_base enters the per-page offset
   // level scratch of a leaf: rep | def of each page, 8-aligned, at 2 * align8(e0) + 64 * (page index within the leaf)
@@ -589,16 +992,20 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   std::vector<uint64_t> rg_rows(n_rg);
   for (uint32_t g = 0; g < n_rg; g++) rg_rows[g] = std::min<uint64_t>(kRowGroupRows, n - (uint64_t)g * kRowGroupRows);
   std::vector<Chunk> wide(n_chunks);
-  for (Chunk& k : wide) { k.offset = k.num_values = k.usize = k.csize = k.null_count = 1ull << 62; k.has_minmax = true; k.min.assign(kStatMax, 'x'); k.max.assign(kStatMax, 'x'); }
+  for (uint32_t c = 0; c < n_chunks; c++) {
+    Chunk& k = wide[c];
+    k.offset = k.num_values = k.usize = k.csize = k.null_count = 1ull << 62; k.has_minmax = true; k.min.assign(kStatMax, 'x'); k.max.assign(kStatMax, 'x');
+    if (has_dict(c % nL)) { k.dict = true; k.data_offset = 1ull << 62; k.data_pages = INT32_MAX; }
+  }
   const char* created_by = "etl-b200 parquet writer";
-  const uint64_t footer_bound = footer(meta, rg_rows, wide, codec, created_by).size() + 8;
+  const uint64_t footer_bound = footer(meta, rg_rows, wide, cc, created_by).size() + 8;
   const uint64_t data_bound = 4 + P * kPageHeaderMax + (snappy ? C_bound : U);
   Page* d_pages = (Page*)dalloc(sizeof(Page) * (P + 1));
   uint64_t* d_pbase = (uint64_t*)dalloc(16 * (n_chunks + 1ull));   // page_base | leaf_page_base
   uint64_t* d_lbase = (uint64_t*)dalloc(8 * (nL + 1ull));
   uint8_t* d_lscr = (uint8_t*)dalloc(lscr_base[nL] + 16);
   uint64_t* d_scan = (uint64_t*)dalloc(8 * 4 * (P + 1));   // uslot | cslot | fbase | file offsets, P + 1 each
-  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 4);
+  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 5);
   uint8_t* d_u = (uint8_t*)dalloc(U + 16);
   uint32_t* d_bool = (uint32_t*)dalloc(bool_words * 4 + 8);
   uint8_t* d_c = snappy ? (uint8_t*)dalloc(C_bound + 16) : nullptr;
@@ -607,6 +1014,25 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   ChunkOut* d_lout = d_cout ? (ChunkOut*)((uint8_t*)d_cout + sizeof(ChunkOut) * n_chunks + 16ull * n_chunks) : nullptr;
   if (!d_pages || !d_pbase || !d_lbase || !d_lscr || !d_scan || !d_stot || !d_u || !d_bool || !d_cout || (snappy && (!d_c || !d_fsz)))
     return fail(ETL_ERR_ALLOC);
+  DictChunk* d_dch = nullptr;
+  unsigned long long* d_tabn = nullptr;
+  unsigned long long* d_dblk = nullptr;
+  uint32_t *d_tab = nullptr, *d_dpos = nullptr, *d_dflag = nullptr, *d_desz = nullptr, *d_dhead = nullptr;
+  uint64_t *d_dfirst = nullptr, *d_desum = nullptr;
+  const uint32_t dlb = (uint32_t)((d_maxI + 1023) / 1024);
+  if (d_items && P) {
+    d_dch = (DictChunk*)dalloc(sizeof(DictChunk) * n_chunks);
+    d_tabn = (unsigned long long*)dalloc(8 * (n_chunks + 1ull));
+    d_dblk = (unsigned long long*)dalloc(8 * (dlb + 2ull));
+    d_tab = (uint32_t*)dalloc(4 * d_slots);
+    d_dpos = (uint32_t*)dalloc(4 * d_items);
+    d_dflag = (uint32_t*)dalloc(4 * d_items);
+    d_desz = (uint32_t*)dalloc(4 * d_items);
+    d_dhead = (uint32_t*)dalloc(4 * d_heads);
+    d_dfirst = (uint64_t*)dalloc(8 * d_items);
+    d_desum = (uint64_t*)dalloc(8 * d_items);
+    if (!d_dch || !d_tabn || !d_dblk || !d_tab || !d_dpos || !d_dflag || !d_desz || !d_dhead || !d_dfirst || !d_desum) return fail(ETL_ERR_ALLOC);
+  }
   if (cudaMalloc(&Fo->dev, data_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
   uint64_t* uslot = d_scan; uint64_t* cslot = d_scan + (P + 1); uint64_t* fbase = d_scan + 2 * (P + 1); uint64_t* foff = d_scan + 3 * (P + 1);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
@@ -617,24 +1043,54 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   CK(cudaMemsetAsync(d_bool, 0, bool_words * 4 + 8, st));
   CK(cudaMemsetAsync(d_lscr, 0, lscr_base[nL] + 16, st));
   if (P) {
-    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages);
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages, dict);
     // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
     auto fill_scan = [&](int which, uint64_t* dst) {
       k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, dst);
       k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)dst, (uint32_t)(P + 1), d_stot + which);
     };
     fill_scan(0, uslot);
-    k_encode<<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, E, n, d_lscr, d_u, uslot, d_bool);
+    if (d_dch) {
+      // dictionaries: tables, inserts, first-occurrence flags and their scans, decisions, dictionary pages
+      k_dict_setup<<<(n_chunks + 256) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, n, NN, d_pbase, d_dch, d_tabn);
+      k_blk_scan64<<<1, 1024, 0, st>>>(d_tabn, n_chunks + 1, d_stot + 4);
+      k_dict_place<<<(n_chunks + 255) / 256, 256, 0, st>>>(n_chunks, d_tabn, d_dch);
+      CK(cudaMemsetAsync(d_tab, 0xff, 4 * d_slots, st));
+      auto scan = [&](const uint32_t* lens, uint64_t cnt, uint64_t* dst) {
+        const uint32_t nb = (uint32_t)((cnt + 1023) / 1024);
+        k_len_blocks<<<nb, 1024, 0, st>>>(lens, cnt, d_dblk);
+        k_blk_scan64<<<1, 1024, 0, st>>>(d_dblk, nb, d_stot + 4);
+        k_offsets<uint64_t><<<nb, 1024, 0, st>>>(lens, cnt, d_dblk, dst);
+      };
+      for (uint32_t l = 0; l < nL; l++) {
+        if (!has_dict(l)) continue;
+        const uint64_t I = tot[l];
+        const uint32_t ib = (uint32_t)((I + 255) / 256);
+        k_dict_insert<<<std::min<uint32_t>(kInsBlocks, ib), kInsThreads, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, d_dch, d_tab, d_dpos);
+        const bool bytes = hl[l].atype == ETL_ARROW_UTF8 || hl[l].atype == ETL_ARROW_LARGE_BINARY;
+        k_dict_mark<<<ib, 256, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, I, d_dch, d_tab, d_dpos, d_dflag, bytes ? d_desz : nullptr);
+        scan(d_dflag + hl[l].dscr, I, d_dfirst + hl[l].dscr);
+        if (bytes) scan(d_desz + hl[l].dscr, I, d_desum + hl[l].dscr);
+      }
+      k_dict_finish<<<(n_chunks + 255) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, d_dfirst, d_desum, d_dch, d_pages);
+      for (uint32_t l = 0; l < nL; l++)
+        if (has_dict(l))
+          k_dict_page<<<(uint32_t)((tot[l] + 255) / 256), 256, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, tot[l], d_dch, d_dfirst, d_desum, d_u, uslot);
+      const DictArgs da{d_dch, d_tab, d_dpos, d_dfirst, d_desz, d_dhead};
+      k_encode<true><<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, E, n, d_lscr, d_u, uslot, d_bool, da);
+    } else {
+      k_encode<false><<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, E, n, d_lscr, d_u, uslot, d_bool, DictArgs{});
+    }
     if (snappy) {
       fill_scan(1, cslot);
       fill_scan(2, fbase);
       k_snappy<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz);
     }
-    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, snappy, fbase, d_fsz, foff);
+    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, snappy, fbase, d_fsz, foff, d_dch);
     CK(cudaMemsetAsync(foff + P, 0, 8, st));
     k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
     k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, snappy, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
-    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout);
+    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout, d_dch);
   }
   if (nL) k_leaf<<<(nL + 63) / 64, 64, 0, st>>>(d_leaves, nL, P ? n_rg : 0, d_cout, d_lout);
   // SYNC 2: chunk and leaf records
@@ -652,9 +1108,10 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   for (uint32_t c = 0; c < n_chunks; c++) {
     const ChunkOut& K = hc[c];
     chunks[c] = Chunk{K.offset, K.num_values, K.usize, K.csize, K.null_count, K.has != 0,
-                      std::string((const char*)K.min, K.min_len), std::string((const char*)K.max, K.max_len)};
+                      std::string((const char*)K.min, K.min_len), std::string((const char*)K.max, K.max_len),
+                      K.dict != 0, K.data_offset, K.data_pages};
   }
-  std::vector<uint8_t> foot = footer(meta, rg_rows, chunks, codec, created_by);
+  std::vector<uint8_t> foot = footer(meta, rg_rows, chunks, cc, created_by);
   const uint32_t flen = (uint32_t)foot.size();
   for (int b = 0; b < 4; b++) foot.push_back((uint8_t)(flen >> (8 * b)));
   for (char ch : std::string("PAR1")) foot.push_back((uint8_t)ch);
@@ -710,7 +1167,10 @@ void etl_dec_parquet_free(etl_parquet_file* f) {
 }  // extern "C"
 
 // ptxas -v, sm_90a, CUDA 12.9 (registers / shared memory / stack):
-//   k_plan 32 / 0 / 0      k_cut 54 / 0 / 0       k_encode 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 12 / 0 / 0
-//   k_snappy 50 / 8192 B / 0                      k_page 30 / 0 / 40 B (the header bytes)   k_gather 23 / 0 / 0
+//   k_plan 32 / 0 / 0      k_cut 53 / 0 / 0       k_encode<false> 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 12 / 0 / 0
+//   k_encode<true> 64 / 4200 B / 16 B (two 8-byte spills)
+//   k_snappy 50 / 8192 B / 0                      k_page 29 / 0 / 40 B (the header bytes)   k_gather 23 / 0 / 0
+//   k_dict_setup 24 / 0 / 0   k_dict_place 10 / 0 / 0   k_dict_insert 46 / 0 / 0   k_dict_mark 24 / 0 / 0
+//   k_dict_finish 22 / 0 / 0  k_dict_page 32 / 0 / 0
 //   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)
 //   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan64 32 / 8192 B, k_offsets<uint64_t> 18 / 8192 B

@@ -743,15 +743,16 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * fields: one per emitted column, in order (n_fields == etl_dec_arrow_cols).  ETL_ERR_INVALID_ARG, before any launch:
  * another n_fields or none (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS), an ETL_ARROW_UNSUPPORTED
  * column (the emit lacked ETL_ARROW_ALL_COLUMNS), row_begin > row_end or row_end > etl_dec_arrow_rows, an unknown
- * codec, a NULL or empty name or one longer than 1 KiB.
+ * codec (codec & 0xFF other than ETL_PQ_UNCOMPRESSED / ETL_PQ_SNAPPY) or a codec bit other than ETL_PQ_DICTIONARY, a NULL or
+ * empty name or one longer than 1 KiB.
  * A null in a required column (a null list of a required List column, or a null value) is data: ETL_OK with size 0 and
  * no bytes, and etl_dec_parquet_required_null gives the smallest such column and its first null row (emit row numbers)
  * — RecordBatch::try_new in rows_to_record_batch fails there before anything is written (a ConversionError in the shim).
- * The file (parity with arrow-rs bytes and defaults is not a goal: its writer adds a dictionary, a page index and an
- * ARROW:schema key; Iceberg readers resolve columns by field id and Parquet type):
+ * The file (parity with arrow-rs bytes and defaults is not a goal: its writer adds a page index and an ARROW:schema key;
+ * Iceberg readers resolve columns by field id and Parquet type):
  *   layout: "PAR1", the column chunks (row-group major, column minor, pages in row order), the footer, its 4-byte LE
  *           length, "PAR1".  Row groups of at most 1 048 576 rows in row order; zero rows: no row group.
- *   pages: data page V1, no dictionary, no CRC, no page statistics; whole rows; a page ends after the first row that
+ *   pages: data page V1, no CRC, no page statistics; whole rows; a page ends after the first row that
  *          brings it to 20 000 rows or to >= 1 MiB of PLAIN value bytes (Boolean: ceil(values / 8)), and at the row
  *          group's end.
  *   values: PLAIN, non-null only: Boolean bit-packed LSB first, INT32 / INT64 / FLOAT / DOUBLE little-endian,
@@ -774,18 +775,45 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  *          unsigned bytewise BYTE_ARRAY / UUID, false < true), NaN excluded, a zero minimum written as -0.0 and a zero
  *          maximum as +0.0; none when the chunk has no non-NaN value or a byte-array min / max is longer than 64 bytes.
  *          column_orders: TypeDefinedOrder for every leaf.
+ *   dictionary (codec | ETL_PQ_DICTIONARY; without it every chunk is PLAIN as above):
+ *          eligible leaves: every leaf but Boolean (a List column's leaf is its element); each column chunk (one leaf in
+ *          one row group) has its own dictionary.  Entries: the distinct PLAIN byte strings of the chunk's non-null
+ *          values (fixed width: the little-endian value; Uuid: the 16 bytes; byte arrays: the bytes), floats compared
+ *          bitwise (+0.0 and -0.0 are two entries, NaNs with equal bits one), in order of first occurrence in item order
+ *          (the order of arrow-rs's interner), independent of thread scheduling.  Decision per chunk: its dictionary size
+ *          is the sum of the entries' PLAIN sizes (byte arrays 4 + length); the chunk is dictionary-encoded iff it has a
+ *          non-null value and that size is <= 1 048 576 bytes, else it is written PLAIN, byte for byte as without the
+ *          flag, wherever it lands (a whole-chunk decision: arrow-rs falls back in the middle of a chunk instead).  A
+ *          file in which no chunk qualifies is the file written without the flag.
+ *          Dictionary page, first in the chunk: PageHeader {type DICTIONARY_PAGE (2), uncompressed / compressed size,
+ *          dictionary_page_header (7) {num_values = entries, encoding PLAIN}}; payload the entries PLAIN in dictionary
+ *          order, compressed as a data page is.  Data pages: the page cuts above, still on PLAIN bytes (arrow-rs cuts on
+ *          encoded size); header encoding RLE_DICTIONARY (8); payload the level sections as above, one byte of bit width
+ *          max(1, bits(entries - 1)) (<= 18: 1 MiB / 4-byte entries bounds entries by 262 144), then the RLE / bit-packed
+ *          hybrid of the page's non-null indices without a length prefix, under the run rule of the levels (groups of 8,
+ *          uniform groups of one value one RLE run of their exact count with the value in ceil(width / 8) LE bytes,
+ *          other stretches bit-packed runs of at most 63 groups, LSB first, the last group zero-padded); a page without a
+ *          non-null value has only the bit-width byte.
+ *          Footer of a dictionary chunk: encodings [PLAIN, RLE (with levels), RLE_DICTIONARY], data_page_offset the first
+ *          data page, dictionary_page_offset (11) and ColumnChunk / RowGroup file_offset the dictionary page,
+ *          encoding_stats (13) [{DICTIONARY_PAGE, PLAIN, 1}, {DATA_PAGE, RLE_DICTIONARY, data pages}].  Statistics and
+ *          the metrics' counts and bounds are those of the values, as without the flag.  ColumnMetaData.codec is
+ *          codec & 0xFF.
  *   footer: Thrift compact, ascending field ids: FileMetaData {version 1, schema, num_rows, row_groups, created_by,
  *          column_orders}, SchemaElement {type, type_length, repetition_type, name, num_children, converted_type,
  *          field_id, logicalType}, RowGroup {columns, total_byte_size, num_rows, file_offset, total_compressed_size,
  *          ordinal}, ColumnChunk {file_offset, meta_data}, ColumnMetaData {type, encodings (PLAIN, + RLE with levels),
  *          path_in_schema, codec, num_values, total_uncompressed_size, total_compressed_size, data_page_offset,
- *          statistics}.
+ *          [dictionary_page_offset,] statistics[, encoding_stats]}.
  * Metrics: one record per leaf (a List column's leaf is its element), over every row group of the file; min / max are
  * the PLAIN statistic bytes, which equal Iceberg's single-value serialization of these types (before truncation).
  * to_host: also copy the file to pinned host memory (etl_dec_parquet_bytes(f, 1); else NULL).  Scratch, beside the
  * file: 36 B per (row, column), 2 B per level entry + 64 B per page, 1 bit per Boolean value, a payload slot per page (values +
- * level bound) and with Snappy a compressed slot per 64 KiB of payload. */
+ * level bound) and with Snappy a compressed slot per 64 KiB of payload; with ETL_PQ_DICTIONARY also 28 B per item of an
+ * eligible leaf (bounded by its level entries) + 0.5 B per item of run heads, a dictionary slot per chunk of at most
+ * 1 MiB, 32 B per data page, and hash tables of at most 16 B per non-null value. */
 enum { ETL_PQ_UNCOMPRESSED = 0, ETL_PQ_SNAPPY = 1 };
+#define ETL_PQ_DICTIONARY 0x100u   /* OR-ed into codec: dictionary-encode the eligible column chunks (codec & 0xFF: compression) */
 #define ETL_PQ_HAS_MIN_MAX 1u   /* etl_parquet_metrics.flags: min / max are set */
 typedef struct etl_parquet_field {
   const char* name;           /* UTF-8 column name, written verbatim into the Parquet schema */
@@ -800,7 +828,7 @@ typedef struct etl_parquet_metrics {   /* one per leaf (= per column; a List col
   uint64_t num_values;        /* level entries (Parquet num_values), summed over row groups */
   uint64_t null_count;        /* entries whose definition level < max */
   uint64_t nan_count;         /* Float / Double leaves only */
-  uint64_t compressed_bytes;  /* column-chunk bytes including page headers, summed over row groups */
+  uint64_t compressed_bytes;  /* column-chunk bytes including page headers (and dictionary pages), summed over row groups */
   uint64_t uncompressed_bytes;
   const uint8_t* min; uint32_t min_len;   /* host memory, PLAIN-encoded statistic bytes, valid until free */
   const uint8_t* max; uint32_t max_len;

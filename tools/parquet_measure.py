@@ -2,6 +2,7 @@
 """Time the Iceberg Parquet writer (etl_dec_parquet_write) on resident Arrow emits, against pyarrow's CPU writer.
 
   python tools/parquet_measure.py [--copy-rows 1000000] [--c3-scale 1] [--c4-scale 0.1] [--reps 7] [--warmup 2]
+                                  [--plain-only] [--no-pyarrow] [--tag NAME]
 
 Workloads: bench.py's 10-column COPY table, C3 (one schema version) and C4 (every schema version: times and sizes are
 sums over the versions), each emitted once with 7 | ETL_ARROW_ALL_COLUMNS | ETL_ARROW_CDC_COLUMNS and kept in HBM.
@@ -10,8 +11,11 @@ to_host 0:
   * write_ms_uncompressed / write_ms_snappy: the whole call, file in HBM;
   * snappy_GBps: page payload bytes before compression / the median Snappy call;
   * file_bytes_* and the pyarrow baseline: pyarrow.parquet.write_table(compression="snappy") with its defaults
-    (dictionary encoding on) over the same columns on the host, into memory — its time and file size show what the
-    device writer's missing dictionary costs in bytes.
+    (dictionary encoding on) over the same columns on the host, into memory;
+  * the dictionary leg (codec | ETL_PQ_DICTIONARY): write_ms_dict_* and file_bytes_dict_*, uncompressed and Snappy.
+A low-cardinality COPY table (status text of a dozen values, small int codes, dates, uuids from a pool of nine and a
+text[] of three tags) runs beside the COPY table.  --plain-only skips the dictionary leg, so that a library without
+ETL_PQ_DICTIONARY can be timed by the same script (ETL_LIB_SUFFIX selects it); --tag labels the lines.
 Prints the card name and power limit in the same run.
 """
 import argparse
@@ -63,9 +67,13 @@ def to_arrow(col):
     return pa.Array.from_buffers(PA_TYPE[t], n, [mask, pa.py_buffer(np.ascontiguousarray(col["values"]).tobytes())])
 
 
+OPTS = dict(plain_only=False, pyarrow=True)
+
+
 def measure_emits(lib, emits, reps, warmup):
     """emits: Arrow batch handles of one workload; sums over them"""
     t0, t1, tp, sizes, payload, rows = [], [], [], [0, 0, 0], 0, 0
+    td, dsizes = {abi.PQ_UNCOMPRESSED: [], abi.PQ_SNAPPY: []}, [0, 0]
     for a in emits:
         cols = emit_columns(lib, a)
         fields = fields_for(cols)
@@ -82,6 +90,16 @@ def measure_emits(lib, emits, reps, warmup):
                     lib.etl_dec_parquet_metrics(h, l, C.byref(m))
                     payload += m.uncompressed_bytes
             lib.etl_dec_parquet_free(h)
+            if OPTS["plain_only"]:
+                continue
+            dc = codec | abi.PQ_DICTIONARY
+            td[codec].append(timed(lambda: lib.etl_dec_parquet_free(pq_write(lib, a, fields, 0, n, dc, 0)[1]), reps, warmup))
+            rc, h = pq_write(lib, a, fields, 0, n, dc, 0)
+            assert rc == 0
+            dsizes[codec] += lib.etl_dec_parquet_size(h)
+            lib.etl_dec_parquet_free(h)
+        if not OPTS["pyarrow"]:
+            continue
         table = pa.table({f[0]: to_arrow(c) for c, f in zip(cols, fields)})
         sink = io.BytesIO()
         pq.write_table(table, sink, compression="snappy")
@@ -91,14 +109,33 @@ def measure_emits(lib, emits, reps, warmup):
             pq.write_table(table, io.BytesIO(), compression="snappy")
         tp.append(timed(cpu, max(3, reps // 2), 1))
     s1 = sum_stats(t1)
-    return dict(rows=int(rows), write_ms_uncompressed=sum_stats(t0), write_ms_snappy=s1,
-                snappy_GBps=round(payload / (s1["median"] * 1e-3) / 1e9, 2) if s1["median"] else None,
-                file_bytes_uncompressed=int(sizes[0]), file_bytes_snappy=int(sizes[1]),
-                pyarrow_snappy_ms=sum_stats(tp), pyarrow_file_bytes=int(sizes[2]))
+    out = dict(rows=int(rows), write_ms_uncompressed=sum_stats(t0), write_ms_snappy=s1,
+               snappy_GBps=round(payload / (s1["median"] * 1e-3) / 1e9, 2) if s1["median"] else None,
+               file_bytes_uncompressed=int(sizes[0]), file_bytes_snappy=int(sizes[1]))
+    if OPTS["pyarrow"]:
+        out.update(pyarrow_snappy_ms=sum_stats(tp), pyarrow_file_bytes=int(sizes[2]))
+    if not OPTS["plain_only"]:
+        out.update(write_ms_dict_uncompressed=sum_stats(td[abi.PQ_UNCOMPRESSED]), write_ms_dict_snappy=sum_stats(td[abi.PQ_SNAPPY]),
+                   file_bytes_dict_uncompressed=int(dsizes[0]), file_bytes_dict_snappy=int(dsizes[1]))
+    return out
 
 
-def copy_table(n_rows, reps, warmup):
-    oids, rows = bench_copy_table(n_rows)
+def low_cardinality_rows(n_rows):
+    """(oids, COPY rows) of the low-cardinality table, seeded"""
+    rng = np.random.default_rng(29)
+    words = ["active", "pending", "shipped", "cancelled", "returned", "on hold", "lost", "refunded", "draft", "open",
+             "closed", "archived"]
+    uuids = ["%08x-0000-4000-8000-%012x" % (k * 7919, k) for k in range(9)]
+    w, code, day, u, nt = (rng.integers(0, 12, n_rows), rng.integers(0, 7, n_rows), rng.integers(1, 29, n_rows),
+                           rng.integers(0, 9, n_rows), rng.integers(0, 4, n_rows))
+    tags = ["{}", "{red}", "{red,green}", "{blue,green,red}"]
+    rows = [("%d\t%s\t%d\t2024-03-%02d\t%s\t%s\n" % (r, words[w[r]], code[r], day[r], uuids[u[r]], tags[nt[r]])).encode()
+            for r in range(n_rows)]
+    return [23, 25, 23, 1082, 2950, 1009], rows
+
+
+def copy_table(n_rows, reps, warmup, tag, low_card=False):
+    oids, rows = low_cardinality_rows(n_rows) if low_card else bench_copy_table(n_rows)
     lib = abi.load()
     blob = b"".join(rows)
     offs = np.zeros(len(rows) + 1, dtype=np.uint64)
@@ -116,14 +153,15 @@ def copy_table(n_rows, reps, warmup):
     with decoder.BatchHandle(dec, h) as bh:
         a = C.c_void_p()
         assert lib.etl_dec_arrow_emit(bh._h, 0, KINDS, 1, C.byref(a)) == 0
-        res = dict(workload="bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
+        res = dict(tag=tag, workload="low-cardinality COPY table (int4, text, int4, date, uuid, text[])" if low_card
+                   else "bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
         res.update(measure_emits(lib, [a], reps, warmup))
         lib.etl_dec_arrow_free(a)
         print(json.dumps(res), flush=True)
     dec.close()
 
 
-def streaming(name, scale, reps, warmup):
+def streaming(name, scale, reps, warmup, tag):
     w = wl.make(name, scale, n_segments=1)
     stream, stats = w.generate()
     st = decoder.Stager(stream.nbytes, 2048)
@@ -132,7 +170,7 @@ def streaming(name, scale, reps, warmup):
     for tid, cols in w.table_schemas().items():
         dec.put_table_schema(tid, cols)
     lib = abi.load()
-    res = dict(workload=name, scale=scale, stream_bytes=int(stream.nbytes))
+    res = dict(tag=tag, workload=name, scale=scale, stream_bytes=int(stream.nbytes))
     with dec.decode_input(st.view(), to_host=False) as bh:
         emits = []
         for si in range(bh.summary().n_schemas):
@@ -154,14 +192,20 @@ def main():
     ap.add_argument("--c4-scale", type=float, default=0.1)
     ap.add_argument("--reps", type=int, default=7)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--plain-only", action="store_true")
+    ap.add_argument("--no-pyarrow", action="store_true")
+    ap.add_argument("--tag", default="")
     a = ap.parse_args()
+    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow)
     if not torch.cuda.is_available():
         raise SystemExit("parquet_measure needs a CUDA device")
     t = time.time()
     print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
-    copy_table(a.copy_rows, a.reps, a.warmup)
+    copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
+    if not a.plain_only:
+        copy_table(a.copy_rows, a.reps, a.warmup, a.tag, low_card=True)
     for name, scale in (("c3", a.c3_scale), ("c4", a.c4_scale)):
-        streaming(name, scale, a.reps, a.warmup)
+        streaming(name, scale, a.reps, a.warmup, a.tag)
     print(json.dumps(dict(wall_s=round(time.time() - t, 1))), flush=True)
 
 
