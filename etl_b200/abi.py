@@ -283,6 +283,8 @@ PQ_UNCOMPRESSED, PQ_SNAPPY = 0, 1
 PQ_HAS_MIN_MAX = 1
 # codec bit: dictionary-encode the eligible column chunks (ETL_PQ_DICTIONARY)
 PQ_DICTIONARY = 0x100
+# codec bit: write a ColumnIndex and an OffsetIndex per column chunk (ETL_PQ_PAGE_INDEX)
+PQ_PAGE_INDEX = 0x400
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

@@ -15,8 +15,11 @@
 //     the RLE / bit-packed hybrid of dictionary indices (bit width 1..18) under the same run rule as the levels, split
 //     into the run classification and the writing of one run, so that the CTA-parallel encoder of parquet_write.cu and
 //     the serial indices_encode below share them;
-//   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders, and
-//     for a dictionary chunk its dictionary_page_offset and encoding_stats.
+//   * the page index pieces (ETL_PQ_PAGE_INDEX): the 64-byte truncation of byte-array ColumnIndex bounds, the
+//     PageLocation of the OffsetIndex and the header of a list field;
+//   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders, for
+//     a dictionary chunk its dictionary_page_offset and encoding_stats, and with a page index the ColumnChunk's offset
+//     and length of its OffsetIndex and ColumnIndex.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -212,6 +215,80 @@ __host__ __device__ inline uint64_t indices_encode(const uint32_t* x, uint64_t n
 // or 4 as (part of) an RLE run
 __host__ __device__ inline uint64_t indices_bound(uint64_t n) { return 1 + ((n + 7) / 8) * 19; }
 
+// ------------------------------------------------------------------------------------------------ page index
+// ColumnIndex bounds of a byte-array value v[0, len) (arrow-rs's truncate_min_value / truncate_max_value with
+// column_index_truncate_length 64; utf8: v is valid UTF-8).  Each writes the bound to out unless it is nullptr and
+// returns its length.  A value of at most 64 bytes is its own bound.
+constexpr uint32_t kIndexTruncate = 64;
+// minimum: the first 64 bytes; Utf8: the longest prefix of at most 64 bytes that ends on a character boundary
+__host__ __device__ inline uint64_t index_min(const uint8_t* v, uint64_t len, bool utf8, uint8_t* out) {
+  uint64_t k = len;
+  if (len > kIndexTruncate) {
+    k = kIndexTruncate;
+    if (utf8) while (k > 1 && (v[k] & 0xC0u) == 0x80u) k--;   // v[k] starts the character after the prefix
+  }
+  if (out) for (uint64_t i = 0; i < k; i++) out[i] = v[i];
+  return k;
+}
+// maximum: the first 64 bytes with the last byte incremented, 0xFF carrying into the byte before it as 0x00; Utf8: the
+// prefix up to the last character boundary at most 64, cut after its last character whose code point + 1 is a Unicode
+// scalar value of the same UTF-8 length, that character incremented.  Nothing to increment: the value itself.
+__host__ __device__ inline uint64_t index_max(const uint8_t* v, uint64_t len, bool utf8, uint8_t* out) {
+  if (len > kIndexTruncate && !utf8) {
+    int64_t j = kIndexTruncate - 1;
+    while (j >= 0 && v[j] == 0xFFu) j--;
+    if (j >= 0) {
+      if (out) {
+        for (int64_t i = 0; i < j; i++) out[i] = v[i];
+        out[j] = (uint8_t)(v[j] + 1);
+        for (uint32_t i = (uint32_t)j + 1; i < kIndexTruncate; i++) out[i] = 0;
+      }
+      return kIndexTruncate;
+    }
+  } else if (len > kIndexTruncate) {
+    uint64_t end = kIndexTruncate;
+    while (end > 0 && (v[end] & 0xC0u) == 0x80u) end--;
+    while (end > 0) {                                   // the characters of v[0, end), last first
+      uint64_t s = end - 1;
+      while (s > 0 && (v[s] & 0xC0u) == 0x80u) s--;
+      const uint32_t l = (uint32_t)(end - s);
+      uint32_t cp = l == 1 ? v[s] : v[s] & (0x7Fu >> l);
+      for (uint32_t i = 1; i < l; i++) cp = (cp << 6) | (v[s + i] & 0x3Fu);
+      const uint32_t nx = cp + 1;
+      const uint32_t nl = nx < 0x80u ? 1 : nx < 0x800u ? 2 : nx < 0x10000u ? 3 : 4;
+      if (nx <= 0x10FFFFu && (nx < 0xD800u || nx > 0xDFFFu) && nl == l) {
+        if (out) {
+          for (uint64_t i = 0; i < s; i++) out[i] = v[i];
+          if (l == 1) out[s] = (uint8_t)nx;
+          else {
+            out[s] = (uint8_t)((0xF00u >> l) | (nx >> (6 * (l - 1))));   // 110xxxxx / 1110xxxx / 11110xxx
+            for (uint32_t i = 1; i < l; i++) out[s + i] = (uint8_t)(0x80u | ((nx >> (6 * (l - 1 - i))) & 0x3Fu));
+          }
+        }
+        return end;
+      }
+      end = s;
+    }
+  }
+  if (out) for (uint64_t i = 0; i < len; i++) out[i] = v[i];
+  return len;
+}
+// PageLocation {1 offset: i64, 2 compressed_page_size: i32, 3 first_row_index: i64}; at most 29 bytes
+__host__ __device__ inline uint32_t page_location(uint8_t* out, uint64_t offset, uint32_t size, uint64_t first_row) {
+  TWriter w(out);
+  w.i64(1, (int64_t)offset);
+  w.i32(2, (int32_t)size);
+  w.i64(3, (int64_t)first_row);
+  w.end();
+  return (uint32_t)w.n;
+}
+// the header of a list field whose id follows the previous field's (one byte) and its size; returns its length
+__host__ __device__ inline uint32_t list_field(uint8_t* out, uint8_t elem_type, uint32_t size) {
+  TWriter w(out);
+  w.list(1, elem_type, size);
+  return (uint32_t)w.n;
+}
+
 // ------------------------------------------------------------------------------------------------ Snappy
 __host__ __device__ inline uint32_t load32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
 __host__ __device__ inline uint32_t snappy_hash(uint32_t v) { return (v * 0x1e35a7bdu) >> (32 - kSnappyHashBits); }
@@ -294,6 +371,9 @@ struct Chunk {
   bool dict = false;                // dictionary chunk: its data pages are RLE_DICTIONARY
   uint64_t data_offset = 0;         // dictionary chunk: the first data page
   uint64_t data_pages = 0;          // dictionary chunk: its data pages
+  bool page_index = false;          // ETL_PQ_PAGE_INDEX: the chunk's OffsetIndex and, when ci_len, its ColumnIndex
+  uint64_t ci_offset = 0, oi_offset = 0;
+  uint32_t ci_len = 0, oi_len = 0;
 };
 
 inline void schema_element(TWriter& w, const Leaf& L, bool element) {
@@ -394,6 +474,11 @@ inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::v
           w.list_struct_begin(); w.i32(1, PAGE_DATA); w.i32(2, ENC_RLE_DICTIONARY); w.i32(3, (int32_t)C.data_pages); w.end();
         }
         w.end();
+        if (C.page_index) {                            // ColumnChunk offset_index_offset / _length, column_index_*
+          w.i64(4, (int64_t)C.oi_offset);
+          w.i32(5, (int32_t)C.oi_len);
+          if (C.ci_len) { w.i64(6, (int64_t)C.ci_offset); w.i32(7, (int32_t)C.ci_len); }
+        }
         w.end();
       }
       w.i64(2, (int64_t)tu);

@@ -31,6 +31,12 @@
 //      per page, copies header + payload (+ fragments) into the file buffer, whose size is the sum of the bounds.
 //   4. Statistics.  k_chunk, a thread per (leaf, row group), folds the page candidates and sizes of its chunk, k_leaf the
 //      chunks of a leaf; both write the PLAIN bytes of min / max (−0.0 / +0.0 for a zero float, none above 64 bytes).
+//   4b. Page index (ETL_PQ_PAGE_INDEX).  k_index<false>, a warp per chunk with lanes over its data pages: each page's
+//      ColumnIndex entry (null flag, bounds truncated by index_min / index_max, null count) and PageLocation sizes, the
+//      boundary order from adjacent non-null pages' untruncated bounds, the chunk's ColumnIndex / OffsetIndex lengths;
+//      one k_blk_scan64 over the 2 × chunks lengths places them behind 4 + data_end (read on the device);
+//      k_index<true> writes them and their offsets into the chunk records.  k_row_max (before SYNC 1) bounds an
+//      untruncated byte-array maximum by the leaf's longest row.
 //      SYNC 2 copies the chunk and leaf records back.
 //   5. Footer, on the host from those records (parquet_format.cuh), copied behind the pages with its length and "PAR1".
 //      SYNC 3 ends the call (and the copy to pinned host memory with to_host).
@@ -39,7 +45,9 @@
 // with Snappy, a compressed slot of snappy_bound per fragment.  ETL_PQ_DICTIONARY adds, per item of an eligible leaf
 // (bounded by its level entries), 4 B slot + 4 B flag + 4 B entry size / index + 2 × 8 B prefix sums and 0.5 B of run
 // heads (+ 12 B per page), the chunks' tables (4 B × pow2 >= 2 × non-null values: at most 16 B per value), a dictionary
-// slot per chunk (at most 1 MiB, at most the chunk's PLAIN bytes) and 32 B more per data page slot.
+// slot per chunk (at most 1 MiB, at most the chunk's PLAIN bytes) and 32 B more per data page slot.  ETL_PQ_PAGE_INDEX
+// adds 4 B per leaf, 40 B of IndexChunk + 16 B of lengths per chunk, and in the file's buffer 189 B per page + 64 B per
+// chunk (+ for a byte-array leaf with a row over 64 bytes, its longest row per page, at most its value bytes).
 // ptxas -v (sm_90a, CUDA 12.9): see the comment at the end of this file.
 #include <cuda_runtime.h>
 
@@ -89,6 +97,8 @@ struct ChunkOut {
   uint64_t data_offset, data_pages;   // the first data page and the data pages (they differ from offset with a dictionary)
   uint32_t has, min_len, max_len, dict;
   uint8_t min[kStatMax], max[kStatMax];
+  uint64_t ci_offset, oi_offset;      // ETL_PQ_PAGE_INDEX: file offsets of the chunk's ColumnIndex (ci_len 0: none) and
+  uint32_t ci_len, oi_len;            // OffsetIndex
 };
 constexpr uint64_t kNone = ~0ull;
 // ETL_PQ_DICTIONARY: one record per chunk (Boolean chunks have none: dict stays 0)
@@ -170,6 +180,15 @@ __global__ void __launch_bounds__(256) k_plan(const LeafDev* leaves, uint64_t rb
     b += is_bytes(L) ? 4 + byte_off(L, k + 1) - byte_off(L, k) : L.fixed;
   }
   ent[at] = e; nn[at] = c; vb[at] = (uint32_t)(L.atype == ETL_ARROW_BOOLEAN ? c : b);
+}
+
+// 1'. ETL_PQ_PAGE_INDEX, per (row, leaf) of a byte-array leaf: the largest PLAIN row bytes of the leaf, which bound an
+// untruncated ColumnIndex maximum
+__global__ void __launch_bounds__(256) k_row_max(const LeafDev* leaves, uint64_t n, const uint32_t* vb, unsigned int* vmax) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (!is_bytes(leaves[blockIdx.y])) return;
+  const unsigned m = __reduce_max_sync(0xffffffffu, i < n ? vb[(uint64_t)blockIdx.y * (n + 1) + i] : 0u);
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(vmax + blockIdx.y, m);
 }
 
 // 1b. a thread per (leaf, row group): greedy page cuts.  pages == nullptr: count into n_pages[chunk]
@@ -804,6 +823,139 @@ __global__ void k_leaf(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, 
   out[l] = C;
 }
 
+// ETL_PQ_PAGE_INDEX: the ColumnIndex bound of present, non-NaN item it: its statistic bytes, a byte array's truncated
+// to 64 bytes (index_min / index_max); out == nullptr counts.  Returns its length.
+__device__ uint64_t index_bound(const LeafDev& L, uint64_t it, bool is_max, uint8_t* out) {
+  if (is_bytes(L)) {
+    const uint64_t a = byte_off(L, it), len = byte_off(L, it + 1) - a;
+    const bool utf8 = L.atype == ETL_ARROW_UTF8;
+    return is_max ? index_max(L.data + a, len, utf8, out) : index_min(L.data + a, len, utf8, out);
+  }
+  uint8_t b[16];
+  uint32_t len = 0;
+  stat_bytes(L, it, is_max, b, &len);
+  if (out) for (uint32_t k = 0; k < len; k++) out[k] = b[k];
+  return len;
+}
+__device__ __forceinline__ uint64_t warp_excl(uint64_t x, uint64_t* total) {
+  const int lane = threadIdx.x & 31;
+  uint64_t s = x;
+  for (int d = 1; d < 32; d <<= 1) { const uint64_t y = __shfl_up_sync(0xffffffffu, s, d); if (lane >= d) s += y; }
+  *total = __shfl_sync(0xffffffffu, s, 31);
+  return s - x;
+}
+// ETL_PQ_PAGE_INDEX: one record per chunk, from k_index<false> to k_index<true>
+struct IndexChunk {
+  uint64_t s_min, s_max, s_nc, s_loc;   // bytes of the min_values / max_values / null_counts entries, of the PageLocations
+  uint32_t order, has_ci;               // BoundaryOrder; a ColumnIndex (no page with values that are all NaN)
+};
+constexpr uint32_t kIdxWarps = 4;
+// 4b. ETL_PQ_PAGE_INDEX, a warp per chunk (row-group major), lanes over its data pages (the dictionary page is not
+// listed).  kWrite false: each page's entry sizes, the boundary order (each non-null page against the previous one, on
+// the untruncated bounds) and the lengths of the chunk's ColumnIndex (lens[c], 0 when it has none) and OffsetIndex
+// (lens[n_chunks + c]); lens[2 n_chunks] = 0, so that their exclusive scan places them behind the pages.  kWrite true:
+// both structures at 4 + data_end + lens[...], and their offsets and lengths into the chunk's record.
+template <bool kWrite>
+__global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves, const Page* pages, const uint64_t* page_base,
+                                                         uint32_t n_chunks, uint32_t n_leaves, const uint64_t* foff, IndexChunk* X,
+                                                         unsigned long long* lens, const unsigned long long* data_end,
+                                                         uint8_t* file, ChunkOut* out) {
+  const uint32_t c = blockIdx.x * kIdxWarps + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (c >= n_chunks) {
+    if (!kWrite && c == n_chunks && lane == 0) lens[2 * n_chunks] = 0;
+    return;
+  }
+  const uint64_t pb = page_base[c];
+  const LeafDev L = leaves[pages[pb].leaf];
+  const uint64_t p0 = pb + pages[pb].kind, k = page_base[c + 1] - p0;
+  const uint64_t g0 = (uint64_t)(c / n_leaves) * kRowGroupRows;
+  const uint32_t lk = list_field(nullptr, TT_BINARY, (uint32_t)k);   // a list field's header
+  IndexChunk I{};
+  uint8_t* ci = nullptr;
+  uint8_t* oi = nullptr;
+  uint64_t o_min = 0, o_max = 0, o_nc = 0;                // kWrite: where the sections' entries start
+  if (kWrite) {
+    I = X[c];
+    const uint64_t base = 4 + *data_end;                  // lens: the exclusive scan of the lengths
+    ci = file + base + lens[c];
+    oi = file + base + lens[n_chunks + c];
+    o_min = lk + k + lk; o_max = o_min + I.s_min + lk; o_nc = o_max + I.s_max + 2 + lk;
+    if (lane == 0) {
+      ChunkOut& C = out[c];
+      C.ci_len = I.has_ci ? (uint32_t)(o_nc + I.s_nc + 1) : 0;
+      C.ci_offset = I.has_ci ? base + lens[c] : 0;
+      C.oi_offset = base + lens[n_chunks + c];
+      C.oi_len = (uint32_t)(lk + I.s_loc + 1);
+      if (I.has_ci) {
+        list_field(ci, TT_TRUE, (uint32_t)k);             // null_pages: list<bool>, one byte per element
+        list_field(ci + lk + k, TT_BINARY, (uint32_t)k);  // min_values
+        list_field(ci + o_min + I.s_min, TT_BINARY, (uint32_t)k);   // max_values
+        ci[o_max + I.s_max] = (1u << 4) | TT_I32;         // boundary_order
+        ci[o_max + I.s_max + 1] = (uint8_t)zigzag(I.order);
+        list_field(ci + o_max + I.s_max + 2, TT_I64, (uint32_t)k);  // null_counts
+        ci[o_nc + I.s_nc] = 0;
+      }
+      list_field(oi, TT_STRUCT, (uint32_t)k);             // page_locations
+      oi[lk + I.s_loc] = 0;
+    }
+  }
+  bool asc = true, desc = true, nan_only = false;
+  uint64_t s_min = 0, s_max = 0, s_nc = 0, s_loc = 0, prev = kNone;
+  for (uint64_t j0 = 0; j0 < k; j0 += 32) {
+    const uint64_t j = j0 + lane, p = p0 + (j < k ? j : 0);
+    const bool in = j < k;
+    const Page& P = pages[p];
+    const bool nonnull = in && P.nn;
+    const bool bounded = nonnull && P.min_it != kNone;
+    if (nonnull && !bounded) nan_only = true;
+    // the previous non-null page: a lane below in this tile, or the last one before it
+    const unsigned m = __ballot_sync(0xffffffffu, bounded), below = m & ((1u << lane) - 1u);
+    const uint64_t q = below ? p0 + j0 + (31 - __clz(below)) : prev;
+    if (bounded && q != kNone) {
+      const Page& Q = pages[q];
+      const int a = cmp_items(L, P.min_it, Q.min_it), b = cmp_items(L, P.max_it, Q.max_it);
+      if (a < 0 || b < 0) asc = false;
+      if (a > 0 || b > 0) desc = false;
+    }
+    if (m) prev = p0 + j0 + (31 - __clz(m));
+    const uint64_t mnl = bounded ? index_bound(L, P.min_it, false, nullptr) : 0;
+    const uint64_t mxl = bounded ? index_bound(L, P.max_it, true, nullptr) : 0;
+    const uint64_t nc = in ? (P.e1 - P.e0) - P.nn : 0;
+    const uint64_t off = 4 + foff[p], first = P.row0 - g0;
+    const uint32_t fsz = (uint32_t)(foff[p + 1] - foff[p]);
+    uint64_t t_min, t_max, t_nc, t_loc;
+    const uint64_t x_min = warp_excl(in ? varint(mnl, nullptr) + mnl : 0, &t_min);
+    const uint64_t x_max = warp_excl(in ? varint(mxl, nullptr) + mxl : 0, &t_max);
+    const uint64_t x_nc = warp_excl(in ? varint(zigzag((int64_t)nc), nullptr) : 0, &t_nc);
+    const uint64_t x_loc = warp_excl(in ? page_location(nullptr, off, fsz, first) : 0, &t_loc);
+    if (kWrite && in) {
+      if (I.has_ci) {
+        ci[lk + j] = nonnull ? TT_FALSE : TT_TRUE;         // null_pages[j]: 0x01 true, 0x02 false
+        uint8_t* d = ci + o_min + s_min + x_min;
+        d += varint(mnl, d);
+        if (bounded) index_bound(L, P.min_it, false, d);
+        d = ci + o_max + s_max + x_max;
+        d += varint(mxl, d);
+        if (bounded) index_bound(L, P.max_it, true, d);
+        varint(zigzag((int64_t)nc), ci + o_nc + s_nc + x_nc);
+      }
+      page_location(oi + lk + s_loc + x_loc, off, fsz, first);
+    }
+    s_min += t_min; s_max += t_max; s_nc += t_nc; s_loc += t_loc;
+  }
+  if (kWrite) return;
+  asc = __all_sync(0xffffffffu, asc); desc = __all_sync(0xffffffffu, desc); nan_only = __any_sync(0xffffffffu, nan_only);
+  if (lane == 0) {
+    I.s_min = s_min; I.s_max = s_max; I.s_nc = s_nc; I.s_loc = s_loc;
+    I.order = asc ? 1 : desc ? 2 : 0;                       // ASCENDING, DESCENDING, UNORDERED
+    I.has_ci = !nan_only;
+    X[c] = I;
+    lens[c] = I.has_ci ? (lk + k) + (lk + s_min) + (lk + s_max) + 2 + (lk + s_nc) + 1 : 0;
+    lens[n_chunks + c] = lk + s_loc + 1;
+  }
+}
+
 uint32_t parquet_type(uint32_t at) {
   switch (at) {
     case ETL_ARROW_BOOLEAN: return PT_BOOLEAN;
@@ -842,10 +994,12 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
                           uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out) {
   // a file needs at least one column (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS has none)
   if (!a || !out || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
-  const uint32_t cc = codec & 0xFFu;                  // the compression codec; ETL_PQ_DICTIONARY is the only flag bit
-  if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) || (codec & ~(0xFFu | ETL_PQ_DICTIONARY)) ||
-      (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY)) return ETL_ERR_INVALID_ARG;
+  const uint32_t cc = codec & 0xFFu;                  // the compression codec; the flag bits are ETL_PQ_DICTIONARY and
+  if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) ||   // ETL_PQ_PAGE_INDEX
+      (codec & ~(0xFFu | ETL_PQ_DICTIONARY | ETL_PQ_PAGE_INDEX)) || (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY))
+    return ETL_ERR_INVALID_ARG;
   const int dict = (codec & ETL_PQ_DICTIONARY) != 0;
+  const int pidx = (codec & ETL_PQ_PAGE_INDEX) != 0;
   std::vector<LeafDev> hl(n_fields);
   std::vector<Leaf> meta(n_fields);
   for (uint32_t c = 0; c < n_fields; c++) {
@@ -908,11 +1062,13 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   const uint32_t lb = (uint32_t)((n + 1023) / 1024);
   unsigned long long* d_blk = (unsigned long long*)dalloc(3ull * nL * (lb + 1) * 8);
   unsigned long long* d_tot = (unsigned long long*)dalloc(3ull * nL * 8);
-  unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull);
+  unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull + 4ull * nL);   // | ETL_PQ_PAGE_INDEX: k_row_max
   uint32_t* d_np = (uint32_t*)dalloc(n_chunks * 4ull);
   if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np) return fail(ETL_ERR_ALLOC);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_req, 0xff, nL * 8ull, st));
+  unsigned int* d_vmax = (unsigned int*)(d_req + nL);
+  if (pidx) CK(cudaMemsetAsync(d_vmax, 0, 4ull * nL, st));
   CK(cudaMemsetAsync(d_tot, 0, 3ull * nL * 8, st));
   CK(cudaMemsetAsync(d_pre, 0, 3 * nr1 * 8, st));
   uint32_t* ent = d_len; uint32_t* nn = d_len + nr1; uint32_t* vb = d_len + 2 * nr1;
@@ -929,14 +1085,17 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
         k_offsets<uint64_t><<<lb, 1024, 0, st>>>(lens, n, blk, d_pre + s * nr1 + (uint64_t)l * (n + 1));
       }
     k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
+    if (pidx) k_row_max<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, n, vb, d_vmax);
   }
   // SYNC 1: page counts, totals, required-column nulls
   std::vector<uint32_t> np(n_chunks);
   std::vector<unsigned long long> tot(3ull * nL), req(nL);
+  std::vector<unsigned int> vmax(nL);
   if (n_chunks) CK(cudaMemcpyAsync(np.data(), d_np, n_chunks * 4ull, cudaMemcpyDeviceToHost, st));
   if (nL) {
     CK(cudaMemcpyAsync(tot.data(), d_tot, 3ull * nL * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(req.data(), d_req, nL * 8ull, cudaMemcpyDeviceToHost, st));
+    if (pidx) CK(cudaMemcpyAsync(vmax.data(), d_vmax, 4ull * nL, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
   for (uint32_t l = 0; l < nL; l++)
@@ -996,16 +1155,26 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     Chunk& k = wide[c];
     k.offset = k.num_values = k.usize = k.csize = k.null_count = 1ull << 62; k.has_minmax = true; k.min.assign(kStatMax, 'x'); k.max.assign(kStatMax, 'x');
     if (has_dict(c % nL)) { k.dict = true; k.data_offset = 1ull << 62; k.data_pages = INT32_MAX; }
+    if (pidx) { k.page_index = true; k.ci_offset = k.oi_offset = 1ull << 62; k.ci_len = k.oi_len = INT32_MAX; }
   }
   const char* created_by = "etl-b200 parquet writer";
   const uint64_t footer_bound = footer(meta, rg_rows, wide, cc, created_by).size() + 8;
   const uint64_t data_bound = 4 + P * kPageHeaderMax + (snappy ? C_bound : U);
+  // ETL_PQ_PAGE_INDEX: per page a ColumnIndex entry (null flag, two bounds of at most 64 bytes + a 10-byte length, a
+  // null count) and a PageLocation, per chunk the fields' and lists' headers; a byte-array maximum that cannot be
+  // incremented stays whole, at most its page's longest row (bounded by the leaf's rows or its value bytes)
+  uint64_t index_bound = 0;
+  if (pidx) {
+    index_bound = P * (1 + 2 * (10 + kIndexTruncate) + 10 + 30) + 64ull * n_chunks;
+    for (uint32_t l = 0; l < nL; l++)
+      if (vmax[l] > kIndexTruncate) index_bound += std::min<uint64_t>(tot[2 * nL + l], (pages_of[l] + n_rg) * (uint64_t)vmax[l]);
+  }
   Page* d_pages = (Page*)dalloc(sizeof(Page) * (P + 1));
   uint64_t* d_pbase = (uint64_t*)dalloc(16 * (n_chunks + 1ull));   // page_base | leaf_page_base
   uint64_t* d_lbase = (uint64_t*)dalloc(8 * (nL + 1ull));
   uint8_t* d_lscr = (uint8_t*)dalloc(lscr_base[nL] + 16);
   uint64_t* d_scan = (uint64_t*)dalloc(8 * 4 * (P + 1));   // uslot | cslot | fbase | file offsets, P + 1 each
-  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 5);
+  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 6);
   uint8_t* d_u = (uint8_t*)dalloc(U + 16);
   uint32_t* d_bool = (uint32_t*)dalloc(bool_words * 4 + 8);
   uint8_t* d_c = snappy ? (uint8_t*)dalloc(C_bound + 16) : nullptr;
@@ -1033,7 +1202,14 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     d_desum = (uint64_t*)dalloc(8 * d_items);
     if (!d_dch || !d_tabn || !d_dblk || !d_tab || !d_dpos || !d_dflag || !d_desz || !d_dhead || !d_dfirst || !d_desum) return fail(ETL_ERR_ALLOC);
   }
-  if (cudaMalloc(&Fo->dev, data_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
+  IndexChunk* d_ix = nullptr;
+  unsigned long long* d_ixlen = nullptr;
+  if (pidx && P) {
+    d_ix = (IndexChunk*)dalloc(sizeof(IndexChunk) * n_chunks);
+    d_ixlen = (unsigned long long*)dalloc(8 * (2ull * n_chunks + 1));
+    if (!d_ix || !d_ixlen) return fail(ETL_ERR_ALLOC);
+  }
+  if (cudaMalloc(&Fo->dev, data_bound + index_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
   uint64_t* uslot = d_scan; uint64_t* cslot = d_scan + (P + 1); uint64_t* fbase = d_scan + 2 * (P + 1); uint64_t* foff = d_scan + 3 * (P + 1);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_pbase, page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
@@ -1091,14 +1267,22 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
     k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, snappy, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
     k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout, d_dch);
+    if (d_ix) {
+      // page index: sizes and boundary orders, their places behind the pages, the bytes
+      const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
+      k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, Fo->dev, d_cout);
+      k_blk_scan64<<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
+      k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, Fo->dev, d_cout);
+    }
   }
   if (nL) k_leaf<<<(nL + 63) / 64, 64, 0, st>>>(d_leaves, nL, P ? n_rg : 0, d_cout, d_lout);
   // SYNC 2: chunk and leaf records
   std::vector<ChunkOut> hc(n_chunks), hlo(nL);
-  unsigned long long data_end = 0;
+  unsigned long long data_end = 0, index_end = 0;   // the pages' bytes, then the page index's (d_stot 3 and 5)
   if (P) {
     CK(cudaMemcpyAsync(hc.data(), d_cout, sizeof(ChunkOut) * n_chunks, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(&data_end, d_stot + 3, 8, cudaMemcpyDeviceToHost, st));
+    if (d_ix) CK(cudaMemcpyAsync(&index_end, d_stot + 5, 8, cudaMemcpyDeviceToHost, st));
   }
   if (nL) CK(cudaMemcpyAsync(hlo.data(), d_lout, sizeof(ChunkOut) * nL, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1109,14 +1293,14 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     const ChunkOut& K = hc[c];
     chunks[c] = Chunk{K.offset, K.num_values, K.usize, K.csize, K.null_count, K.has != 0,
                       std::string((const char*)K.min, K.min_len), std::string((const char*)K.max, K.max_len),
-                      K.dict != 0, K.data_offset, K.data_pages};
+                      K.dict != 0, K.data_offset, K.data_pages, pidx != 0, K.ci_offset, K.oi_offset, K.ci_len, K.oi_len};
   }
   std::vector<uint8_t> foot = footer(meta, rg_rows, chunks, cc, created_by);
   const uint32_t flen = (uint32_t)foot.size();
   for (int b = 0; b < 4; b++) foot.push_back((uint8_t)(flen >> (8 * b)));
   for (char ch : std::string("PAR1")) foot.push_back((uint8_t)ch);
-  Fo->size = 4 + data_end + foot.size();
-  CK(cudaMemcpyAsync(Fo->dev + 4 + data_end, foot.data(), foot.size(), cudaMemcpyHostToDevice, st));
+  Fo->size = 4 + data_end + index_end + foot.size();
+  CK(cudaMemcpyAsync(Fo->dev + 4 + data_end + index_end, foot.data(), foot.size(), cudaMemcpyHostToDevice, st));
   if (to_host) {
     if (cudaHostAlloc((void**)&Fo->host, Fo->size, cudaHostAllocDefault) != cudaSuccess) { Fo->host = nullptr; return fail(ETL_ERR_ALLOC); }
     CK(cudaMemcpyAsync(Fo->host, Fo->dev, Fo->size, cudaMemcpyDeviceToHost, st));
@@ -1173,4 +1357,5 @@ void etl_dec_parquet_free(etl_parquet_file* f) {
 //   k_dict_setup 24 / 0 / 0   k_dict_place 10 / 0 / 0   k_dict_insert 46 / 0 / 0   k_dict_mark 24 / 0 / 0
 //   k_dict_finish 22 / 0 / 0  k_dict_page 32 / 0 / 0
 //   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)
+//   k_row_max 12 / 0 / 0   k_index<false> 72 / 0 / 40 B and k_index<true> 64 / 0 / 80 B (a fixed-width bound's bytes)
 //   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan64 32 / 8192 B, k_offsets<uint64_t> 18 / 8192 B

@@ -743,13 +743,13 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * fields: one per emitted column, in order (n_fields == etl_dec_arrow_cols).  ETL_ERR_INVALID_ARG, before any launch:
  * another n_fields or none (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS), an ETL_ARROW_UNSUPPORTED
  * column (the emit lacked ETL_ARROW_ALL_COLUMNS), row_begin > row_end or row_end > etl_dec_arrow_rows, an unknown
- * codec (codec & 0xFF other than ETL_PQ_UNCOMPRESSED / ETL_PQ_SNAPPY) or a codec bit other than ETL_PQ_DICTIONARY, a NULL or
- * empty name or one longer than 1 KiB.
+ * codec (codec & 0xFF other than ETL_PQ_UNCOMPRESSED / ETL_PQ_SNAPPY) or a codec bit other than ETL_PQ_DICTIONARY and
+ * ETL_PQ_PAGE_INDEX, a NULL or empty name or one longer than 1 KiB.
  * A null in a required column (a null list of a required List column, or a null value) is data: ETL_OK with size 0 and
  * no bytes, and etl_dec_parquet_required_null gives the smallest such column and its first null row (emit row numbers)
  * — RecordBatch::try_new in rows_to_record_batch fails there before anything is written (a ConversionError in the shim).
- * The file (parity with arrow-rs bytes and defaults is not a goal: its writer adds a page index and an ARROW:schema key;
- * Iceberg readers resolve columns by field id and Parquet type):
+ * The file (parity with arrow-rs bytes and defaults is not a goal: its writer adds an ARROW:schema key and page
+ * statistics; Iceberg readers resolve columns by field id and Parquet type):
  *   layout: "PAR1", the column chunks (row-group major, column minor, pages in row order), the footer, its 4-byte LE
  *           length, "PAR1".  Row groups of at most 1 048 576 rows in row order; zero rows: no row group.
  *   pages: data page V1, no CRC, no page statistics; whole rows; a page ends after the first row that
@@ -799,10 +799,38 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  *          encoding_stats (13) [{DICTIONARY_PAGE, PLAIN, 1}, {DATA_PAGE, RLE_DICTIONARY, data pages}].  Statistics and
  *          the metrics' counts and bounds are those of the values, as without the flag.  ColumnMetaData.codec is
  *          codec & 0xFF.
+ *   page index (codec | ETL_PQ_PAGE_INDEX; without it no chunk has one, and bytes [0, 4 + data end) of a file with it
+ *          are the file written without it, the same codec and dictionary bit): the ColumnIndex and OffsetIndex arrow-rs
+ *          writes by default, for page pruning by readers.
+ *          Layout: after the last column chunk the ColumnIndex of every chunk that has one, row-group major and column
+ *          minor, then the OffsetIndex of every chunk in the same order, then the footer.  Zero rows: no row group, no
+ *          index.  ColumnChunk adds offset_index_offset (4, i64), offset_index_length (5, i32) and, with a ColumnIndex,
+ *          column_index_offset (6, i64), column_index_length (7, i32), after meta_data; offsets are file offsets.
+ *          OffsetIndex {1 page_locations: list<PageLocation>}: one per data page (not the dictionary page, so the first
+ *          is data_page_offset): {1 offset: i64 of the page header, 2 compressed_page_size: i32 of the page's file bytes
+ *          (header and Snappy preamble included), 3 first_row_index: i64, the page's first row relative to its row
+ *          group (rows, not level entries)}.
+ *          ColumnIndex {1 null_pages: list<bool> (element type 1, one byte per element: 0x01 true, 0x02 false), 2
+ *          min_values, 3 max_values: list<binary>, 4 boundary_order: i32, 5 null_counts: list<i64>}, one entry per data
+ *          page.  A null page has no non-null value; its bounds are empty.  Bounds: the PLAIN statistic bytes of the
+ *          page's min / max under the statistics' rules (type order, NaN excluded, a zero minimum -0.0 and a zero maximum
+ *          +0.0), byte arrays longer than 64 bytes truncated (arrow-rs's column_index_truncate_length; the chunk
+ *          statistics keep their rule): Utf8 min the longest prefix of at most 64 bytes ending on a character boundary;
+ *          Utf8 max the prefix up to the last character boundary at most 64, cut after its last character whose code
+ *          point + 1 is a Unicode scalar value of the same UTF-8 length, that character incremented (none: the whole
+ *          value; U+D7FF, U+FFFF, U+10FFFF and U+007F / U+07FF cannot be incremented); LargeBinary min the first 64
+ *          bytes; LargeBinary max the first 64 bytes with the last one incremented, 0xFF carrying as 0x00 into the
+ *          byte before (all 0xFF: the whole value).  boundary_order compares each non-null page with the previous one on
+ *          the untruncated bounds: ASCENDING (1) unless a min or max is below the previous page's, else DESCENDING (2)
+ *          unless one is above, else UNORDERED (0) (one page, a constant chunk or an all-null chunk: ASCENDING).
+ *          null_counts: level entries minus non-null values of each page.  A chunk with a page whose non-null values
+ *          are all NaN (no bounds) has no ColumnIndex, only its OffsetIndex.  Not written: level histograms and
+ *          SizeStatistics, page-header statistics, bloom filters.  The metrics' compressed_bytes stay the chunks' page
+ *          bytes (Iceberg's column_sizes); etl_dec_parquet_size counts the whole file.
  *   footer: Thrift compact, ascending field ids: FileMetaData {version 1, schema, num_rows, row_groups, created_by,
  *          column_orders}, SchemaElement {type, type_length, repetition_type, name, num_children, converted_type,
  *          field_id, logicalType}, RowGroup {columns, total_byte_size, num_rows, file_offset, total_compressed_size,
- *          ordinal}, ColumnChunk {file_offset, meta_data}, ColumnMetaData {type, encodings (PLAIN, + RLE with levels),
+ *          ordinal}, ColumnChunk {file_offset, meta_data[, page index fields]}, ColumnMetaData {type, encodings (PLAIN, + RLE with levels),
  *          path_in_schema, codec, num_values, total_uncompressed_size, total_compressed_size, data_page_offset,
  *          [dictionary_page_offset,] statistics[, encoding_stats]}.
  * Metrics: one record per leaf (a List column's leaf is its element), over every row group of the file; min / max are
@@ -811,9 +839,12 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * file: 36 B per (row, column), 2 B per level entry + 64 B per page, 1 bit per Boolean value, a payload slot per page (values +
  * level bound) and with Snappy a compressed slot per 64 KiB of payload; with ETL_PQ_DICTIONARY also 28 B per item of an
  * eligible leaf (bounded by its level entries) + 0.5 B per item of run heads, a dictionary slot per chunk of at most
- * 1 MiB, 32 B per data page, and hash tables of at most 16 B per non-null value. */
+ * 1 MiB, 32 B per data page, and hash tables of at most 16 B per non-null value; with ETL_PQ_PAGE_INDEX 40 B per chunk
+ * and, in the file's buffer, 189 B per page + 64 B per chunk (+ the longest row per page of a byte-array leaf with a
+ * value over 64 bytes, at most its value bytes). */
 enum { ETL_PQ_UNCOMPRESSED = 0, ETL_PQ_SNAPPY = 1 };
 #define ETL_PQ_DICTIONARY 0x100u   /* OR-ed into codec: dictionary-encode the eligible column chunks (codec & 0xFF: compression) */
+#define ETL_PQ_PAGE_INDEX 0x400u   /* OR-ed into codec: write a ColumnIndex and an OffsetIndex per column chunk */
 #define ETL_PQ_HAS_MIN_MAX 1u   /* etl_parquet_metrics.flags: min / max are set */
 typedef struct etl_parquet_field {
   const char* name;           /* UTF-8 column name, written verbatim into the Parquet schema */

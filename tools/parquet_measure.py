@@ -3,6 +3,7 @@
 
   python tools/parquet_measure.py [--copy-rows 1000000] [--c3-scale 1] [--c4-scale 0.1] [--reps 7] [--warmup 2]
                                   [--plain-only] [--no-pyarrow] [--tag NAME]
+  python tools/parquet_measure.py --page-index [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
 
 Workloads: bench.py's 10-column COPY table, C3 (one schema version) and C4 (every schema version: times and sizes are
 sums over the versions), each emitted once with 7 | ETL_ARROW_ALL_COLUMNS | ETL_ARROW_CDC_COLUMNS and kept in HBM.
@@ -16,6 +17,9 @@ to_host 0:
 A low-cardinality COPY table (status text of a dozen values, small int codes, dates, uuids from a pool of nine and a
 text[] of three tags) runs beside the COPY table.  --plain-only skips the dictionary leg, so that a library without
 ETL_PQ_DICTIONARY can be timed by the same script (ETL_LIB_SUFFIX selects it); --tag labels the lines.
+--page-index instead writes each emit of the COPY table, C5 and C4 with and without ETL_PQ_PAGE_INDEX, alternating the
+two in every repetition, with Snappy and with Snappy | ETL_PQ_DICTIONARY: the CUDA-event time of the call (median over
+the repetitions, summed over the emits) and the index bytes as a share of the file.
 Prints the card name and power limit in the same run.
 """
 import argparse
@@ -67,7 +71,7 @@ def to_arrow(col):
     return pa.Array.from_buffers(PA_TYPE[t], n, [mask, pa.py_buffer(np.ascontiguousarray(col["values"]).tobytes())])
 
 
-OPTS = dict(plain_only=False, pyarrow=True)
+OPTS = dict(plain_only=False, pyarrow=True, page_index=False)
 
 
 def measure_emits(lib, emits, reps, warmup):
@@ -120,6 +124,39 @@ def measure_emits(lib, emits, reps, warmup):
     return out
 
 
+def page_index_emits(lib, emits, reps, warmup):
+    """ETL_PQ_PAGE_INDEX: per codec, the call's CUDA-event time without / with the flag, alternated, and the index's bytes"""
+    out = {}
+    for codec, name in ((abi.PQ_SNAPPY, "snappy"), (abi.PQ_SNAPPY | abi.PQ_DICTIONARY, "snappy_dict")):
+        ms, size = {0: [], abi.PQ_PAGE_INDEX: []}, {0: 0, abi.PQ_PAGE_INDEX: 0}
+        for a in emits:
+            fields = fields_for(emit_columns(lib, a))
+            n = lib.etl_dec_arrow_rows(a)
+            t = {0: [], abi.PQ_PAGE_INDEX: []}
+            for r in range(warmup + reps):
+                for flag in (0, abi.PQ_PAGE_INDEX):
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    rc, h = pq_write(lib, a, fields, 0, n, codec | flag, 0)
+                    e1.record()
+                    e1.synchronize()
+                    assert rc == 0
+                    if r == 0:
+                        size[flag] += lib.etl_dec_parquet_size(h)
+                    lib.etl_dec_parquet_free(h)
+                    if r >= warmup:
+                        t[flag].append(e0.elapsed_time(e1))
+            for flag in t:
+                ms[flag].append(float(np.median(t[flag])))
+        base, with_idx = sum(ms[0]), sum(ms[abi.PQ_PAGE_INDEX])
+        out[name] = dict(write_ms=round(base, 3), write_ms_page_index=round(with_idx, 3),
+                         cost_pct=round(100 * (with_idx - base) / base, 1) if base else None,
+                         file_bytes=int(size[0]), file_bytes_page_index=int(size[abi.PQ_PAGE_INDEX]),
+                         index_share_pct=round(100 * (size[abi.PQ_PAGE_INDEX] - size[0]) / size[abi.PQ_PAGE_INDEX], 3)
+                         if size[abi.PQ_PAGE_INDEX] else None)
+    return out
+
+
 def low_cardinality_rows(n_rows):
     """(oids, COPY rows) of the low-cardinality table, seeded"""
     rng = np.random.default_rng(29)
@@ -155,7 +192,7 @@ def copy_table(n_rows, reps, warmup, tag, low_card=False):
         assert lib.etl_dec_arrow_emit(bh._h, 0, KINDS, 1, C.byref(a)) == 0
         res = dict(tag=tag, workload="low-cardinality COPY table (int4, text, int4, date, uuid, text[])" if low_card
                    else "bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
-        res.update(measure_emits(lib, [a], reps, warmup))
+        res.update(page_index_emits(lib, [a], reps, warmup) if OPTS["page_index"] else measure_emits(lib, [a], reps, warmup))
         lib.etl_dec_arrow_free(a)
         print(json.dumps(res), flush=True)
     dec.close()
@@ -177,7 +214,8 @@ def streaming(name, scale, reps, warmup, tag):
             a = C.c_void_p()
             assert lib.etl_dec_arrow_emit(bh._h, si, KINDS, 1, C.byref(a)) == 0
             emits.append(a)
-        res.update(measure_emits(lib, emits, reps, warmup), versions=len(emits))
+        res.update(page_index_emits(lib, emits, reps, warmup) if OPTS["page_index"] else measure_emits(lib, emits, reps, warmup),
+                   versions=len(emits))
         for a in emits:
             lib.etl_dec_arrow_free(a)
     st.close()
@@ -195,13 +233,20 @@ def main():
     ap.add_argument("--plain-only", action="store_true")
     ap.add_argument("--no-pyarrow", action="store_true")
     ap.add_argument("--tag", default="")
+    ap.add_argument("--page-index", action="store_true")
+    ap.add_argument("--c5-scale", type=float, default=0.02)
     a = ap.parse_args()
-    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow)
+    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index)
     if not torch.cuda.is_available():
         raise SystemExit("parquet_measure needs a CUDA device")
     t = time.time()
     print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
     copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
+    if a.page_index:
+        for name, scale in (("c5", a.c5_scale), ("c4", a.c4_scale)):
+            streaming(name, scale, a.reps, a.warmup, a.tag)
+        print(json.dumps(dict(wall_s=round(time.time() - t, 1))), flush=True)
+        return
     if not a.plain_only:
         copy_table(a.copy_rows, a.reps, a.warmup, a.tag, low_card=True)
     for name, scale in (("c3", a.c3_scale), ("c4", a.c4_scale)):
