@@ -123,7 +123,9 @@ EXPORTS = [
     "etl_dec_copy_decode", "etl_dec_arrow_emit", "etl_dec_arrow_rows", "etl_dec_arrow_cols", "etl_dec_arrow_row_records",
     "etl_dec_arrow_column", "etl_dec_arrow_list_child", "etl_dec_arrow_first_skipped", "etl_dec_arrow_free", "etl_dec_rowbinary_emit", "etl_dec_rowbinary_rows", "etl_dec_rowbinary_bytes",
     "etl_dec_rowbinary_data", "etl_dec_rowbinary_row_offsets", "etl_dec_rowbinary_row_records", "etl_dec_rowbinary_issues",
-    "etl_dec_rowbinary_free", "etl_dec_bigquery_emit", "etl_dec_bigquery_rows", "etl_dec_bigquery_bytes", "etl_dec_bigquery_data",
+    "etl_dec_rowbinary_free", "etl_dec_rowbinary_lz4", "etl_dec_rowbinary_lz4_inserts", "etl_dec_rowbinary_lz4_insert_rows",
+    "etl_dec_rowbinary_lz4_insert_offsets", "etl_dec_rowbinary_lz4_bytes", "etl_dec_rowbinary_lz4_data", "etl_dec_rowbinary_lz4_free",
+    "etl_dec_bigquery_emit", "etl_dec_bigquery_rows", "etl_dec_bigquery_bytes", "etl_dec_bigquery_data",
     "etl_dec_bigquery_row_offsets", "etl_dec_bigquery_row_records", "etl_dec_bigquery_issues", "etl_dec_bigquery_free",
     "etl_dec_ducklake_emit", "etl_dec_ducklake_mutations", "etl_dec_ducklake_kinds", "etl_dec_ducklake_records",
     "etl_dec_ducklake_text", "etl_dec_ducklake_issues", "etl_dec_ducklake_sub_batches", "etl_dec_ducklake_copy_fingerprint",
@@ -210,6 +212,15 @@ def load(build: bool = True):
     L.etl_dec_rowbinary_issues.argtypes = [vp, C.POINTER(RowBinaryIssues)]
     L.etl_dec_rowbinary_free.argtypes = [vp]
     L.etl_dec_rowbinary_free.restype = None
+    L.etl_dec_rowbinary_lz4.argtypes = [vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int, C.POINTER(vp)]
+    for f in ("etl_dec_rowbinary_lz4_inserts", "etl_dec_rowbinary_lz4_bytes"):
+        getattr(L, f).argtypes = [vp]
+        getattr(L, f).restype = C.c_uint64
+    for f in ("etl_dec_rowbinary_lz4_insert_rows", "etl_dec_rowbinary_lz4_insert_offsets", "etl_dec_rowbinary_lz4_data"):
+        getattr(L, f).argtypes = [vp, C.c_int]
+        getattr(L, f).restype = C.c_void_p
+    L.etl_dec_rowbinary_lz4_free.argtypes = [vp]
+    L.etl_dec_rowbinary_lz4_free.restype = None
     L.etl_dec_bigquery_emit.argtypes = [vp, C.c_uint32, C.c_int, C.POINTER(vp)]
     for f in ("etl_dec_bigquery_rows", "etl_dec_bigquery_bytes"):
         getattr(L, f).argtypes = [vp]

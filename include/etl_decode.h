@@ -566,6 +566,37 @@ const uint64_t* etl_dec_rowbinary_row_records(const etl_rowbinary_batch*, int ho
 int etl_dec_rowbinary_issues(const etl_rowbinary_batch*, etl_rowbinary_issues* out);
 void etl_dec_rowbinary_free(etl_rowbinary_batch*);
 
+/* ---------------------------------------------------------------- ClickHouse compressed INSERT bodies
+ * Rows [row_begin, row_end) of a RowBinary emit as the INSERT bodies the ClickHouse destination posts with
+ * decompress=1, split and compressed on the device.  Replaces insert_rows's buffered chunks (client.rs:336-379) and
+ * the clickhouse crate's LZ4 compression of each chunk into ClickHouse compressed blocks.
+ * Split: insert_rows's greedy rule from row_begin: an INSERT takes rows while the bytes counted so far are below
+ * max_bytes_per_insert, so the row that crosses the limit still goes into it, and the next INSERT starts after that
+ * row.  insert_rows (n_inserts + 1 emit rows, [0] = row_begin, [n_inserts] = row_end): INSERT k is rows
+ * [insert_rows[k], insert_rows[k+1]); its body is data[insert_offsets[k], insert_offsets[k+1]).  An empty range gives
+ * zero INSERTs (one entry each).
+ * Body: a sequence of ClickHouse compressed blocks whose decompressed bytes, concatenated, are the emit's
+ * data[off[insert_rows[k]], off[insert_rows[k+1]]) (blocks may cut rows).  A block holds up to 16 KiB of those bytes
+ * (the last of a body fewer) and is: 16 bytes of checksum, CityHash128 v1.0.2 of the 9 header bytes and the payload,
+ * written as low64 then high64, each little-endian; the method byte 0x82 (LZ4); u32 LE compressed size (9 + payload);
+ * u32 LE decompressed size; the payload, one LZ4 block: the last sequence is literals only, the last 5 bytes are
+ * literals, no match starts within the last 12 bytes.  Deterministic: the same emit and arguments give the same bytes.
+ * Not byte-identical to the clickhouse crate's own compression (lz4_flex, 256 KiB chunks); the server accepts any valid
+ * LZ4 block up to 1 GiB.
+ * ETL_ERR_INVALID_ARG: a NULL emit or out, max_bytes_per_insert 0 (the reference's loop never advances), row_begin >
+ * row_end, row_end > n_rows.  Runs on the library's stream with three host syncs (the cuts, the output size, the end
+ * of the call) and owns its output: the emit may be freed once the call returns.  Scratch, beside the output: 16 B per
+ * INSERT, 16 B per block, and the compressed slots: 256/255 of the range's bytes + 56 B per block. */
+typedef struct etl_rowbinary_lz4 etl_rowbinary_lz4;
+int etl_dec_rowbinary_lz4(const etl_rowbinary_batch*, uint64_t row_begin, uint64_t row_end, uint64_t max_bytes_per_insert,
+                          int to_host, etl_rowbinary_lz4** out);
+uint64_t etl_dec_rowbinary_lz4_inserts(const etl_rowbinary_lz4*);
+const uint64_t* etl_dec_rowbinary_lz4_insert_rows(const etl_rowbinary_lz4*, int host);      /* n_inserts + 1 emit rows */
+const uint64_t* etl_dec_rowbinary_lz4_insert_offsets(const etl_rowbinary_lz4*, int host);   /* n_inserts + 1 byte offsets */
+uint64_t etl_dec_rowbinary_lz4_bytes(const etl_rowbinary_lz4*);
+const uint8_t* etl_dec_rowbinary_lz4_data(const etl_rowbinary_lz4*, int host);
+void etl_dec_rowbinary_lz4_free(etl_rowbinary_lz4*);
+
 /* ---------------------------------------------------------------- BigQuery Storage Write emitter
  * The rows of ONE replicated-schema version of a decoded batch as the serialized protobuf messages the BigQuery
  * destination puts into ProtoRows.serialized_rows, built on the device, plus n_rows + 1 u64 row offsets: row i is

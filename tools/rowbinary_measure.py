@@ -3,7 +3,7 @@
 (row_kinds 3|ALL|CDC, COPY: 1|ALL|CDC) and etl_shim_materialise of the same batch.
 
   python tools/rowbinary_measure.py [--c2-scale 1] [--c3-scale 1] [--c4-scale 0.1] [--c5-scale 0.1] [--copy-rows 1000000]
-                                    [--reps 7] [--warmup 2] [--profile OUT_DIR]
+                                    [--reps 7] [--warmup 2] [--profile OUT_DIR] [--lz4]
 
 Workloads: C2, C3 (one batch, one schema version), C4 (one batch, every schema version: times are sums over the
 versions), C5 at 0.1, about 1 GiB (both tables: TOAST, key-only deletes, partial updates), and bench.py's 10-column COPY table.  The stream
@@ -13,6 +13,11 @@ of wall time around the call (each emit syncs before it returns), with to_host 0
 time with to_host 0.  Prints the card name and power limit in the same run.
 --profile: one emit per workload under torch.profiler instead (separate run), written to OUT_DIR as a table of CUDA
 kernel time and CUDA runtime API time (cudaMallocAsync / cudaFreeAsync / cudaMalloc / cudaFree / syncs) per workload.
+--lz4: instead, the compressed INSERT bodies (etl_dec_rowbinary_lz4) of each emit at the 64 MiB default
+max_bytes_per_insert: the call's time with to_host 0 and 1, uncompressed GB/s (RowBinary bytes / median to_host 0 time),
+the compression ratio (RowBinary bytes / body bytes), and the same INSERTs cut at the same block size compressed on one
+host thread by pyarrow's lz4_raw (liblz4, standing in for the clickhouse crate's lz4_flex): its time and ratio.  With
+--profile, the LZ4 call's kernels under torch.profiler.
 """
 import argparse
 import ctypes as C
@@ -56,6 +61,76 @@ def sum_stats(parts):
     return {k: round(sum(p[k] for p in parts), 3) for k in ("median", "min", "max")}
 
 
+LZ4_MAX = 64 << 20        # the destination's default max_bytes_per_insert
+
+
+def lz4_once(lib, h, to_host):
+    z = C.c_void_p()
+    assert lib.etl_dec_rowbinary_lz4(h, 0, lib.etl_dec_rowbinary_rows(h), LZ4_MAX, to_host, C.byref(z)) == 0
+    return z
+
+
+def measure_lz4(lib, bh, versions, flags_of, reps, warmup):
+    """per version: etl_dec_rowbinary_lz4 over the whole emit (to_host 0 / 1) and liblz4 on one host thread over the
+    same INSERTs and block cuts; summed over the versions"""
+    import pyarrow as pa
+    sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
+    import clickhouse_lz4_ref as Z
+    codec = pa.Codec("lz4_raw")
+    t0s, t1s, host_ms, raw, dev_z, host_z = [], [], 0.0, 0, 0, 0
+    for si in versions:
+        h = rb_once(lib, bh, si, flags_of(si), 1)
+        t0s.append(timed(lambda: lib.etl_dec_rowbinary_lz4_free(lz4_once(lib, h, 0)), reps, warmup))
+        t1s.append(timed(lambda: lib.etl_dec_rowbinary_lz4_free(lz4_once(lib, h, 1)), reps, warmup))
+        z = lz4_once(lib, h, 1)
+        n_ins = lib.etl_dec_rowbinary_lz4_inserts(z)
+        cuts = np.ctypeslib.as_array(C.cast(lib.etl_dec_rowbinary_lz4_insert_rows(z, 1), C.POINTER(C.c_uint64)), shape=(n_ins + 1,)).copy()
+        dev_z += lib.etl_dec_rowbinary_lz4_bytes(z)
+        lib.etl_dec_rowbinary_lz4_free(z)
+        n = lib.etl_dec_rowbinary_rows(h)
+        nbytes = lib.etl_dec_rowbinary_bytes(h)
+        raw += nbytes
+        if nbytes:
+            offs = np.ctypeslib.as_array(C.cast(lib.etl_dec_rowbinary_row_offsets(h, 1), C.POINTER(C.c_uint64)), shape=(n + 1,))
+            data = bytes((C.c_uint8 * nbytes).from_address(lib.etl_dec_rowbinary_data(h, 1)))
+            blocks = [data[a:min(a + Z.KBLOCK, int(offs[cuts[k + 1]]))]
+                      for k in range(n_ins) for a in range(int(offs[cuts[k]]), int(offs[cuts[k + 1]]), Z.KBLOCK)]
+            t = time.perf_counter()
+            host_z += sum(Z.HEADER + len(codec.compress(b, asbytes=True)) for b in blocks)
+            host_ms += (time.perf_counter() - t) * 1e3
+        lib.etl_dec_rowbinary_free(h)
+    t0 = sum_stats(t0s)
+    return dict(rowbinary_bytes=int(raw), lz4_bytes=int(dev_z), lz4_block=Z.KBLOCK, lz4_ms_to_host0=t0, lz4_ms_to_host1=sum_stats(t1s),
+                lz4_GBps_uncompressed=round(raw / (t0["median"] * 1e-3) / 1e9, 2) if t0["median"] else None,
+                lz4_ratio=round(raw / dev_z, 3) if dev_z else None, liblz4_1thread_ms=round(host_ms, 1),
+                liblz4_ratio=round(raw / host_z, 3) if host_z else None, versions=len(versions))
+
+
+def profile_lz4(lib, bh, versions, flags_of, label, out_dir):
+    """one warm etl_dec_rowbinary_lz4 call per version under torch.profiler: kernel time by name"""
+    from torch.profiler import ProfilerActivity, profile
+    hs = [rb_once(lib, bh, si, flags_of(si), 0) for si in versions]
+    for h in hs:
+        lib.etl_dec_rowbinary_lz4_free(lz4_once(lib, h, 0))
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        for h in hs:
+            lib.etl_dec_rowbinary_lz4_free(lz4_once(lib, h, 0))
+        torch.cuda.synchronize()
+    for h in hs:
+        lib.etl_dec_rowbinary_free(h)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, f"lz4_profile_{label}.txt"), "w") as f:
+        f.write(prof.key_averages().table(sort_by="self_cuda_time_total", row_limit=30) + "\n")
+    kern = {}
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", 0) or getattr(e, "cuda_time_total", 0)
+        if t and not e.key.startswith("cu"):
+            kern[e.key[:60]] = round(t / 1e3, 3)
+    res = dict(profile=label, lz4_kernel_ms=kern)
+    print(json.dumps(res), flush=True)
+    return res
+
+
 def measure_batch(lib, bh, versions, flags_of, arrow_kinds, reps, warmup):
     """per version: RowBinary emit (to_host 0 / 1) and the Arrow emit; summed over the versions"""
     rb0, rb1, ar, rows, nbytes = [], [], [], 0, 0
@@ -79,7 +154,7 @@ def measure_batch(lib, bh, versions, flags_of, arrow_kinds, reps, warmup):
                 arrow_all_cdc_ms=sum_stats(ar), versions=len(versions))
 
 
-def streaming(name, scale, reps, warmup, profile=None):
+def streaming(name, scale, reps, warmup, profile=None, lz4=False):
     w = wl.make(name, scale, n_segments=1)
     stream, stats = w.generate()
     st = decoder.Stager(stream.nbytes, 2048)
@@ -97,6 +172,11 @@ def streaming(name, scale, reps, warmup, profile=None):
     with dec.decode_input(inp, to_host=profile is None) as bh:
         s = bh.summary()
         versions = list(range(s.n_schemas))
+        if lz4:
+            flags_of = lambda si: create_table_flags(lib, bh, si)  # noqa: E731
+            res.update(profile_lz4(lib, bh, versions, flags_of, name, profile) if profile else measure_lz4(lib, bh, versions, flags_of, reps, warmup))
+            print(json.dumps(res), flush=True)
+            return res
         if profile is not None:
             return profile_emits(lib, bh, versions, lambda si: create_table_flags(lib, bh, si), name, profile)
         res["decode_kernel_ms"] = round(s.kernel_ms, 3)
@@ -112,7 +192,7 @@ def streaming(name, scale, reps, warmup, profile=None):
     return res
 
 
-def copy_table(n_rows, reps, warmup, profile=None):
+def copy_table(n_rows, reps, warmup, profile=None, lz4=False):
     oids, rows = bench_copy_table(n_rows)
     lib = abi.load()
     blob = b"".join(rows)
@@ -130,6 +210,12 @@ def copy_table(n_rows, reps, warmup, profile=None):
     assert lib.etl_dec_copy_decode(dec._ctx, 9, C.byref(inp), 0, C.byref(h)) == 0, lib.etl_dec_last_error(dec._ctx)
     flags = create_table_flags(lib, None, 0, oids)
     with decoder.BatchHandle(dec, h) as bh:
+        if lz4:
+            res = dict(workload="bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
+            res.update(profile_lz4(lib, bh, [0], lambda si: flags, "copy", profile) if profile else measure_lz4(lib, bh, [0], lambda si: flags, reps, warmup))
+            dec.close()
+            print(json.dumps(res), flush=True)
+            return res
         if profile is not None:
             return profile_emits(lib, bh, [0], lambda si: flags, "copy", profile)
         res = dict(workload="bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
@@ -174,11 +260,12 @@ def main():
     ap.add_argument("--reps", type=int, default=7)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--profile", default=None)
+    ap.add_argument("--lz4", action="store_true")
     a = ap.parse_args()
     print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
-    copy_table(a.copy_rows, a.reps, a.warmup, a.profile)
+    copy_table(a.copy_rows, a.reps, a.warmup, a.profile, a.lz4)
     for name, scale in (("c2", a.c2_scale), ("c3", a.c3_scale), ("c4", a.c4_scale), ("c5", a.c5_scale)):
-        streaming(name, scale, a.reps, a.warmup, a.profile)
+        streaming(name, scale, a.reps, a.warmup, a.profile, a.lz4)
 
 
 if __name__ == "__main__":
