@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(kRowsThreads, ETL_ROWS_CTAS) k_copy_rows(Decod
   }
   __syncthreads();
   const uint32_t bar = smem_u32(smem + kRowsBarOff + 8u * wid);
-  uint8_t* const slot = smem + kRowsSlotsOff + ((uint32_t)wid * 32u + (uint32_t)lane) * kRowsSlot;
+  uint8_t* const slot = smem + kCopySlotsOff + ((uint32_t)wid * 32u + (uint32_t)lane) * kCopySlot;
   const uint32_t slot_s = smem_u32(slot);
   uint32_t parity = 0;
   const uint32_t n_rows = (uint32_t)P.total[0].n_rec, n_cols = P.copy_cols;
@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(kRowsThreads, ETL_ROWS_CTAS) k_copy_rows(Decod
       if (!done && from < end) {
         const uint64_t g0 = (goff + from) & ~15ull;
         const uint64_t gend = (goff + end + 15ull) & ~15ull;
-        n = (uint32_t)min((uint64_t)kRowsWin, gend - g0);
+        n = (uint32_t)min((uint64_t)kCopyWin, gend - g0);
         W.delta = (int32_t)((int64_t)g0 - (int64_t)goff);
         W.w1 = (uint32_t)(W.delta + (int32_t)n);
         mbar_arrive_expect_tx(bar, n);

@@ -1460,7 +1460,7 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
     if (nc) CKB(cudaMemsetAsync(P.cell_tag, 0, nc, st));   // a row that failed leaves cells unwritten: k_heavy must not see stale tags
     CKB(cudaEventRecord(ctx->ev[1], st));
     if (nr) {
-      k_copy_rows<<<(uint32_t)((nr + kRowsThreads - 1) / kRowsThreads), kRowsThreads, kRowsSmemBytes, st>>>(P);
+      k_copy_rows<<<(uint32_t)((nr + kRowsThreads - 1) / kRowsThreads), kRowsThreads, kCopySmemBytes, st>>>(P);
       k_heavy<<<std::min<uint32_t>((uint32_t)((nc + kHeavyTile - 1) / kHeavyTile) + 1u, (uint32_t)sm_count(ctx) * 3u), kHeavyThreads, kHeavySmemBytes, st>>>(P);
       ctx->launches += 2;
       CKB(cudaGetLastError());

@@ -8,6 +8,9 @@
 //            the whole warp on bytes that sit in shared memory.  The cell-header hop chain and the value bytes
 //            are read from HBM exactly once (by the copy engine); there is no descriptor round trip, and an
 //            unchanged-TOAST cell takes the value the same lane decoded for the old image a few steps earlier.
+//            A lane's output cells go to its warp's stage in shared memory, not to the planes: at every step the 32
+//            lanes write 32 different records' cells, which straight to the planes touched ~60 lines per step.  The
+//            warp flushes the stage as runs of consecutive cells of one record (stage_flush).
 //            k_rows itself parses the LIGHT decode classes (text, bool, integers, date / timestamp(tz), uuid in the
 //            spellings Postgres emits): ~100 registers, no stack, 20+ warps per SM.  Every other cell (json, numeric,
 //            floats, bytea, time, arrays, and any spelling the fast paths decline) is left in the cell plane as a
@@ -23,8 +26,21 @@
 
 namespace etl {
 
+// k_rows: the window and the cell stage share the shared memory of 5 CTAs per SM.  A 4-cell stage per lane (1.6 KB per
+// warp) is paid for by a 240-byte window instead of 304; 240 is the largest window that still fits 5 CTAs next to a
+// 4-cell stage (256 fits, 272 misses by ~0.5 KB), and a 16-cell stage (6.5 KB per warp) would leave under 160 bytes.
+// Measured on C5 / C2 (H100 SXM, 700 W), k_rows + k_heavy + k_fix: no stage, 304 B 2.05 / 0.53 ms; 4 cells, 240 B
+// 1.41 / 0.46 ms; 8 cells, 208 B 1.59 / 0.54 ms; 8 cells, 176 B 1.74 / 0.58 ms: the window's restages cost more than
+// the longer runs save.
+#ifndef ETL_TUPLE_WIN
+#define ETL_TUPLE_WIN 240                // k_rows: bytes of one record's frame staged per pass (multiple of 16)
+#endif
+// k_copy_rows has no cell stage and keeps the whole window
 #ifndef ETL_ROWS_WIN
-#define ETL_ROWS_WIN 304                 // bytes of one record's frame staged per pass (multiple of 16)
+#define ETL_ROWS_WIN 304                 // k_copy_rows: bytes of one COPY row staged per pass (multiple of 16)
+#endif
+#ifndef ETL_ROWS_STAGE
+#define ETL_ROWS_STAGE 4                 // output cells per lane staged in shared memory between flushes (power of 2, ≤ 16)
 #endif
 #ifndef ETL_ROWS_CTAS
 #define ETL_ROWS_CTAS 5                  // resident CTAs per SM the register budget is set for
@@ -34,15 +50,29 @@ namespace etl {
 #endif
 constexpr uint32_t kRowsWarps = ETL_ROWS_WARPS;
 constexpr uint32_t kRowsThreads = kRowsWarps * 32;
-constexpr uint32_t kRowsWin = ETL_ROWS_WIN;
+constexpr uint32_t kRowsWin = ETL_TUPLE_WIN;
 constexpr uint32_t kRowsSlot = kRowsWin + 16;                      // slot stride: 16-byte aligned, skews the banks
 constexpr uint32_t kRowsBarOff = 0;                                // one mbarrier per warp
 constexpr uint32_t kRowsColsOff = kRowsBarOff + 128;               // per warp: 256 column kinds + 256 column flags of its schema
 constexpr uint32_t kRowsColsCached = 256;
-constexpr uint32_t kRowsSlotsOff = kRowsColsOff + kRowsWarps * 2 * kRowsColsCached;
+// per warp: the cell stage, kRowsStage rows of 32 entries as planes val (u64), aux (u32), tag (u8)
+constexpr uint32_t kRowsStage = ETL_ROWS_STAGE;
+constexpr uint32_t kRowsStageRuns = 32 / kRowsStage;               // lanes' runs stored per round of a flush
+constexpr uint32_t kRowsStageBytes = kRowsStage * 32 * 13;
+constexpr uint32_t kRowsStageOff = kRowsColsOff + kRowsWarps * 2 * kRowsColsCached;
+constexpr uint32_t kRowsSlotsOff = kRowsStageOff + kRowsWarps * kRowsStageBytes;
 constexpr uint32_t kRowsSmemBytes = kRowsSlotsOff + kRowsWarps * 32 * kRowsSlot + 64;   // + tail padding for word reads
 constexpr uint32_t kRowsMaxInWin = kRowsWin - 24;                  // a text cell up to this long always fits a fresh window
 static_assert(kRowsWarps <= 15 && kRowsWin % 16 == 0, "k_rows geometry");
+static_assert(kRowsStage >= 2 && kRowsStage <= 16 && (kRowsStage & (kRowsStage - 1)) == 0 && kRowsStageBytes % 16 == 0, "k_rows stage");
+// k_copy_rows: the same barriers and column cache, no stage, its own window
+constexpr uint32_t kCopyWin = ETL_ROWS_WIN;
+constexpr uint32_t kCopySlot = kCopyWin + 16;
+constexpr uint32_t kCopySlotsOff = kRowsStageOff;
+constexpr uint32_t kCopySmemBytes = kCopySlotsOff + kRowsWarps * 32 * kCopySlot + 64;
+static_assert(kCopyWin % 16 == 0, "k_copy_rows geometry");
+static_assert((size_t)ETL_ROWS_CTAS * (kRowsSmemBytes + 1024) <= 228u * 1024u, "k_rows: the CTAs per SM must fit the shared memory");
+static_assert((size_t)ETL_ROWS_CTAS * (kCopySmemBytes + 1024) <= 228u * 1024u, "k_copy_rows: the CTAs per SM must fit the shared memory");
 
 // ---- mbarrier / bulk-copy primitives (PTX ISA 8.x; SASS: SYNCS.*, UBLKCP)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -147,6 +177,14 @@ struct TextCell { uint32_t voff, len, kind, dest, seq; };   // voff frame-relati
 #define W_DATA_ERROR(seq_, code_) do { report_error(P, P.dc->record_index_base + w.rec_local, (seq_), (code_)); w.bits &= ~WB_EMIT; } while (0)
 #define W_MALFORMED() do { report_error(P, P.dc->record_index_base + w.rec_local, SEQ_MALFORMED, ETL_E_MALFORMED_FRAME); W_SET_STAGE(W_DONE); } while (0)
 
+// The dest of the next cell `w` can write (the start of a fresh run).
+__device__ __forceinline__ uint32_t rk_next_dest(const Wk& w) {
+  const uint32_t stage = w.bits & 7u, n_old = w.keyi_nold >> 16;
+  if (stage == W_OLD_CELLS) return ((w.bits >> 5) & 3u) == WO_KEY ? (w.cmap_kout >> 16) : (w.rem_wire >> 16);
+  if (stage == W_NEW_CELLS) return n_old + (w.rem_wire >> 16);
+  return stage == W_NEW_HDR ? n_old : 0u;
+}
+
 // The staged window of a lane: frame-relative bytes [max(delta,0), w1) live at win[pos - delta].
 struct RowWin { const uint8_t* win; int32_t delta; uint32_t w1; };
 __device__ __forceinline__ bool win_has(const RowWin& W, uint32_t pos, uint32_t n, uint32_t end) {
@@ -175,9 +213,54 @@ __device__ __forceinline__ bool rk_peek(const Wk& w, const RowWin& W, uint64_t* 
   return w.pos + 5u + len > W.w1;
 }
 
+// ---- the cell stage.  Neighbouring lanes walk different records, so a cell stored straight to the planes at every step
+// touches ~60 lines per warp for 13 useful bytes per lane.  Instead each lane writes its cells into its warp's stage, at
+// dest − rb (rb = the dest its current run starts at), and the warp flushes the stage as runs: S lanes store S
+// consecutive cells of one record, a few lines per run.  Within one tuple the dests a lane writes are consecutive (a
+// skipped or failed cell ends the writes of its tuple), so a run is full when its entry S − 1 is written; the old
+// image is flushed before the new tuple starts (an unchanged-TOAST cell reads its source from the planes).
+// sg = rb | valid entries << 16.  Entry (j, lane) sits at row j, column lane ^ (j · runs per round): the lanes of one
+// step write one row, and the lanes of one flush round read 32 distinct banks.
+__device__ __forceinline__ uint32_t stage_entry(uint32_t j, uint32_t lane) { return j * 32u + (lane ^ ((j * kRowsStageRuns) & 31u)); }
+__device__ __forceinline__ void stage_put(const DecodeParams& P, uint8_t* st, uint32_t& sg, uint64_t cell0, uint32_t dest, uint32_t tag, uint64_t val, uint32_t aux) {
+  const uint32_t j = dest - (sg & 0xFFFFu);
+  // Unreachable while the run invariants hold (consecutive dests within a tuple, a flush when a run is full and before
+  // a new tuple starts elsewhere).  A store that missed the stage still lands in the plane, so a broken invariant
+  // would cost coalescing, not correctness; tests/test_gpu_rows_stage.py covers the run edges.
+  if (j >= kRowsStage) { put_cell(P, cell0 + dest, tag, val, aux); return; }
+  const uint32_t e = stage_entry(j, threadIdx.x & 31u);
+  reinterpret_cast<uint64_t*>(st)[e] = val;
+  reinterpret_cast<uint32_t*>(st + kRowsStage * 256u)[e] = aux;
+  st[kRowsStage * 384u + e] = (uint8_t)tag;
+  sg |= 1u << (16u + j);
+}
+// Warp-wide: every lane's staged entries to the planes, run after run; the next run of each lane starts at rb_next.
+__device__ __forceinline__ void stage_flush(const DecodeParams& P, const uint8_t* st, uint32_t& sg, uint64_t cell0, uint32_t rb_next) {
+  const uint32_t lane = threadIdx.x & 31u, j = lane & (kRowsStage - 1u);
+  const uint32_t vm = sg >> 16;
+  const unsigned have = __ballot_sync(0xffffffffu, vm != 0u);
+  if (have) {
+    __syncwarp();
+    const uint64_t base = cell0 + (sg & 0xFFFFu);
+    for (uint32_t r = 0; r < 32u; r += kRowsStageRuns) {
+      if (!((have >> r) & ((1u << kRowsStageRuns) - 1u))) continue;
+      const uint32_t src = r + lane / kRowsStage;
+      const uint32_t vs = __shfl_sync(0xffffffffu, vm, src);
+      const uint64_t bs = __shfl_sync(0xffffffffu, base, src);
+      if ((vs >> j) & 1u) {
+        const uint32_t e = stage_entry(j, src);
+        put_cell(P, bs + j, st[kRowsStage * 384u + e], reinterpret_cast<const uint64_t*>(st)[e], reinterpret_cast<const uint32_t*>(st + kRowsStage * 256u)[e]);
+      }
+    }
+    __syncwarp();
+  }
+  sg = rb_next;
+}
+
 // One step: a tuple header or ONE wire cell (event.rs:550-919).  Returns 0 when no wire cell was consumed
 // (header, end of a tuple, malformed), 1 when one was consumed and needs no parsing, 2 when it is a text cell.
-__device__ __forceinline__ uint32_t rk_step(const DecodeParams& P, Wk& w, TextCell& tc, const uint64_t x, const uint8_t* kinds, const uint8_t* flags) {
+__device__ __forceinline__ uint32_t rk_step(const DecodeParams& P, Wk& w, TextCell& tc, const uint64_t x, const uint8_t* kinds, const uint8_t* flags,
+                                           uint8_t* st, uint32_t& sg) {
   const uint32_t stage = w.bits & 7u, kind = (w.bits >> 3) & 3u, old = (w.bits >> 5) & 3u;
   const bool emit = (w.bits & WB_EMIT) != 0;
   const uint32_t n_cols = w.nc_ni & 0xFFFFu, n_ident = w.nc_ni >> 16;
@@ -257,7 +340,7 @@ __device__ __forceinline__ uint32_t rk_step(const DecodeParams& P, Wk& w, TextCe
     }
     if (tag == 'n') {                               // convert_tuple_data_to_cell event.rs:941-957
       if (resolver_key) w.keyi_nold++;
-      if (cflags & 1) put_cell(P, w.cell0 + dest, ETL_CELL_NULL, 0, 0);
+      if (cflags & 1) stage_put(P, st, sg, w.cell0, dest, ETL_CELL_NULL, 0, 0);
       else W_DATA_ERROR(seq, ETL_E_NOT_NULL);
       break;
     }
@@ -270,13 +353,13 @@ __device__ __forceinline__ uint32_t rk_step(const DecodeParams& P, Wk& w, TextCe
           const uint32_t stag = P.cell_tag[src];
           const uint32_t saux = P.cell_aux[src];
           if ((stag & ETL_CELL_PENDING_MASK) == ETL_CELL_PENDING) {     // the old cell waits for k_heavy: k_fix copies it afterwards
-            put_cell(P, w.cell0 + dest, ETL_CELL_PENDING_COPY, src, w.rec_local);
+            stage_put(P, st, sg, w.cell0, dest, ETL_CELL_PENDING_COPY, src, w.rec_local);
             atomicAdd(P.copy_count, 1u);
           } else {
-            put_cell(P, w.cell0 + dest, stag, P.cell_val[src], saux);
+            stage_put(P, st, sg, w.cell0, dest, stag, P.cell_val[src], saux);
             w.hint += cell_clone_hint(stag, saux);  // the clone owns its own heap buffer (Cell::clone)
           }
-        } else { put_cell(P, w.cell0 + dest, ETL_CELL_MISSING, 0, 0); w.bits |= WB_PARTIAL; }
+        } else { stage_put(P, st, sg, w.cell0, dest, ETL_CELL_MISSING, 0, 0); w.bits |= WB_PARTIAL; }
       } else W_DATA_ERROR(seq, (!is_new && old == WO_KEY) ? ETL_E_KEY_MISSING_VALUE : ETL_E_FULL_ROW_MISSING);
       break;
     }
@@ -348,9 +431,14 @@ __device__ __forceinline__ void rows_body(const DecodeParams& P, uint8_t* smem) 
   }
   RowWin W;
   W.win = slot; W.delta = 0x7FFFFFFF; W.w1 = 0;     // empty window: the first peek stages
+  uint8_t* const st = smem + kRowsStageOff + (uint32_t)wid * kRowsStageBytes;
+  uint32_t sg = 0;                                  // the lane's run: rb | staged entries << 16
   for (;;) {
     const bool act = (w.bits & 7u) != W_DONE;
     if (!__any_sync(0xffffffffu, act)) break;
+    // a lane whose run is full, or whose new tuple starts elsewhere than its run (the old image is staged): flush
+    const bool flush = ((sg >> (15u + kRowsStage)) & 1u) || ((w.bits & 7u) == W_NEW_HDR && (sg & 0xFFFFu) != (w.keyi_nold >> 16));
+    if (__any_sync(0xffffffffu, flush)) stage_flush(P, st, sg, w.cell0, rk_next_dest(w));
     uint64_t hdr;
     const bool need = rk_peek(w, W, &hdr);
     if (__any_sync(0xffffffffu, need)) {
@@ -373,7 +461,7 @@ __device__ __forceinline__ void rows_body(const DecodeParams& P, uint8_t* smem) 
     }
     TextCell tc;
     tc.voff = 0; tc.len = 0; tc.kind = 0; tc.dest = 0; tc.seq = 0;
-    const uint32_t got = act ? rk_step(P, w, tc, hdr, kinds, flags) : 0u;
+    const uint32_t got = act ? rk_step(P, w, tc, hdr, kinds, flags, st, sg) : 0u;
     const bool is_text = got == 2u;
     if (!__any_sync(0xffffffffu, is_text)) continue;
     // ---- the text cells of this step: UTF-8 (event.rs:972), the per-kind parser, the cell plane and the heap
@@ -457,10 +545,11 @@ __device__ __forceinline__ void rows_body(const DecodeParams& P, uint8_t* smem) 
     }
     if (is_text) {
       if (code) { report_error(P, P.dc->record_index_base + w.rec_local, tc.seq, code); w.bits &= ~WB_EMIT; }
-      else if (defer) put_cell(P, w.cell0 + tc.dest, ETL_CELL_PENDING | kind, ((uint64_t)w.rec_local << 32) | tc.voff, len);
-      else { put_cell(P, w.cell0 + tc.dest, o.tag, o.val, o.aux); w.hint += cell_heap_hint(o.tag, o.aux); }
+      else if (defer) stage_put(P, st, sg, w.cell0, tc.dest, ETL_CELL_PENDING | kind, ((uint64_t)w.rec_local << 32) | tc.voff, len);
+      else { stage_put(P, st, sg, w.cell0, tc.dest, o.tag, o.val, o.aux); w.hint += cell_heap_hint(o.tag, o.aux); }
     }
   }
+  stage_flush(P, st, sg, w.cell0, 0);
   // ---- per-record epilogue: Partial flag, tuple bytes + size hint planes; tuple-byte metrics (one atomic per warp and op kind)
   if (my_rec != 0xFFFFFFFFu) {
     if (w.bits & WB_PARTIAL) P.rec_flags[w.rec_local] |= ETL_RF_NEW_PARTIAL;
