@@ -305,16 +305,12 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
   if (!batch || !out) return ETL_ERR_INVALID_ARG;
   const bool all = (row_kinds & ETL_ARROW_ALL_COLUMNS) != 0;
   const bool cdc = (row_kinds & ETL_ARROW_CDC_COLUMNS) != 0;
-  const uint8_t* dev_stream = etl_dec_batch_device_stream(batch);
-  etl_dec_planes P;
-  etl_dec_summary S;
-  etl_dec_schema_info sc{};
-  if (etl_dec_batch_planes(batch, 0, &P) != ETL_OK || etl_dec_batch_summary(batch, &S) != ETL_OK) return ETL_ERR_INVALID_ARG;
   // a COPY batch (no record kinds) has one implicit schema: the columns it was decoded with
-  const bool copy = P.rec_kind == nullptr;
-  if (copy) {
-    if (schema_index != 0 || !etl_copy_batch_columns(batch, &sc.table_id, &sc.col_kind, &sc.n_cols)) return ETL_ERR_INVALID_ARG;
-  } else if (etl_dec_batch_schema(batch, schema_index, &sc) != ETL_OK) return ETL_ERR_INVALID_ARG;
+  EmitBatch E;
+  if (open_emit_batch(batch, schema_index, &E) != ETL_OK) return ETL_ERR_INVALID_ARG;
+  const etl_dec_planes& P = E.P;
+  const etl_dec_schema_info& sc = E.sc;
+  const uint8_t* dev_stream = E.stream;
   cudaStream_t st = cudaStreamPerThread;
   etl_arrow_batch* A = new etl_arrow_batch();
   // scratch of the ETL_ARROW_ALL_COLUMNS stages, freed on every exit
@@ -323,26 +319,18 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
   auto fail = [&](int rc) { free_pool(); if (A->dev) cudaFree(A->dev); if (A->host) cudaFreeHost(A->host); delete A; return rc; };
 #define CKA(call) do { if ((call) != cudaSuccess) { cudaGetLastError(); return fail(ETL_ERR_CUDA); } } while (0)
   // rows of the valid prefix only
-  const uint64_t n_valid = S.first_error.record_index == UINT64_MAX ? P.n_records : std::min<uint64_t>(P.n_records, S.first_error.record_index - S.record_index_base);
+  const uint64_t n_valid = E.n_valid;
   const uint32_t nb = (uint32_t)((n_valid + kSelThreads - 1) / kSelThreads);
   uint32_t* d_blk = nullptr; uint64_t* d_cell0 = nullptr; uint64_t* d_rec = nullptr; unsigned long long* d_n = nullptr;
   CKA(cudaMalloc(&d_blk, (nb + 1) * 4ull)); CKA(cudaMalloc(&d_cell0, (n_valid + 1) * 8)); CKA(cudaMalloc(&d_rec, (n_valid + 1) * 8)); CKA(cudaMalloc(&d_n, 16));
   auto free_tmp = [&]() { cudaFree(d_blk); cudaFree(d_cell0); cudaFree(d_rec); cudaFree(d_n); };
   SelParams Sp{P.rec_kind, P.rec_flags, P.rec_schema, P.rec_cell_base, n_valid, (int32_t)schema_index, row_kinds, sc.n_cols, d_blk, d_cell0, d_rec, d_n};
-  unsigned long long n_rows = 0;
-  if (copy) {                                           // every row of the valid prefix when inserts are selected: no sync
-    n_rows = (row_kinds & 1u) ? n_valid : 0;
-    if (n_rows) k_copy_sel<<<(uint32_t)((n_rows + 255) / 256), 256, 0, st>>>(n_rows, sc.n_cols, d_cell0, d_rec);
-  } else if (nb) {
-    unsigned long long sel[2] = {0, UINT64_MAX};        // rows, first skipped record
-    cudaMemsetAsync(d_n + 1, 0xff, 8, st);
-    k_sel_count<ArrowRows><<<nb, kSelThreads, 0, st>>>(Sp);
-    k_blk_scan<<<1, kSelThreads, 0, st>>>(d_blk, nb, d_n);
-    k_sel_scatter<ArrowRows><<<nb, kSelThreads, 0, st>>>(Sp);
-    if (cudaMemcpyAsync(sel, d_n, 16, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { free_tmp(); return fail(ETL_ERR_CUDA); }
-    n_rows = sel[0];
-    A->first_skipped = sel[1];
-  }
+  // COPY: every row of the valid prefix when inserts are selected
+  unsigned long long sel[2] = {0, UINT64_MAX};          // rows, first skipped record
+  if (!E.copy && nb) cudaMemsetAsync(d_n + 1, 0xff, 8, st);
+  if (select_rows<ArrowRows>(Sp, E.copy, (row_kinds & 1u) ? n_valid : 0, st, sel) != ETL_OK) { free_tmp(); return fail(ETL_ERR_CUDA); }
+  const uint64_t n_rows = sel[0];
+  A->first_skipped = sel[1];
   A->n_rows = n_rows;
   // pass 1: validity + fixed values + lengths (into a scratch), per column; var-width sizes need a sync before the data buffers exist
   const uint64_t vbytes = ((n_rows + 31) / 32 * 4 + 63) & ~63ull;
@@ -363,7 +351,7 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
   }
   const uint64_t fixed_bytes = cur;
   uint32_t* d_lens = nullptr; unsigned long long* d_lblk = nullptr; unsigned long long* d_tot = nullptr;
-  const uint32_t lb = (uint32_t)((n_rows + 1023) / 1024);
+  const uint32_t lb = scan_blocks(n_rows);
   if (n_var) { if (cudaMalloc(&d_lens, (size_t)n_var * (n_rows + 1) * 4) != cudaSuccess || cudaMalloc(&d_lblk, (size_t)n_var * (lb + 1) * 8) != cudaSuccess || cudaMalloc(&d_tot, n_var * 8 + 8) != cudaSuccess) { free_tmp(); return fail(ETL_ERR_ALLOC); } }
   uint8_t* d_fixed = nullptr;
   if (cudaMalloc(&d_fixed, fixed_bytes + 64) != cudaSuccess) { free_tmp(); cudaFree(d_lens); cudaFree(d_lblk); cudaFree(d_tot); return fail(ETL_ERR_ALLOC); }
@@ -383,13 +371,12 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
     if (var) Cp.lens = d_lens + (size_t)vi * (n_rows + 1);
     k_col_fixed<<<(uint32_t)((n_rows + 255) / 256), 256, 0, st>>>(Cp);
     if (var) {
-      k_len_blocks<<<lb, 1024, 0, st>>>(Cp.lens, n_rows, d_lblk + (size_t)vi * (lb + 1));
-      k_blk_scan64<<<1, 1024, 0, st>>>(d_lblk + (size_t)vi * (lb + 1), lb, d_tot + vi);
+      unsigned long long* blk = d_lblk + (size_t)vi * (lb + 1);
       if (col.text && col.kind == ETL_K_JSON) {
         if (!(json_in[c] = (uint64_t*)dalloc((n_rows + 1) * 8))) { free_stage(); return fail(ETL_ERR_ALLOC); }
-        k_offsets<uint64_t><<<lb, 1024, 0, st>>>(Cp.lens, n_rows, d_lblk + (size_t)vi * (lb + 1), json_in[c]);
-      } else if (col.arrow_type == ETL_ARROW_LARGE_BINARY) k_offsets<int64_t><<<lb, 1024, 0, st>>>(Cp.lens, n_rows, d_lblk + (size_t)vi * (lb + 1), (int64_t*)(d_fixed + col.offsets_off));
-      else k_offsets<int32_t><<<lb, 1024, 0, st>>>(Cp.lens, n_rows, d_lblk + (size_t)vi * (lb + 1), (int32_t*)(d_fixed + col.offsets_off));
+        scan_lengths(Cp.lens, n_rows, blk, d_tot + vi, json_in[c], st);
+      } else if (col.arrow_type == ETL_ARROW_LARGE_BINARY) scan_lengths(Cp.lens, n_rows, blk, d_tot + vi, (int64_t*)(d_fixed + col.offsets_off), st);
+      else scan_lengths(Cp.lens, n_rows, blk, d_tot + vi, (int32_t*)(d_fixed + col.offsets_off), st);
       vi++;
     }
   }
@@ -404,17 +391,6 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
   if (all && n_rows) {
     if (!(d_bad = (unsigned*)dalloc(8))) { free_stage(); return fail(ETL_ERR_ALLOC); }
     cudaMemsetAsync(d_bad, 0, 4, st);
-    // a var-width item set: lengths → offsets (+ total), one scan
-    auto scan = [&](uint32_t* lens, uint64_t n, void* offs, int width, unsigned long long* tot) -> bool {
-      const uint32_t b = (uint32_t)((n + 1023) / 1024);
-      unsigned long long* blk = (unsigned long long*)dalloc((b + 1) * 8ull);
-      if (!blk) return false;
-      k_len_blocks<<<b, 1024, 0, st>>>(lens, n, blk);
-      k_blk_scan64<<<1, 1024, 0, st>>>(blk, b, tot);
-      if (width == 4) k_offsets<int32_t><<<b, 1024, 0, st>>>(lens, n, blk, (int32_t*)offs);
-      else k_offsets<uint64_t><<<b, 1024, 0, st>>>(lens, n, blk, (uint64_t*)offs);
-      return true;
-    };
     // Json canonicalisation of n items whose input offsets are in_off (total input bytes t_in); new lengths → offs
     uint32_t* work = nullptr;
     uint64_t work_words = 0;
@@ -429,7 +405,10 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
       if (!canon || !work) return false;
       k_json_canon<<<(uint32_t)((Cp.n_rows + 127) / 128), 128, 0, st>>>(Cp, in_off, canon, work, d_bad);
       *canon_out = canon;
-      return scan(Cp.lens, Cp.n_rows, offs, 4, tot);
+      unsigned long long* blk = (unsigned long long*)dalloc((scan_blocks(Cp.n_rows) + 1) * 8ull);
+      if (!blk) return false;
+      scan_lengths(Cp.lens, Cp.n_rows, blk, tot, offs, st);
+      return true;
     };
     unsigned long long* d_tot2 = (unsigned long long*)dalloc(8ull * (2 * sc.n_cols + 2));
     if (!d_tot2) { free_stage(); return fail(ETL_ERR_ALLOC); }
@@ -475,8 +454,12 @@ int etl_dec_arrow_emit(const etl_dec_batch* batch, uint32_t schema_index, uint32
         if (is_var(kid.arrow_type)) {
           const bool json = kid.kind == ETL_K_JSON;
           if (json && !(ks.in_off = (uint64_t*)dalloc((ne + 1) * 8))) { free_stage(); return fail(ETL_ERR_ALLOC); }
-          void* offs = json ? (void*)ks.in_off : (void*)(kf + kid.offsets_off);
-          if (!scan(ks.lens, ne, offs, kid.arrow_type == ETL_ARROW_UTF8 && !json ? 4 : 8, d_tot2 + sc.n_cols + A->kids.size())) { free_stage(); return fail(ETL_ERR_ALLOC); }
+          unsigned long long* blk = (unsigned long long*)dalloc((scan_blocks(ne) + 1) * 8ull);
+          if (!blk) { free_stage(); return fail(ETL_ERR_ALLOC); }
+          unsigned long long* tot = d_tot2 + sc.n_cols + A->kids.size();
+          if (json) scan_lengths(ks.lens, ne, blk, tot, ks.in_off, st);
+          else if (kid.arrow_type == ETL_ARROW_UTF8) scan_lengths(ks.lens, ne, blk, tot, (int32_t*)(kf + kid.offsets_off), st);
+          else scan_lengths(ks.lens, ne, blk, tot, (uint64_t*)(kf + kid.offsets_off), st);
         }
       }
       A->kids.push_back(kid);

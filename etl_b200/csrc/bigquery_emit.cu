@@ -15,14 +15,13 @@
 //
 // Passes (one CUDA stream, four syncs: selection, Json sizes when a Json column exists, row count (not for COPY),
 // output size):
-//   1. k_sel_count / k_blk_scan / k_sel_scatter<BigQueryRecords> (emit_scan.cuh): the version's records that give rows,
-//      in record order, and the first record write_events rejects.  COPY: k_copy_sel, no sync.
-//   2. Json (k_json_len / k_json_canon, row_emit_common.cuh): items are (record, Json column, image): the new image's
+//   1. select_rows<BigQueryRecords> (emit_scan.cuh): the version's records that give rows, in record order, and the
+//      first record write_events rejects.  COPY: k_copy_sel, no sync.
+//   2. Json (stage_json, row_emit_common.cuh): items are (record, Json column, image): the new image's
 //      Json cells and the old image's primary-key Json cells, canonicalised once.  The key comparison and the rows read
 //      the canonical text.
 //   3. k_bq_expand (warp per record): 1 or 2 rows; an Update compares its old and new primary-key cells with Cell's
-//      PartialEq, long payloads compared by the warp.  The counts are scanned (k_len_blocks / k_blk_scan64 /
-//      k_offsets) and k_bq_rows writes each row's descriptor and record.
+//      PartialEq, long payloads compared by the warp.  The counts are scanned (scan_lengths, emit_scan.cuh) and k_bq_rows writes each row's descriptor and record.
 //   4. k_bq_size: thread per (row, field) over W = n_cols + 2: the field's bytes; the first value issue by warp-reduced
 //      atomicMin of (row << 32 | column).  k_row_scan (row_emit_common.cuh) turns them into in-row offsets and row
 //      lengths, scanned into u64 row offsets.
@@ -36,7 +35,6 @@
 // spills, as in the RowBinary emitter), k_json_len 22, k_row_scan 24; no other spills.
 #include <cuda_runtime.h>
 
-#include <algorithm>
 #include <vector>
 
 #include "etl_decode.h"
@@ -99,8 +97,6 @@ struct BqParams {
   uint8_t* out;
   unsigned long long* issues;   // kIssue*: (row << 32 | column) of the first value issue, flags, its kind, its element
 };
-
-__device__ __forceinline__ const etl_array_elem* elems_of(const BqParams& P, uint64_t val) { return array_elems(P.heap, val); }
 
 // the cell of column c in image img (0 new, 1 old) of selected record s; false: no such cell (a Delete has no new
 // image, an Insert no old one, an old image only gives the primary-key columns)
@@ -170,18 +166,18 @@ __device__ bool cells_eq_warp(const BqParams& P, uint64_t a, uint64_t b, const u
   if (ta == ETL_CELL_NULL) return true;
   const uint64_t va = P.cell_val[a], vb = P.cell_val[b];
   const uint32_t xa = P.cell_aux[a], xb = P.cell_aux[b];
-  if (ta == ETL_CELL_JSON) return value_eq_warp(ta, 0, stage_rd32(ja), ja + 4, 0, stage_rd32(jb), jb + 4);
+  if (ta == ETL_CELL_JSON) return value_eq_warp(ta, 0, rd32(ja), ja + 4, 0, rd32(jb), jb + 4);
   if (ta != ETL_CELL_ARRAY) return value_eq_warp(ta, va, xa, scalar_payload(P, ta, va), vb, xb, scalar_payload(P, tb, vb));
   if (xa != xb) return false;
-  const etl_array_elem* A = elems_of(P, va);
-  const etl_array_elem* B = elems_of(P, vb);
+  const etl_array_elem* A = array_elems(P.heap, va);
+  const etl_array_elem* B = array_elems(P.heap, vb);
   for (uint32_t k = 0; k < xa; k++) {
     const etl_array_elem ea = A[k], eb = B[k];
     if (ea.tag != eb.tag) return false;
     if (ea.tag == ETL_CELL_NULL) continue;
     bool eq;
     if (ea.tag == ETL_CELL_JSON) {
-      eq = value_eq_warp(ea.tag, 0, stage_rd32(ja), ja + 4, 0, stage_rd32(jb), jb + 4);
+      eq = value_eq_warp(ea.tag, 0, rd32(ja), ja + 4, 0, rd32(jb), jb + 4);
       ja += 4 + ea.aux;
       jb += 4 + eb.aux;
     } else eq = value_eq_warp(ea.tag, ea.val, ea.aux, P.heap + ea.val, eb.val, eb.aux, P.heap + eb.val);
@@ -272,7 +268,7 @@ __device__ __forceinline__ void text_write(uint32_t tag, uint64_t val, uint32_t 
 // element or an element that fails a check
 __device__ uint64_t array_field(const BqParams& P, uint32_t field, uint64_t val, uint32_t aux, const uint8_t* canon, uint8_t* o, bool* issue) {
   if (aux == 0) return 0;
-  const etl_array_elem* E = elems_of(P, val);
+  const etl_array_elem* E = array_elems(P.heap, val);
   const uint32_t ek = reinterpret_cast<const etl_array_hdr*>(P.heap + val)->elem_kind;
   const bool packed = ek == ETL_K_BOOL || ek == ETL_K_I16 || ek == ETL_K_I32 || ek == ETL_K_U32 || ek == ETL_K_I64 ||
                       ek == ETL_K_F32 || ek == ETL_K_F64;
@@ -296,7 +292,7 @@ __device__ uint64_t array_field(const BqParams& P, uint32_t field, uint64_t val,
     const uint8_t* src = P.heap + e.val;
     uint32_t n = e.aux;
     if (e.tag == ETL_CELL_JSON) {
-      n = stage_rd32(canon); src = canon + 4; canon += 4 + e.aux;
+      n = rd32(canon); src = canon + 4; canon += 4 + e.aux;
       if (etl_bq::json_int_bad(src, n)) *issue = true;
     }
     if (e.tag == ETL_CELL_NUMERIC && etl_bq::numeric_scale_bad(P.heap + e.val, e.aux)) *issue = true;
@@ -309,12 +305,6 @@ __device__ uint64_t array_field(const BqParams& P, uint32_t field, uint64_t val,
     at += t;
   }
   return at;
-}
-
-__device__ __forceinline__ void report_min(unsigned long long key, unsigned long long* slot) {
-  if (!__any_sync(kFull, key != ~0ull)) return;
-  for (int d = 16; d > 0; d >>= 1) key = min(key, __shfl_xor_sync(kFull, key, d));
-  if ((threadIdx.x & 31) == 0) atomicMin(slot, key);
 }
 
 // (row, field) → the cell behind a user column; false for a NULL-free absence (a DELETE row's non-key column)
@@ -352,7 +342,7 @@ __global__ void __launch_bounds__(256) k_bq_size(BqParams P) {
           uint32_t n = aux;
           if (tag == ETL_CELL_JSON) {
             const uint8_t* t = canon_of(P, s, j, img);
-            n = stage_rd32(t);
+            n = rd32(t);
             issue = etl_bq::json_int_bad(t + 4, n);
           }
           if (tag == ETL_CELL_NUMERIC) issue = etl_bq::numeric_scale_bad(P.heap + val, aux);
@@ -411,7 +401,7 @@ __global__ void __launch_bounds__(256) k_bq_write(BqParams P) {
         } else {
           uint32_t n = aux;
           const uint8_t* src = nullptr;
-          if (tag == ETL_CELL_JSON) { const uint8_t* t = canon_of(P, s, j, img); n = stage_rd32(t); src = t + 4; }
+          if (tag == ETL_CELL_JSON) { const uint8_t* t = canon_of(P, s, j, img); n = rd32(t); src = t + 4; }
           else if (tag == ETL_CELL_STRING) src = cell_text(P.stream, P.heap, val);
           else if (tag == ETL_CELL_BYTES) src = P.heap + val;
           const uint32_t t = text_len(tag, val, aux, P.heap, n);
@@ -449,7 +439,7 @@ __global__ void k_bq_issue(BqParams P) {
   if (tag == ETL_CELL_NUMERIC) { P.issues[kIssueKind] = ETL_BQ_ISSUE_NUMERIC_SCALE; return; }
   if (tag == ETL_CELL_JSON) { P.issues[kIssueKind] = ETL_BQ_ISSUE_JSON_INTEGER; return; }
   if (tag != ETL_CELL_ARRAY) return;
-  const etl_array_elem* E = elems_of(P, P.cell_val[cell]);
+  const etl_array_elem* E = array_elems(P.heap, P.cell_val[cell]);
   for (uint32_t k = 0; k < aux; k++)
     if (E[k].tag == ETL_CELL_NULL) { P.issues[kIssueKind] = ETL_BQ_ISSUE_ARRAY_NULL; P.issues[kIssueElem] = k; return; }
   const uint8_t* canon = j >= 0 ? canon_of(P, s, j, img) : nullptr;
@@ -458,7 +448,7 @@ __global__ void k_bq_issue(BqParams P) {
       P.issues[kIssueKind] = ETL_BQ_ISSUE_NUMERIC_SCALE; P.issues[kIssueElem] = k; return;
     }
     if (E[k].tag == ETL_CELL_JSON) {
-      const bool bad = etl_bq::json_int_bad(canon + 4, stage_rd32(canon));
+      const bool bad = etl_bq::json_int_bad(canon + 4, rd32(canon));
       canon += 4 + E[k].aux;
       if (bad) { P.issues[kIssueKind] = ETL_BQ_ISSUE_JSON_INTEGER; P.issues[kIssueElem] = k; return; }
     }
@@ -467,11 +457,7 @@ __global__ void k_bq_issue(BqParams P) {
 
 }  // namespace
 
-struct etl_bigquery_batch {
-  uint64_t n_rows = 0, bytes = 0;
-  uint8_t* meta = nullptr;    // device: n_rows + 1 row offsets | n_rows row records
-  uint8_t* data = nullptr;    // device: the serialized messages
-  uint8_t* host = nullptr;    // pinned: meta | data (to_host)
+struct etl_bigquery_batch : RowPayload {
   etl_bigquery_issues issues{};
 };
 
@@ -479,18 +465,13 @@ extern "C" {
 
 int etl_dec_bigquery_emit(const etl_dec_batch* batch, uint32_t schema_index, int to_host, etl_bigquery_batch** out) {
   if (!batch || !out) return ETL_ERR_INVALID_ARG;
-  const uint8_t* dev_stream = etl_dec_batch_device_stream(batch);
-  etl_dec_planes P;
-  etl_dec_summary S;
-  etl_dec_schema_info sc{};
-  if (etl_dec_batch_planes(batch, 0, &P) != ETL_OK || etl_dec_batch_summary(batch, &S) != ETL_OK) return ETL_ERR_INVALID_ARG;
-  const bool copy = P.rec_kind == nullptr;
+  EmitBatch E;
+  if (open_emit_batch(batch, schema_index, &E) != ETL_OK) return ETL_ERR_INVALID_ARG;
+  const etl_dec_planes& P = E.P;
+  const etl_dec_schema_info& sc = E.sc;
+  const bool copy = E.copy;
   const uint8_t* pk = nullptr;
-  if (copy) {
-    if (schema_index != 0 || !etl_copy_batch_columns(batch, &sc.table_id, &sc.col_kind, &sc.n_cols)) return ETL_ERR_INVALID_ARG;
-  } else if (etl_dec_batch_schema(batch, schema_index, &sc) != ETL_OK || !etl_schema_pk_columns(batch, schema_index, &pk)) {
-    return ETL_ERR_INVALID_ARG;
-  }
+  if (!copy && !etl_schema_pk_columns(batch, schema_index, &pk)) return ETL_ERR_INVALID_ARG;
   const uint32_t W = sc.n_cols + 2;
   // column descriptors: primary-key membership and key slot, the Json item index; identity_matches_primary_key
   std::vector<BqCol> cols(sc.n_cols);
@@ -508,28 +489,22 @@ int etl_dec_bigquery_emit(const etl_dec_batch* batch, uint32_t schema_index, int
 
   cudaStream_t st = cudaStreamPerThread;
   etl_bigquery_batch* B = new etl_bigquery_batch();
-  std::vector<void*> scratch;                           // stream-ordered, released on every exit
-  auto salloc = [&](uint64_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMallocAsync(&p, bytes + 64, st) != cudaSuccess) return nullptr;
-    scratch.push_back(p);
-    return p;
-  };
+  Scratch scratch(st);
   auto fail = [&](int rc) {
-    for (void* p : scratch) cudaFreeAsync(p, st);
+    scratch.release();
     cudaStreamSynchronize(st);
     cudaGetLastError();
-    etl_dec_bigquery_free(B);
+    delete B;
     return rc;
   };
-  const uint64_t n_valid = S.first_error.record_index == UINT64_MAX ? P.n_records : std::min<uint64_t>(P.n_records, S.first_error.record_index - S.record_index_base);
+  const uint64_t n_valid = E.n_valid;
   const uint32_t nb = (uint32_t)((n_valid + kSelThreads - 1) / kSelThreads);
-  uint32_t* d_blk = (uint32_t*)salloc((nb + 1) * 4ull);
-  uint64_t* d_cell0 = (uint64_t*)salloc((n_valid + 1) * 8);
-  uint64_t* d_rec = (uint64_t*)salloc((n_valid + 1) * 8);
-  unsigned long long* d_n = (unsigned long long*)salloc(8 * (2 + kIssueSlots));   // records, first invalid | issues
+  uint32_t* d_blk = (uint32_t*)scratch((nb + 1) * 4ull);
+  uint64_t* d_cell0 = (uint64_t*)scratch((n_valid + 1) * 8);
+  uint64_t* d_rec = (uint64_t*)scratch((n_valid + 1) * 8);
+  unsigned long long* d_n = (unsigned long long*)scratch(8 * (2 + kIssueSlots));   // records, first invalid | issues
   const size_t cols_bytes = (sizeof(BqCol) * cols.size() + 7) & ~(size_t)7;
-  uint8_t* d_cols = (uint8_t*)salloc(cols_bytes + 4ull * (json_col.size() + pk_col.size()));
+  uint8_t* d_cols = (uint8_t*)scratch(cols_bytes + 4ull * (json_col.size() + pk_col.size()));
   if (!d_blk || !d_cell0 || !d_rec || !d_n || !d_cols) return fail(ETL_ERR_ALLOC);
   unsigned long long* d_issues = d_n + 2;
   uint32_t* d_json_col = reinterpret_cast<uint32_t*>(d_cols + cols_bytes);
@@ -541,59 +516,35 @@ int etl_dec_bigquery_emit(const etl_dec_batch* batch, uint32_t schema_index, int
       (!pk_col.empty() && cudaMemcpyAsync(d_pk_col, pk_col.data(), 4 * pk_col.size(), cudaMemcpyHostToDevice, st) != cudaSuccess))
     return fail(ETL_ERR_CUDA);
   unsigned long long sel[2] = {0, UINT64_MAX};          // selected records, first invalid record
-  if (copy) {
-    sel[0] = n_valid;
-    if (n_valid) k_copy_sel<<<(uint32_t)((n_valid + 255) / 256), 256, 0, st>>>(n_valid, sc.n_cols, d_cell0, d_rec);
-  } else if (nb) {
-    SelParams Sp{P.rec_kind, P.rec_flags, P.rec_schema, P.rec_cell_base, n_valid, (int32_t)schema_index, identity_is_pk ? 1u : 0u,
-                 sc.n_cols, d_blk, d_cell0, d_rec, d_n};
-    k_sel_count<BigQueryRecords><<<nb, kSelThreads, 0, st>>>(Sp);
-    k_blk_scan<<<1, kSelThreads, 0, st>>>(d_blk, nb, d_n);
-    k_sel_scatter<BigQueryRecords><<<nb, kSelThreads, 0, st>>>(Sp);
-    if (cudaMemcpyAsync(sel, d_n, 16, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-  }
+  const SelParams Sp{P.rec_kind, P.rec_flags, P.rec_schema, P.rec_cell_base, n_valid, (int32_t)schema_index, identity_is_pk ? 1u : 0u,
+                     sc.n_cols, d_blk, d_cell0, d_rec, d_n};
+  if (select_rows<BigQueryRecords>(Sp, copy, n_valid, st, sel) != ETL_OK) return fail(ETL_ERR_CUDA);
   const uint64_t n_sel = sel[0];
   B->issues.first_invalid_record = sel[1];
 
-  BqParams R{P.cell_tag, P.cell_val, P.cell_aux, P.heap, dev_stream, P.rec_kind, P.rec_flags, P.rec_commit_lsn, P.rec_tx_ordinal,
+  BqParams R{P.cell_tag, P.cell_val, P.cell_aux, P.heap, E.stream, P.rec_kind, P.rec_flags, P.rec_commit_lsn, P.rec_tx_ordinal,
              P.rec_cell_base, d_cell0, d_rec, n_sel, reinterpret_cast<const BqCol*>(d_cols), d_json_col, d_pk_col,
              sc.n_cols, W, (uint32_t)json_col.size(), (uint32_t)pk_col.size(), nullptr, nullptr, nullptr, nullptr,
              nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, d_issues};
   // Json: input lengths → item offsets → (sync) canonical text
   const uint64_t n_items = n_sel * 2 * R.n_json;
   if (n_items) {
-    const uint32_t jb = (uint32_t)((n_items + 1023) / 1024);
-    uint32_t* jl = (uint32_t*)salloc(n_items * 4);
-    uint64_t* joff = (uint64_t*)salloc((n_items + 1) * 8);
-    unsigned long long* jblk = (unsigned long long*)salloc((jb + 1) * 8ull);
-    if (!jl || !joff || !jblk) return fail(ETL_ERR_ALLOC);
-    JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, dev_stream, n_items, joff, nullptr, nullptr,
+    JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, E.stream, n_items, nullptr, nullptr, nullptr,
                 d_issues + kIssueFlags, (unsigned long long)kFlagBadJson};
-    k_json_len<BqJsonCells><<<(uint32_t)((n_items + 255) / 256), 256, 0, st>>>(J, BqJsonCells{R}, jl);
-    k_len_blocks<<<jb, 1024, 0, st>>>(jl, n_items, jblk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(jblk, jb, jblk + jb);
-    k_offsets<uint64_t><<<jb, 1024, 0, st>>>(jl, n_items, jblk, joff);
-    unsigned long long jt = 0;
-    if (cudaMemcpyAsync(&jt, jblk + jb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-    R.json_off = joff;
-    J.canon = (uint8_t*)salloc(jt);
-    J.work = (uint32_t*)salloc(16 * jt);
-    if (!J.canon || !J.work) return fail(ETL_ERR_ALLOC);
+    if (int rc = stage_json(scratch, J, BqJsonCells{R}, st)) return fail(rc);
+    R.json_off = J.off;
     R.canon = J.canon;
-    if (jt) k_json_canon<BqJsonCells><<<(uint32_t)((n_items + 127) / 128), 128, 0, st>>>(J, BqJsonCells{R});
   }
   // rows: 1 or 2 per record, scanned (sync); COPY: one per record
   uint64_t n_rows = n_sel;
   if (n_sel && !copy) {
-    const uint32_t sb = (uint32_t)((n_sel + 1023) / 1024);
-    R.sel_cnt = (uint32_t*)salloc(n_sel * 4);
-    uint64_t* row0 = (uint64_t*)salloc((n_sel + 1) * 8);
-    unsigned long long* sblk = (unsigned long long*)salloc((sb + 1) * 8ull);
+    const uint32_t sb = scan_blocks(n_sel);
+    R.sel_cnt = (uint32_t*)scratch(n_sel * 4);
+    uint64_t* row0 = (uint64_t*)scratch((n_sel + 1) * 8);
+    unsigned long long* sblk = (unsigned long long*)scratch((sb + 1) * 8ull);
     if (!R.sel_cnt || !row0 || !sblk) return fail(ETL_ERR_ALLOC);
     k_bq_expand<<<(uint32_t)((n_sel * 32 + 255) / 256), 256, 0, st>>>(R);
-    k_len_blocks<<<sb, 1024, 0, st>>>(R.sel_cnt, n_sel, sblk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(sblk, sb, sblk + sb);
-    k_offsets<uint64_t><<<sb, 1024, 0, st>>>(R.sel_cnt, n_sel, sblk, row0);
+    scan_lengths(R.sel_cnt, n_sel, sblk, sblk + sb, row0, st);
     unsigned long long nr = 0;
     if (cudaMemcpyAsync(&nr, sblk + sb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
     n_rows = nr;
@@ -601,28 +552,25 @@ int etl_dec_bigquery_emit(const etl_dec_batch* batch, uint32_t schema_index, int
   }
   B->n_rows = n_rows;
   R.n_rows = n_rows;
-  const uint64_t meta_bytes = (2 * n_rows + 1) * 8;
-  if (cudaMalloc(&B->meta, meta_bytes) != cudaSuccess) { B->meta = nullptr; return fail(ETL_ERR_ALLOC); }
+  if (cudaMalloc(&B->meta, B->meta_bytes()) != cudaSuccess) { B->meta = nullptr; return fail(ETL_ERR_ALLOC); }
   if (cudaMemsetAsync(B->meta, 0, 8, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
   R.row_off = reinterpret_cast<const uint64_t*>(B->meta);
   R.row_rec = reinterpret_cast<uint64_t*>(B->meta) + n_rows + 1;
   unsigned long long tot[2] = {0, 0};                   // output bytes, issue flags
   if (n_rows) {
-    R.row_desc = (uint64_t*)salloc(n_rows * 8);
+    R.row_desc = (uint64_t*)scratch(n_rows * 8);
     const uint64_t n_cells = n_rows * W;
-    const uint32_t rb = (uint32_t)((n_rows + 1023) / 1024);
-    R.cell_len = (uint32_t*)salloc(n_cells * 4);
-    R.row_len = (uint32_t*)salloc(n_rows * 4);
-    unsigned long long* rblk = (unsigned long long*)salloc((rb + 1) * 8ull);
+    const uint32_t rb = scan_blocks(n_rows);
+    R.cell_len = (uint32_t*)scratch(n_cells * 4);
+    R.row_len = (uint32_t*)scratch(n_rows * 4);
+    unsigned long long* rblk = (unsigned long long*)scratch((rb + 1) * 8ull);
     if (!R.row_desc || !R.cell_len || !R.row_len || !rblk) return fail(ETL_ERR_ALLOC);
     k_bq_rows<<<(uint32_t)((n_sel + 255) / 256), 256, 0, st>>>(R);
     // sizes → in-row offsets → row offsets (sync)
     k_bq_size<<<(uint32_t)((n_cells + 255) / 256), 256, 0, st>>>(R);
     k_row_scan<<<(uint32_t)((n_rows * 32 + 255) / 256), 256, 0, st>>>(R.cell_len, W, n_rows, R.row_len, d_issues + kIssueFlags,
                                                                        (unsigned long long)kFlagRowTooLong);
-    k_len_blocks<<<rb, 1024, 0, st>>>(R.row_len, n_rows, rblk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(rblk, rb, rblk + rb);
-    k_offsets<uint64_t><<<rb, 1024, 0, st>>>(R.row_len, n_rows, rblk, (uint64_t*)B->meta);
+    scan_lengths(R.row_len, n_rows, rblk, rblk + rb, (uint64_t*)B->meta, st);
     if (cudaMemcpyAsync(&tot[0], rblk + rb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
         cudaMemcpyAsync(&tot[1], d_issues + kIssueFlags, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
         cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
@@ -637,14 +585,11 @@ int etl_dec_bigquery_emit(const etl_dec_batch* batch, uint32_t schema_index, int
     k_bq_issue<<<1, 1, 0, st>>>(R);
   }
   if (to_host) {
-    if (cudaHostAlloc((void**)&B->host, meta_bytes + B->bytes + 64, cudaHostAllocDefault) != cudaSuccess) { B->host = nullptr; return fail(ETL_ERR_ALLOC); }
-    if (cudaMemcpyAsync(B->host, B->meta, meta_bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(B->host + meta_bytes, B->data, B->bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
+    if (int rc = B->copy_to_host(st)) return fail(rc);
   }
   unsigned long long iss[kIssueSlots];
   if (cudaMemcpyAsync(iss, d_issues, sizeof iss, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-  for (void* p : scratch) cudaFreeAsync(p, st);
-  scratch.clear();
+  scratch.release();
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
   etl_bq_issue v{UINT64_MAX, UINT32_MAX, UINT32_MAX, 0, 0};
   if (iss[kIssueKey] != ~0ull) {
@@ -657,34 +602,16 @@ int etl_dec_bigquery_emit(const etl_dec_batch* batch, uint32_t schema_index, int
   *out = B;
   return ETL_OK;
 }
-uint64_t etl_dec_bigquery_rows(const etl_bigquery_batch* b) { return b ? b->n_rows : 0; }
-uint64_t etl_dec_bigquery_bytes(const etl_bigquery_batch* b) { return b ? b->bytes : 0; }
-const uint8_t* etl_dec_bigquery_data(const etl_bigquery_batch* b, int host) {
-  if (!b) return nullptr;
-  if (!host) return b->data;
-  return b->host ? b->host + (2 * b->n_rows + 1) * 8 : nullptr;
-}
-const uint64_t* etl_dec_bigquery_row_offsets(const etl_bigquery_batch* b, int host) {
-  if (!b) return nullptr;
-  const uint8_t* base = host ? b->host : b->meta;
-  return base ? reinterpret_cast<const uint64_t*>(base) : nullptr;
-}
-const uint64_t* etl_dec_bigquery_row_records(const etl_bigquery_batch* b, int host) {
-  if (!b) return nullptr;
-  const uint8_t* base = host ? b->host : b->meta;
-  return base ? reinterpret_cast<const uint64_t*>(base) + b->n_rows + 1 : nullptr;
-}
+uint64_t etl_dec_bigquery_rows(const etl_bigquery_batch* b) { return RowPayload::rows_of(b); }
+uint64_t etl_dec_bigquery_bytes(const etl_bigquery_batch* b) { return RowPayload::bytes_of(b); }
+const uint8_t* etl_dec_bigquery_data(const etl_bigquery_batch* b, int host) { return RowPayload::data_of(b, host); }
+const uint64_t* etl_dec_bigquery_row_offsets(const etl_bigquery_batch* b, int host) { return RowPayload::offsets_of(b, host); }
+const uint64_t* etl_dec_bigquery_row_records(const etl_bigquery_batch* b, int host) { return RowPayload::records_of(b, host); }
 int etl_dec_bigquery_issues(const etl_bigquery_batch* b, etl_bigquery_issues* out) {
   if (!b || !out) return ETL_ERR_INVALID_ARG;
   *out = b->issues;
   return ETL_OK;
 }
-void etl_dec_bigquery_free(etl_bigquery_batch* b) {
-  if (!b) return;
-  if (b->meta) cudaFree(b->meta);
-  if (b->data) cudaFree(b->data);
-  if (b->host) cudaFreeHost(b->host);
-  delete b;
-}
+void etl_dec_bigquery_free(etl_bigquery_batch* b) { delete b; }
 
 }  // extern "C"

@@ -21,7 +21,7 @@
 //      ends within its last 5, and the last sequence is literals only.  Lane 0 writes the 9-byte header.
 //   4. k_checksum, a thread per block: CityHash128 v1.0.2 of header + payload, a serial chain over the slot the
 //      compressor just wrote, into the slot's first 16 bytes.
-//   5. k_len_blocks / k_blk_scan64 / k_offsets (emit_scan.cuh) over the block sizes (25 + payload) → block offsets
+//   5. scan_lengths (emit_scan.cuh) over the block sizes (25 + payload) → block offsets
 //      in the output (sync: total), k_ins_off takes each INSERT's offset from its first block, k_gather (a warp per
 //      block) copies the slots into place.
 // Slots: block b whose first byte lies u bytes into the range starts at round_up_16(u + u / 255 + 56 b), which leaves
@@ -31,7 +31,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "etl_decode.h"
 #include "clickhouse_lz4.cuh"
@@ -96,7 +95,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 // the 4 bytes at p of the staged window (word-aligned loads and a funnel shift)
-__device__ __forceinline__ uint32_t rd32(const uint32_t* w, uint32_t p) {
+__device__ __forceinline__ uint32_t window_rd32(const uint32_t* w, uint32_t p) {
   return __funnelshift_r(w[p >> 2], w[(p >> 2) + 1], (p & 3u) * 8u);
 }
 __device__ __forceinline__ uint32_t lz4_hash(uint32_t v) { return (v * 2654435761u) >> (32 - kHashBits); }
@@ -135,12 +134,12 @@ __global__ void __launch_bounds__(32) k_lz4(const uint8_t* data, const uint64_t*
   while (ip < lim) {
     const uint32_t p = ip + lane;
     const bool act = p < lim;
-    const uint32_t v = act ? rd32(words, head + p) : 0u;
+    const uint32_t v = act ? window_rd32(words, head + p) : 0u;
     const uint32_t h = act ? lz4_hash(v) : 0x80000000u | lane;   // inactive lanes: a group of their own
     const unsigned grp = __match_any_sync(kFull, h);
     const unsigned lower = grp & below;
     const uint32_t cand = lower ? ip + 31u - __clz(lower) : act ? table[h] : 0u;
-    const bool m = act && cand < p && p - cand <= 65535u && rd32(words, head + cand) == v;
+    const bool m = act && cand < p && p - cand <= 65535u && window_rd32(words, head + cand) == v;
     const unsigned mb = __ballot_sync(kFull, m);
     const uint32_t f = mb ? __ffs(mb) - 1u : 32u;
     const unsigned ins = __ballot_sync(kFull, act && lane <= f);
@@ -215,15 +214,9 @@ int etl_dec_rowbinary_lz4(const etl_rowbinary_batch* rb, uint64_t row_begin, uin
 
   cudaStream_t st = cudaStreamPerThread;
   etl_rowbinary_lz4* Z = new etl_rowbinary_lz4();
-  std::vector<void*> scratch;                           // stream-ordered, released on every exit
-  auto salloc = [&](uint64_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMallocAsync(&p, bytes + 64, st) != cudaSuccess) return nullptr;
-    scratch.push_back(p);
-    return p;
-  };
+  Scratch scratch(st);
   auto fail = [&](int rc) {
-    for (void* p : scratch) cudaFreeAsync(p, st);
+    scratch.release();
     cudaStreamSynchronize(st);
     cudaGetLastError();
     etl_dec_rowbinary_lz4_free(Z);
@@ -231,9 +224,9 @@ int etl_dec_rowbinary_lz4(const etl_rowbinary_batch* rb, uint64_t row_begin, uin
   };
   // 1. cuts: at most one INSERT per row, and every INSERT but the last holds max_bytes_per_insert bytes or more
   const uint64_t ins_bound = std::min<uint64_t>(row_end - row_begin, emit_bytes / max_bytes_per_insert + 1);
-  uint64_t* d_ins_rows = (uint64_t*)salloc((ins_bound + 1) * 8);
-  uint64_t* d_blk_base = (uint64_t*)salloc((ins_bound + 1) * 8);
-  unsigned long long* d_res = (unsigned long long*)salloc(32);
+  uint64_t* d_ins_rows = (uint64_t*)scratch((ins_bound + 1) * 8);
+  uint64_t* d_blk_base = (uint64_t*)scratch((ins_bound + 1) * 8);
+  unsigned long long* d_res = (unsigned long long*)scratch(32);
   if (!d_ins_rows || !d_blk_base || !d_res) return fail(ETL_ERR_ALLOC);
   unsigned long long res[4] = {0, 0, 0, 0};            // INSERTs, blocks, off[row_begin], off[row_end]
   k_cut<<<1, 1, 0, st>>>(d_off, row_begin, row_end, max_bytes_per_insert, d_ins_rows, d_blk_base, d_res);
@@ -250,21 +243,19 @@ int etl_dec_rowbinary_lz4(const etl_rowbinary_batch* rb, uint64_t row_begin, uin
   uint64_t* d_bstart = nullptr; uint8_t* d_slots = nullptr; uint32_t* d_csize = nullptr; uint64_t* d_boff = nullptr;
   if (nb) {
     // 2-4. block table, compression, checksums
-    d_bstart = (uint64_t*)salloc((nb + 1) * 8);
-    d_csize = (uint32_t*)salloc(nb * 4);
-    d_boff = (uint64_t*)salloc((nb + 1) * 8);
-    d_slots = (uint8_t*)salloc(range + range / 255 + 56 * nb + 32);
-    const uint32_t sb = (uint32_t)((nb + 1023) / 1024);
-    unsigned long long* d_sblk = (unsigned long long*)salloc((sb + 1) * 8ull);
+    d_bstart = (uint64_t*)scratch((nb + 1) * 8);
+    d_csize = (uint32_t*)scratch(nb * 4);
+    d_boff = (uint64_t*)scratch((nb + 1) * 8);
+    d_slots = (uint8_t*)scratch(range + range / 255 + 56 * nb + 32);
+    const uint32_t sb = scan_blocks(nb);
+    unsigned long long* d_sblk = (unsigned long long*)scratch((sb + 1) * 8ull);
     if (!d_bstart || !d_csize || !d_boff || !d_slots || !d_sblk) return fail(ETL_ERR_ALLOC);
     if (cudaFuncSetAttribute(k_lz4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem) != cudaSuccess) return fail(ETL_ERR_CUDA);
     k_blocks<<<(uint32_t)((nb + 256) / 256), 256, 0, st>>>(d_off, d_ins_rows, d_blk_base, n_ins, nb, d_bstart);
     k_lz4<<<(uint32_t)nb, 32, kSmem, st>>>(d_data, d_bstart, d_slots, d_csize);
     k_checksum<<<(uint32_t)((nb + 127) / 128), 128, 0, st>>>(d_bstart, nb, d_slots, d_csize);
     // 5. block offsets (sync: the output size)
-    k_len_blocks<<<sb, 1024, 0, st>>>(d_csize, nb, d_sblk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(d_sblk, sb, d_sblk + sb);
-    k_offsets<uint64_t><<<sb, 1024, 0, st>>>(d_csize, nb, d_sblk, d_boff);
+    scan_lengths(d_csize, nb, d_sblk, d_sblk + sb, d_boff, st);
     k_ins_off<<<(uint32_t)((n_ins + 256) / 256), 256, 0, st>>>(d_blk_base, n_ins, d_boff, ins_off);
     if (cudaMemcpyAsync(&total, d_sblk + sb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
       return fail(ETL_ERR_CUDA);
@@ -279,8 +270,7 @@ int etl_dec_rowbinary_lz4(const etl_rowbinary_batch* rb, uint64_t row_begin, uin
     if (cudaMemcpyAsync(Z->host, Z->meta, meta_bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
         cudaMemcpyAsync(Z->host + meta_bytes, Z->data, total, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
   }
-  for (void* p : scratch) cudaFreeAsync(p, st);
-  scratch.clear();
+  scratch.release();
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
   *out = Z;
   return ETL_OK;

@@ -1567,6 +1567,11 @@ bool etl_copy_batch_pk_columns(const etl_dec_batch* b, const uint8_t** pk) {
   *pk = b->copy_pk.data();
   return true;
 }
+uint64_t etl_batch_valid_records(const etl_dec_batch* b) {
+  const etl_dec_summary& S = b->summary;
+  const uint64_t n = b->dev.n_records;
+  return S.first_error.record_index == UINT64_MAX ? n : std::min<uint64_t>(n, S.first_error.record_index - S.record_index_base);
+}
 bool etl_copy_batch_columns(const etl_dec_batch* b, uint32_t* table_id, const uint8_t** col_kind, uint32_t* n_cols) {
   if (!b || !b->copy) return false;
   *table_id = b->copy_table; *col_kind = b->copy_kinds.data(); *n_cols = (uint32_t)b->copy_kinds.size();

@@ -14,9 +14,9 @@
 // text sizes):
 //   1. k_dl_trunc + scan (emit_scan.cuh): the truncate-free segment of each record.  COPY: none.
 //   2. k_dl_decide (warp per record): the mutation kind, the reject reason, empty partial rows, MF_ARRAY, and the
-//      segment flags behind mixed_versions; the mutations are scanned into place (k_len_blocks / k_blk_scan64 /
-//      k_offsets) and k_dl_scatter writes their records, kinds, segments and LSNs.
-//   3. Json (k_json_len / k_json_canon, row_emit_common.cuh): items (mutation, Json column, image), canonicalised once.
+//      segment flags behind mixed_versions; the mutations are scanned into place (scan_lengths) and k_dl_scatter writes
+//      their records, kinds, segments and LSNs.
+//   3. Json (stage_json, row_emit_common.cuh): items (mutation, Json column, image), canonicalised once.
 //   4. k_dl_size: thread per (text, mutation, column + 1) over the three texts: the piece's bytes (separator, name,
 //      literal); a String / Json value above kLongCell bytes has its quotes counted by the warp.  k_row_scan
 //      (row_emit_common.cuh) turns them into in-text offsets and text lengths, scanned into u64 text offsets.
@@ -34,7 +34,6 @@
 // in the other emitters), k_json_len 22, k_row_scan 24; no other spills and no stack frames.
 #include <cuda_runtime.h>
 
-#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -250,7 +249,7 @@ __device__ uint64_t array_lit(const DlParams& P, uint64_t val, uint32_t aux, con
     if (k) { if (o) { o[at] = ','; o[at + 1] = ' '; } at += 2; }
     const uint8_t* src = P.heap + e.val;
     uint32_t n = e.aux;
-    if (e.tag == ETL_CELL_JSON) { n = stage_rd32(canon); src = canon + 4; canon += 4 + e.aux; }
+    if (e.tag == ETL_CELL_JSON) { n = rd32(canon); src = canon + 4; canon += 4 + e.aux; }
     at += o ? value_write(e.tag, e.val, e.aux, P.heap, src, n, o + at) : value_len(e.tag, e.val, e.aux, P.heap, src, n);
   }
   if (o) o[at] = ']';
@@ -267,7 +266,7 @@ __device__ uint64_t cell_lit(const DlParams& P, uint64_t cell, const uint8_t* ca
   if (tag == ETL_CELL_ARRAY) return array_lit(P, val, aux, canon, o);
   const uint8_t* src = nullptr;
   uint32_t n = aux;
-  if (tag == ETL_CELL_JSON) { n = stage_rd32(canon); src = canon + 4; }
+  if (tag == ETL_CELL_JSON) { n = rd32(canon); src = canon + 4; }
   else if (tag == ETL_CELL_STRING) src = cell_text(P.stream, P.heap, val);
   else if (tag == ETL_CELL_BYTES) src = P.heap + val;
   if (src && n > kLongCell) {
@@ -543,19 +542,13 @@ extern "C" {
 int etl_dec_ducklake_emit(const etl_dec_batch* batch, uint32_t schema_index, const char* const* quoted_names, uint32_t n_names,
                           int to_host, etl_ducklake_batch** out) {
   if (!batch || !out) return ETL_ERR_INVALID_ARG;
-  const uint8_t* dev_stream = etl_dec_batch_device_stream(batch);
-  etl_dec_planes P;
-  etl_dec_summary S;
-  etl_dec_schema_info sc{};
-  if (etl_dec_batch_planes(batch, 0, &P) != ETL_OK || etl_dec_batch_summary(batch, &S) != ETL_OK) return ETL_ERR_INVALID_ARG;
-  const bool copy = P.rec_kind == nullptr;
+  EmitBatch E;
+  if (open_emit_batch(batch, schema_index, &E) != ETL_OK) return ETL_ERR_INVALID_ARG;
+  const etl_dec_planes& P = E.P;
+  const etl_dec_schema_info& sc = E.sc;
+  const bool copy = E.copy;
   const uint8_t* pk = nullptr;
-  if (copy) {
-    if (schema_index != 0 || !etl_copy_batch_columns(batch, &sc.table_id, &sc.col_kind, &sc.n_cols) ||
-        !etl_copy_batch_pk_columns(batch, &pk)) return ETL_ERR_INVALID_ARG;
-  } else if (etl_dec_batch_schema(batch, schema_index, &sc) != ETL_OK) {
-    return ETL_ERR_INVALID_ARG;
-  }
+  if (copy && !etl_copy_batch_pk_columns(batch, &pk)) return ETL_ERR_INVALID_ARG;
   if (n_names != sc.n_cols || (sc.n_cols && !quoted_names)) return ETL_ERR_INVALID_ARG;
   // column descriptors: predicate slot (identity; COPY: primary key), Json item index, quoted names
   std::vector<DlCol> cols(sc.n_cols);
@@ -580,25 +573,19 @@ int etl_dec_ducklake_emit(const etl_dec_batch* batch, uint32_t schema_index, con
   etl_ducklake_batch* B = new etl_ducklake_batch();
   B->copy = copy;
   B->n_cols = sc.n_cols;
-  std::vector<void*> scratch;                           // stream-ordered, released on every exit
-  auto salloc = [&](uint64_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMallocAsync(&p, bytes + 64, st) != cudaSuccess) return nullptr;
-    scratch.push_back(p);
-    return p;
-  };
+  Scratch scratch(st);
   auto fail = [&](int rc) {
-    for (void* p : scratch) cudaFreeAsync(p, st);
+    scratch.release();
     cudaStreamSynchronize(st);
     cudaGetLastError();
     etl_dec_ducklake_free(B);
     return rc;
   };
-  const uint64_t n_valid = S.first_error.record_index == UINT64_MAX ? P.n_records : std::min<uint64_t>(P.n_records, S.first_error.record_index - S.record_index_base);
+  const uint64_t n_valid = E.n_valid;
   const uint32_t W = sc.n_cols + 1;
   const size_t cols_bytes = (sizeof(DlCol) * cols.size() + 7) & ~(size_t)7;
-  uint8_t* d_cols = (uint8_t*)salloc(cols_bytes + 4ull * json_col.size() + names.size());
-  unsigned long long* d_issues = (unsigned long long*)salloc(8 * kIssueSlots);
+  uint8_t* d_cols = (uint8_t*)scratch(cols_bytes + 4ull * json_col.size() + names.size());
+  unsigned long long* d_issues = (unsigned long long*)scratch(8 * kIssueSlots);
   if (cudaMalloc(&B->name_len, 4ull * sc.n_cols + 4) != cudaSuccess) { B->name_len = nullptr; return fail(ETL_ERR_ALLOC); }
   if (!d_cols || !d_issues) return fail(ETL_ERR_ALLOC);
   uint32_t* d_json_col = reinterpret_cast<uint32_t*>(d_cols + cols_bytes);
@@ -611,7 +598,7 @@ int etl_dec_ducklake_emit(const etl_dec_batch* batch, uint32_t schema_index, con
     return fail(ETL_ERR_CUDA);
 
   DlParams R{};
-  R.cell_tag = P.cell_tag; R.cell_val = P.cell_val; R.cell_aux = P.cell_aux; R.heap = P.heap; R.stream = dev_stream;
+  R.cell_tag = P.cell_tag; R.cell_val = P.cell_val; R.cell_aux = P.cell_aux; R.heap = P.heap; R.stream = E.stream;
   R.rec_kind = P.rec_kind; R.rec_flags = P.rec_flags; R.rec_schema = P.rec_schema; R.rec_rel = P.rec_rel;
   R.rec_cell_base = P.rec_cell_base; R.rec_start_lsn = P.rec_start_lsn; R.rec_commit_lsn = P.rec_commit_lsn;
   R.rec_tx_ordinal = P.rec_tx_ordinal;
@@ -621,37 +608,33 @@ int etl_dec_ducklake_emit(const etl_dec_batch* batch, uint32_t schema_index, con
   R.issues = d_issues; R.w = W;
 
   // 1-2. segments, mutations (sync)
-  const uint32_t rb = (uint32_t)((n_valid + 1023) / 1024);
+  const uint32_t rb = scan_blocks(n_valid);
   const uint32_t tb = (uint32_t)((n_valid + 255) / 256);
   uint64_t n_mut = 0;
   unsigned long long iss[kIssueSlots] = {~0ull, ~0ull, 0};
   if (n_valid) {
-    uint32_t* lens = (uint32_t*)salloc(n_valid * 4);
-    unsigned long long* blk = (unsigned long long*)salloc((rb + 1) * 8ull);
-    R.seg_flags = (uint32_t*)salloc((n_valid + 1) * 4);
-    R.rec_mkind = (uint8_t*)salloc(n_valid);
-    uint64_t* mpos = (uint64_t*)salloc((n_valid + 1) * 8);
+    uint32_t* lens = (uint32_t*)scratch(n_valid * 4);
+    unsigned long long* blk = (unsigned long long*)scratch((rb + 1) * 8ull);
+    R.seg_flags = (uint32_t*)scratch((n_valid + 1) * 4);
+    R.rec_mkind = (uint8_t*)scratch(n_valid);
+    uint64_t* mpos = (uint64_t*)scratch((n_valid + 1) * 8);
     if (!lens || !blk || !R.seg_flags || !R.rec_mkind || !mpos) return fail(ETL_ERR_ALLOC);
     if (cudaMemsetAsync(R.seg_flags, 0, (n_valid + 1) * 4, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
     if (!copy) {
-      uint64_t* seg = (uint64_t*)salloc((n_valid + 1) * 8);
+      uint64_t* seg = (uint64_t*)scratch((n_valid + 1) * 8);
       if (!seg) return fail(ETL_ERR_ALLOC);
       k_dl_trunc<<<tb, 256, 0, st>>>(R, lens);
-      k_len_blocks<<<rb, 1024, 0, st>>>(lens, n_valid, blk);
-      k_blk_scan64<<<1, 1024, 0, st>>>(blk, rb, blk + rb);
-      k_offsets<uint64_t><<<rb, 1024, 0, st>>>(lens, n_valid, blk, seg);
+      scan_lengths(lens, n_valid, blk, blk + rb, seg, st);
       R.seg_off = seg;
     } else {
-      uint64_t* seg = (uint64_t*)salloc((n_valid + 1) * 8);
+      uint64_t* seg = (uint64_t*)scratch((n_valid + 1) * 8);
       if (!seg || cudaMemsetAsync(seg, 0, (n_valid + 1) * 8, st) != cudaSuccess) return fail(ETL_ERR_ALLOC);
       R.seg_off = seg;
     }
-    R.rec_mut = (uint32_t*)salloc(n_valid * 4);
+    R.rec_mut = (uint32_t*)scratch(n_valid * 4);
     if (!R.rec_mut) return fail(ETL_ERR_ALLOC);
     k_dl_decide<<<(uint32_t)((n_valid * 32 + 255) / 256), 256, 0, st>>>(R);
-    k_len_blocks<<<rb, 1024, 0, st>>>(R.rec_mut, n_valid, blk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(blk, rb, blk + rb);
-    k_offsets<uint64_t><<<rb, 1024, 0, st>>>(R.rec_mut, n_valid, blk, mpos);
+    scan_lengths(R.rec_mut, n_valid, blk, blk + rb, mpos, st);
     R.mut_pos = mpos;
     k_dl_mixed<<<(uint32_t)((n_valid + 1 + 255) / 256), 256, 0, st>>>(R.seg_flags, n_valid + 1, d_issues + kIssueFlags);
     unsigned long long nm = 0;
@@ -682,44 +665,28 @@ int etl_dec_ducklake_emit(const etl_dec_batch* batch, uint32_t schema_index, con
   // 3. Json: input lengths → item offsets → (sync) canonical text
   const uint64_t n_items = n_mut * 2 * R.n_json;
   if (n_items) {
-    const uint32_t jb = (uint32_t)((n_items + 1023) / 1024);
-    uint32_t* jl = (uint32_t*)salloc(n_items * 4);
-    uint64_t* joff = (uint64_t*)salloc((n_items + 1) * 8);
-    unsigned long long* jblk = (unsigned long long*)salloc((jb + 1) * 8ull);
-    if (!jl || !joff || !jblk) return fail(ETL_ERR_ALLOC);
-    JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, dev_stream, n_items, joff, nullptr, nullptr,
+    JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, E.stream, n_items, nullptr, nullptr, nullptr,
                 d_issues + kIssueFlags, (unsigned long long)kFlagBadJson};
-    k_json_len<DlJsonCells><<<(uint32_t)((n_items + 255) / 256), 256, 0, st>>>(J, DlJsonCells{R}, jl);
-    k_len_blocks<<<jb, 1024, 0, st>>>(jl, n_items, jblk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(jblk, jb, jblk + jb);
-    k_offsets<uint64_t><<<jb, 1024, 0, st>>>(jl, n_items, jblk, joff);
-    unsigned long long jt = 0;
-    if (cudaMemcpyAsync(&jt, jblk + jb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-    R.json_off = joff;
-    J.canon = (uint8_t*)salloc(jt);
-    J.work = (uint32_t*)salloc(16 * jt);
-    if (!J.canon || !J.work) return fail(ETL_ERR_ALLOC);
+    if (int rc = stage_json(scratch, J, DlJsonCells{R}, st)) return fail(rc);
+    R.json_off = J.off;
     R.canon = J.canon;
-    if (jt) k_json_canon<DlJsonCells><<<(uint32_t)((n_items + 127) / 128), 128, 0, st>>>(J, DlJsonCells{R});
   }
 
   // 4. sizes → in-text offsets → text offsets (sync)
   unsigned long long tot[4] = {0, 0, 0, 0};             // bytes of each text, flags
   if (n_mut) {
     const uint64_t n_pieces = 3 * n_mut * W;
-    const uint32_t mb = (uint32_t)((n_mut + 1023) / 1024);
-    R.cell_len = (uint32_t*)salloc(n_pieces * 4);
-    uint32_t* tlen = (uint32_t*)salloc(n_mut * 4);
-    unsigned long long* mblk = (unsigned long long*)salloc(3 * (mb + 1) * 8ull);
+    const uint32_t mb = scan_blocks(n_mut);
+    R.cell_len = (uint32_t*)scratch(n_pieces * 4);
+    uint32_t* tlen = (uint32_t*)scratch(n_mut * 4);
+    unsigned long long* mblk = (unsigned long long*)scratch(3 * (mb + 1) * 8ull);
     if (!R.cell_len || !tlen || !mblk) return fail(ETL_ERR_ALLOC);
     k_dl_size<<<(uint32_t)((n_pieces + 255) / 256), 256, 0, st>>>(R);
     for (int t = 0; t < 3; t++) {
       unsigned long long* tb_ = mblk + t * (mb + 1);
       k_row_scan<<<(uint32_t)((n_mut * 32 + 255) / 256), 256, 0, st>>>(R.cell_len + t * n_mut * W, W, n_mut, tlen, d_issues + kIssueFlags,
                                                                         (unsigned long long)kFlagTextTooLong);
-      k_len_blocks<<<mb, 1024, 0, st>>>(tlen, n_mut, tb_);
-      k_blk_scan64<<<1, 1024, 0, st>>>(tb_, mb, tb_ + mb);
-      k_offsets<uint64_t><<<mb, 1024, 0, st>>>(tlen, n_mut, tb_, const_cast<uint64_t*>(R.text_off[t]));
+      scan_lengths(tlen, n_mut, tb_, tb_ + mb, const_cast<uint64_t*>(R.text_off[t]), st);
       if (cudaMemcpyAsync(&tot[t], tb_ + mb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
     }
     if (cudaMemcpyAsync(&tot[3], d_issues + kIssueFlags, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
@@ -755,8 +722,7 @@ int etl_dec_ducklake_emit(const etl_dec_batch* batch, uint32_t schema_index, con
       at += B->bytes[t];
     }
   }
-  for (void* p : scratch) cudaFreeAsync(p, st);
-  scratch.clear();
+  scratch.release();
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
   *out = B;
   return ETL_OK;
@@ -795,15 +761,9 @@ int etl_dec_ducklake_sub_batches(etl_ducklake_batch* b, const uint8_t* table_nam
   if (!b || !out || !n || b->copy || (name_len && !table_name)) return ETL_ERR_INVALID_ARG;
   cudaStream_t st = cudaStreamPerThread;
   const uint64_t nm = b->n_mut;
-  std::vector<void*> scratch;
-  auto salloc = [&](uint64_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMallocAsync(&p, bytes + 64, st) != cudaSuccess) return nullptr;
-    scratch.push_back(p);
-    return p;
-  };
+  Scratch scratch(st);
   auto done = [&](int rc) {
-    for (void* p : scratch) cudaFreeAsync(p, st);
+    scratch.release();
     if (cudaStreamSynchronize(st) != cudaSuccess && rc == ETL_OK) rc = ETL_ERR_CUDA;
     if (cudaGetLastError() != cudaSuccess && rc == ETL_OK) rc = ETL_ERR_CUDA;
     return rc;
@@ -817,12 +777,12 @@ int etl_dec_ducklake_sub_batches(etl_ducklake_batch* b, const uint8_t* table_nam
   S.key_commit = last_key ? last_key[0] : 0; S.key_tx = last_key ? last_key[1] : 0;
   uint64_t n_chunks = 0;
   if (nm) {
-    const uint32_t tb = (uint32_t)((nm + 255) / 256), mb = (uint32_t)((nm + 1023) / 1024);
-    uint8_t* tname = (uint8_t*)salloc(name_len);
-    S.first = (unsigned long long*)salloc(8);
-    S.start = (uint32_t*)salloc(nm * 4);
-    uint64_t* chunk_of = (uint64_t*)salloc((nm + 1) * 8);
-    unsigned long long* blk = (unsigned long long*)salloc((mb + 1) * 8ull);
+    const uint32_t tb = (uint32_t)((nm + 255) / 256), mb = scan_blocks(nm);
+    uint8_t* tname = (uint8_t*)scratch(name_len);
+    S.first = (unsigned long long*)scratch(8);
+    S.start = (uint32_t*)scratch(nm * 4);
+    uint64_t* chunk_of = (uint64_t*)scratch((nm + 1) * 8);
+    unsigned long long* blk = (unsigned long long*)scratch((mb + 1) * 8ull);
     if (!tname || !S.first || !S.start || !chunk_of || !blk) return done(ETL_ERR_ALLOC);
     S.table_name = tname;
     S.chunk_of = chunk_of;
@@ -830,9 +790,7 @@ int etl_dec_ducklake_sub_batches(etl_ducklake_batch* b, const uint8_t* table_nam
         cudaMemsetAsync(S.first, last_key ? 0xff : 0, 8, st) != cudaSuccess) return done(ETL_ERR_CUDA);
     if (last_key) k_dl_first_kept<<<tb, 256, 0, st>>>(S);
     k_dl_chunk_mark<<<tb, 256, 0, st>>>(S);
-    k_len_blocks<<<mb, 1024, 0, st>>>(S.start, nm, blk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(blk, mb, blk + mb);
-    k_offsets<uint64_t><<<mb, 1024, 0, st>>>(S.start, nm, blk, chunk_of);
+    scan_lengths(S.start, nm, blk, blk + mb, chunk_of, st);
     unsigned long long nc = 0;
     if (cudaMemcpyAsync(&nc, blk + mb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return done(ETL_ERR_CUDA);
     n_chunks = nc;

@@ -34,7 +34,7 @@
 //   4b. Page index (ETL_PQ_PAGE_INDEX).  k_index<false>, a warp per chunk with lanes over its data pages: each page's
 //      ColumnIndex entry (null flag, bounds truncated by index_min / index_max, null count) and PageLocation sizes, the
 //      boundary order from adjacent non-null pages' untruncated bounds, the chunk's ColumnIndex / OffsetIndex lengths;
-//      one k_blk_scan64 over the 2 × chunks lengths places them behind 4 + data_end (read on the device);
+//      one k_blk_scan over the 2 × chunks lengths places them behind 4 + data_end (read on the device);
 //      k_index<true> writes them and their offsets into the chunk records.  k_row_max (before SYNC 1) bounds an
 //      untruncated byte-array maximum by the leaf's longest row.
 //      SYNC 2 copies the chunk and leaf records back.
@@ -1059,7 +1059,7 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   const uint64_t nr1 = (uint64_t)nL * (n + 1);
   uint32_t* d_len = (uint32_t*)dalloc(3 * nr1 * 4);
   uint64_t* d_pre = (uint64_t*)dalloc(3 * nr1 * 8);
-  const uint32_t lb = (uint32_t)((n + 1023) / 1024);
+  const uint32_t lb = scan_blocks(n);
   unsigned long long* d_blk = (unsigned long long*)dalloc(3ull * nL * (lb + 1) * 8);
   unsigned long long* d_tot = (unsigned long long*)dalloc(3ull * nL * 8);
   unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull + 4ull * nL);   // | ETL_PQ_PAGE_INDEX: k_row_max
@@ -1079,10 +1079,7 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
       for (uint32_t l = 0; l < nL; l++) {
         const uint64_t at = (uint64_t)(s * nL + l);
         uint32_t* lens = d_len + s * nr1 + (uint64_t)l * (n + 1);
-        unsigned long long* blk = d_blk + at * (lb + 1);
-        k_len_blocks<<<lb, 1024, 0, st>>>(lens, n, blk);
-        k_blk_scan64<<<1, 1024, 0, st>>>(blk, lb, d_tot + at);
-        k_offsets<uint64_t><<<lb, 1024, 0, st>>>(lens, n, blk, d_pre + s * nr1 + (uint64_t)l * (n + 1));
+        scan_lengths(lens, n, d_blk + at * (lb + 1), d_tot + at, d_pre + s * nr1 + (uint64_t)l * (n + 1), st);
       }
     k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
     if (pidx) k_row_max<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, n, vb, d_vmax);
@@ -1188,7 +1185,7 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   unsigned long long* d_dblk = nullptr;
   uint32_t *d_tab = nullptr, *d_dpos = nullptr, *d_dflag = nullptr, *d_desz = nullptr, *d_dhead = nullptr;
   uint64_t *d_dfirst = nullptr, *d_desum = nullptr;
-  const uint32_t dlb = (uint32_t)((d_maxI + 1023) / 1024);
+  const uint32_t dlb = scan_blocks(d_maxI);
   if (d_items && P) {
     d_dch = (DictChunk*)dalloc(sizeof(DictChunk) * n_chunks);
     d_tabn = (unsigned long long*)dalloc(8 * (n_chunks + 1ull));
@@ -1223,21 +1220,15 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
     auto fill_scan = [&](int which, uint64_t* dst) {
       k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, dst);
-      k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)dst, (uint32_t)(P + 1), d_stot + which);
+      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)dst, (uint32_t)(P + 1), d_stot + which);
     };
     fill_scan(0, uslot);
     if (d_dch) {
       // dictionaries: tables, inserts, first-occurrence flags and their scans, decisions, dictionary pages
       k_dict_setup<<<(n_chunks + 256) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, n, NN, d_pbase, d_dch, d_tabn);
-      k_blk_scan64<<<1, 1024, 0, st>>>(d_tabn, n_chunks + 1, d_stot + 4);
+      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_tabn, n_chunks + 1, d_stot + 4);
       k_dict_place<<<(n_chunks + 255) / 256, 256, 0, st>>>(n_chunks, d_tabn, d_dch);
       CK(cudaMemsetAsync(d_tab, 0xff, 4 * d_slots, st));
-      auto scan = [&](const uint32_t* lens, uint64_t cnt, uint64_t* dst) {
-        const uint32_t nb = (uint32_t)((cnt + 1023) / 1024);
-        k_len_blocks<<<nb, 1024, 0, st>>>(lens, cnt, d_dblk);
-        k_blk_scan64<<<1, 1024, 0, st>>>(d_dblk, nb, d_stot + 4);
-        k_offsets<uint64_t><<<nb, 1024, 0, st>>>(lens, cnt, d_dblk, dst);
-      };
       for (uint32_t l = 0; l < nL; l++) {
         if (!has_dict(l)) continue;
         const uint64_t I = tot[l];
@@ -1245,8 +1236,8 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
         k_dict_insert<<<std::min<uint32_t>(kInsBlocks, ib), kInsThreads, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, d_dch, d_tab, d_dpos);
         const bool bytes = hl[l].atype == ETL_ARROW_UTF8 || hl[l].atype == ETL_ARROW_LARGE_BINARY;
         k_dict_mark<<<ib, 256, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, I, d_dch, d_tab, d_dpos, d_dflag, bytes ? d_desz : nullptr);
-        scan(d_dflag + hl[l].dscr, I, d_dfirst + hl[l].dscr);
-        if (bytes) scan(d_desz + hl[l].dscr, I, d_desum + hl[l].dscr);
+        scan_lengths(d_dflag + hl[l].dscr, I, d_dblk, d_stot + 4, d_dfirst + hl[l].dscr, st);
+        if (bytes) scan_lengths(d_desz + hl[l].dscr, I, d_dblk, d_stot + 4, d_desum + hl[l].dscr, st);
       }
       k_dict_finish<<<(n_chunks + 255) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, d_dfirst, d_desum, d_dch, d_pages);
       for (uint32_t l = 0; l < nL; l++)
@@ -1264,14 +1255,14 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     }
     k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, snappy, fbase, d_fsz, foff, d_dch);
     CK(cudaMemsetAsync(foff + P, 0, 8, st));
-    k_blk_scan64<<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
+    k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
     k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, snappy, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
     k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout, d_dch);
     if (d_ix) {
       // page index: sizes and boundary orders, their places behind the pages, the bytes
       const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
       k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, Fo->dev, d_cout);
-      k_blk_scan64<<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
+      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
       k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, Fo->dev, d_cout);
     }
   }
@@ -1358,4 +1349,5 @@ void etl_dec_parquet_free(etl_parquet_file* f) {
 //   k_dict_finish 22 / 0 / 0  k_dict_page 32 / 0 / 0
 //   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)
 //   k_row_max 12 / 0 / 0   k_index<false> 72 / 0 / 40 B and k_index<true> 64 / 0 / 80 B (a fixed-width bound's bytes)
-//   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan64 32 / 8192 B, k_offsets<uint64_t> 18 / 8192 B
+//   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan<unsigned long long> 32 / 8192 B,
+//   k_offsets<uint64_t> 18 / 8192 B

@@ -1,20 +1,23 @@
-// row_emit_common.cuh — the pieces the row-payload emitters (rowbinary_emit.cu, bigquery_emit.cu) share: the Json
-// canonicalisation staging and the warp-per-row scan of cell lengths.  Each emitter includes it once; the kernels have
-// internal linkage, so every translation unit gets its own copy.
+// row_emit_common.cuh — the pieces the row-payload emitters (rowbinary_emit.cu, bigquery_emit.cu, ducklake_emit.cu)
+// share: the cell readers, the warp-reduced issue report, the Json canonicalisation staging (stage_json), the
+// warp-per-row scan of cell lengths, and the result buffers of a row payload (RowPayload).  Each emitter includes it
+// once; the kernels have internal linkage, so every translation unit gets its own copy.
 //
 // Json staging: an emitter numbers its Json "items" (RowBinary: (row, Json column); BigQuery: (record, Json column,
 // image)) and passes a locator, a default-copyable functor with
 //   __device__ bool operator()(uint64_t item, uint64_t* cell) const
 // that gives the cell behind an item (false: no cell).  k_json_len sizes each item at 4 + input bytes per document (the
-// Json cell, or each Json element of an array cell); the emitter scans those lengths into item offsets, and
+// Json cell, or each Json element of an array cell); stage_json scans those lengths into item offsets, and
 // k_json_canon writes every document as [u32 canonical length][text] (etl_fmt::json_canon) at its item's offset.  The
 // canonical text is never longer than the input, so the records of an item are walked with the input lengths.
 #pragma once
+#include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "etl_decode.h"
 #include "arrow_format.cuh"
 #include "rowbinary_format.cuh"
+#include "emit_scan.cuh"
 
 namespace {
 
@@ -27,13 +30,19 @@ struct JsonStage {
   unsigned long long bad_flag;
 };
 
-__device__ __forceinline__ uint32_t stage_rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
+__device__ __forceinline__ uint32_t rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
 // a String / Json cell's text: a span of the staged stream, or of the heap (COPY values that needed unescaping)
 __device__ __forceinline__ const uint8_t* cell_text(const uint8_t* stream, const uint8_t* heap, uint64_t val) {
   return val & ETL_COPY_VAL_IN_HEAP ? heap + (val & ~ETL_COPY_VAL_IN_HEAP) : stream + val;
 }
 __device__ __forceinline__ const etl_array_elem* array_elems(const uint8_t* heap, uint64_t val) {
   return reinterpret_cast<const etl_array_elem*>(heap + val + sizeof(etl_array_hdr));
+}
+// the smallest key of the warp (~0: none) into *slot by one atomicMin
+__device__ __forceinline__ void report_min(unsigned long long key, unsigned long long* slot) {
+  if (!__any_sync(0xffffffffu, key != ~0ull)) return;
+  for (int d = 16; d > 0; d >>= 1) key = min(key, __shfl_xor_sync(0xffffffffu, key, d));
+  if ((threadIdx.x & 31) == 0) atomicMin(slot, key);
 }
 
 template <class Locate>
@@ -74,6 +83,29 @@ __global__ void __launch_bounds__(128) k_json_canon(JsonStage J, Locate L) {
   }
 }
 
+// the Json items of J (n_items, flags, the planes): input lengths → item offsets J.off → (sync) canonical text J.canon,
+// with its node scratch J.work.  ETL_OK, ETL_ERR_ALLOC or ETL_ERR_CUDA
+template <class Locate>
+int stage_json(Scratch& scratch, JsonStage& J, Locate L, cudaStream_t st) {
+  const uint64_t n = J.n_items;
+  const uint32_t nb = scan_blocks(n);
+  uint32_t* lens = (uint32_t*)scratch(n * 4);
+  uint64_t* off = (uint64_t*)scratch((n + 1) * 8);
+  unsigned long long* blk = (unsigned long long*)scratch((nb + 1) * 8ull);
+  if (!lens || !off || !blk) return ETL_ERR_ALLOC;
+  J.off = off;
+  k_json_len<Locate><<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(J, L, lens);
+  scan_lengths(lens, n, blk, blk + nb, off, st);
+  unsigned long long total = 0;
+  if (cudaMemcpyAsync(&total, blk + nb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+    return ETL_ERR_CUDA;
+  J.canon = (uint8_t*)scratch(total);
+  J.work = (uint32_t*)scratch(16 * total);
+  if (!J.canon || !J.work) return ETL_ERR_ALLOC;
+  if (total) k_json_canon<Locate><<<(uint32_t)((n + 127) / 128), 128, 0, st>>>(J, L);
+  return ETL_OK;
+}
+
 // warp per row: the row's w cell lengths (cell_len[row * w ..]) → offsets inside the row, and the row's length; a row
 // of 4 GiB or more ORs too_long into *flags
 __global__ void __launch_bounds__(256) k_row_scan(uint32_t* cell_len, uint32_t w, uint64_t n_rows, uint32_t* row_len,
@@ -101,3 +133,43 @@ __global__ void __launch_bounds__(256) k_row_scan(uint32_t* cell_len, uint32_t w
 }
 
 }  // namespace
+
+// the result of a row-payload emit (etl_rowbinary_batch, etl_bigquery_batch): the rows' offsets and records, the bytes
+struct RowPayload {
+  uint64_t n_rows = 0, bytes = 0;
+  uint8_t* meta = nullptr;    // device: n_rows + 1 row offsets | n_rows row records
+  uint8_t* data = nullptr;    // device: the payload
+  uint8_t* host = nullptr;    // pinned: meta | data (to_host)
+  RowPayload() = default;
+  RowPayload(const RowPayload&) = delete;
+  RowPayload& operator=(const RowPayload&) = delete;
+  ~RowPayload() {
+    if (meta) cudaFree(meta);
+    if (data) cudaFree(data);
+    if (host) cudaFreeHost(host);
+  }
+  uint64_t meta_bytes() const { return (2 * n_rows + 1) * 8; }
+  // pinned meta | data, copied on st
+  int copy_to_host(cudaStream_t st) {
+    if (cudaHostAlloc((void**)&host, meta_bytes() + bytes + 64, cudaHostAllocDefault) != cudaSuccess) { host = nullptr; return ETL_ERR_ALLOC; }
+    if (cudaMemcpyAsync(host, meta, meta_bytes(), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(host + meta_bytes(), data, bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) return ETL_ERR_CUDA;
+    return ETL_OK;
+  }
+  static uint64_t rows_of(const RowPayload* b) { return b ? b->n_rows : 0; }
+  static uint64_t bytes_of(const RowPayload* b) { return b ? b->bytes : 0; }
+  static const uint8_t* data_of(const RowPayload* b, int host) {
+    if (!b) return nullptr;
+    if (!host) return b->data;
+    return b->host ? b->host + b->meta_bytes() : nullptr;
+  }
+  static const uint64_t* offsets_of(const RowPayload* b, int host) {
+    if (!b) return nullptr;
+    const uint8_t* base = host ? b->host : b->meta;
+    return base ? reinterpret_cast<const uint64_t*>(base) : nullptr;
+  }
+  static const uint64_t* records_of(const RowPayload* b, int host) {
+    const uint64_t* off = offsets_of(b, host);
+    return off ? off + b->n_rows + 1 : nullptr;
+  }
+};

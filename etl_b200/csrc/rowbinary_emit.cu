@@ -11,16 +11,16 @@
 // columns are the schema's, then cdc_operation (String) and cdc_lsn (UInt64).  Values follow the cell's variant.
 //
 // Passes (one CUDA stream, three syncs: selection, Json sizes when a Json column exists, output size):
-//   1. k_sel_count / k_blk_scan / k_sel_scatter<ClickHouseRows> (emit_scan.cuh): rows in record order, first partial
-//      update.  COPY: k_copy_sel, no sync.
-//   2. Json (k_json_len / k_json_canon, row_emit_common.cuh): every Json cell and Json array element is canonicalised
+//   1. select_rows<ClickHouseRows> (emit_scan.cuh): rows in record order, first partial update.  COPY: k_copy_sel, no
+//      sync.
+//   2. Json (stage_json, row_emit_common.cuh): every Json cell and Json array element is canonicalised
 //      once (etl_fmt::json_canon) into scratch laid out per item (row, Json column) from a scan of the input lengths:
 //      [u32 canonical length][text] per document, each record 4 + input bytes long (the canonical text is never longer
 //      than the input).
 //   3. k_rb_size: thread per (row, column) over W = n_cols + 2 in row-major order: the cell's byte length with its
 //      marker; the first Date32 violation and the first NULL under a cleared flag by warp-reduced atomicMin.
 //   4. k_row_scan (warp per row, row_emit_common.cuh): lengths → u32 in-row cell offsets + the row's length; the row
-//      lengths are scanned into u64 row offsets (k_len_blocks / k_blk_scan64 / k_offsets); the total sizes the output.
+//      lengths are scanned into u64 row offsets (scan_lengths, emit_scan.cuh); the total sizes the output.
 //   5. k_rb_write: thread per (row, column), so consecutive lanes store adjacent bytes of a row; String / Json / hex
 //      payloads above kLongCell bytes are copied by the whole warp.  k_rb_date_elem finds the element of an array
 //      Date32 violation.
@@ -28,7 +28,6 @@
 // column) + 8 B per item + 17 B per input Json byte.  Scratch is stream-ordered (cudaMallocAsync), the output is not.
 #include <cuda_runtime.h>
 
-#include <algorithm>
 #include <vector>
 
 #include "etl_decode.h"
@@ -79,21 +78,13 @@ struct RbParams {
   const uint64_t* row_cell0; const uint64_t* row_rec; uint64_t n_rows;
   const RbCol* cols; const uint32_t* json_col;   // W entries; n_json column indices
   uint32_t n_cols, w, n_ident, n_json;
-  const uint64_t* json_off; uint8_t* canon; uint32_t* work;   // per Json item: offset of its records in canon
+  const uint64_t* json_off; uint8_t* canon;   // per Json item: offset of its records in canon
   uint32_t* cell_len;        // n_rows * w: lengths, then offsets inside the row
   uint32_t* row_len;
   const uint64_t* row_off;   // n_rows + 1
   uint8_t* out;
   unsigned long long* issues;   // kIssue*: (row << 32 | column) of the first Date32 / NULL issue, flags, element
 };
-
-__device__ __forceinline__ uint32_t rd32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
-__device__ __forceinline__ const uint8_t* text_of(const RbParams& P, uint64_t val) {
-  return val & ETL_COPY_VAL_IN_HEAP ? P.heap + (val & ~ETL_COPY_VAL_IN_HEAP) : P.stream + val;
-}
-__device__ __forceinline__ const etl_array_elem* elems_of(const RbParams& P, uint64_t val) {
-  return reinterpret_cast<const etl_array_elem*>(P.heap + val + sizeof(etl_array_hdr));
-}
 
 // the cell behind column c of row `row`: kFromCell and its index, or a key image's kKeyNull / kKeyDefault
 __device__ __forceinline__ uint32_t cell_at(const RbParams& P, uint64_t row, uint32_t c, uint64_t* cell) {
@@ -175,7 +166,7 @@ __device__ __forceinline__ uint64_t scalar_write(uint32_t tag, uint64_t val, uin
 // an array value: varint(n), then every element as Nullable (encoding.rs:238-244).  `canon` walks the item's Json
 // records (Json elements).  Sizing when o == NULL; *bad_date = first element out of the Date32 range
 __device__ uint64_t array_value(const RbParams& P, uint64_t val, uint32_t aux, const uint8_t* canon, uint8_t* o, uint32_t* bad_date) {
-  const etl_array_elem* E = elems_of(P, val);
+  const etl_array_elem* E = array_elems(P.heap, val);
   uint64_t len = o ? etl_rb::varint_write(aux, o) : etl_rb::varint_len(aux);
   for (uint32_t k = 0; k < aux; k++) {
     const etl_array_elem e = E[k];
@@ -188,12 +179,6 @@ __device__ uint64_t array_value(const RbParams& P, uint64_t val, uint32_t aux, c
     else len += 1 + scalar_len(e.tag, e.val, e.aux, P.heap, n);
   }
   return len;
-}
-
-__device__ __forceinline__ void report_min(unsigned long long key, unsigned long long* slot) {
-  if (!__any_sync(kFull, key != ~0ull)) return;
-  for (int d = 16; d > 0; d >>= 1) key = min(key, __shfl_xor_sync(kFull, key, d));
-  if ((threadIdx.x & 31) == 0) atomicMin(slot, key);
 }
 
 // ---------------------------------------------------------------- Json
@@ -210,7 +195,7 @@ struct RbJsonCells {
 // the payload of a String / Json / Bytes scalar cell
 __device__ __forceinline__ const uint8_t* payload(const RbParams& P, uint64_t row, const RbCol& col, uint32_t tag, uint64_t val, uint32_t* n) {
   if (tag == ETL_CELL_JSON) { const uint8_t* r = P.canon + P.json_off[row * P.n_json + col.json]; *n = rd32(r); return r + 4; }
-  if (tag == ETL_CELL_STRING) return text_of(P, val);
+  if (tag == ETL_CELL_STRING) return cell_text(P.stream, P.heap, val);
   return P.heap + val;
 }
 
@@ -312,18 +297,14 @@ __global__ void k_rb_date_elem(RbParams P) {
   const uint32_t c = (uint32_t)(key & 0xffffffffu);
   uint64_t cell = 0;
   if (cell_at(P, row, c, &cell) != kFromCell || P.cell_tag[cell] != ETL_CELL_ARRAY) return;
-  const etl_array_elem* E = elems_of(P, P.cell_val[cell]);
+  const etl_array_elem* E = array_elems(P.heap, P.cell_val[cell]);
   for (uint32_t k = 0; k < P.cell_aux[cell]; k++)
     if (E[k].tag == ETL_CELL_DATE && !etl_rb::date32_ok((int64_t)E[k].val)) { P.issues[kIssueElem] = k; return; }
 }
 
 }  // namespace
 
-struct etl_rowbinary_batch {
-  uint64_t n_rows = 0, bytes = 0;
-  uint8_t* meta = nullptr;    // device: n_rows + 1 row offsets | n_rows row records
-  uint8_t* data = nullptr;    // device: the RowBinary bytes
-  uint8_t* host = nullptr;    // pinned: meta | data (to_host)
+struct etl_rowbinary_batch : RowPayload {
   etl_rowbinary_issues issues{};
 };
 
@@ -332,18 +313,12 @@ extern "C" {
 int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, const uint8_t* nullable_flags, uint32_t n_flags,
                            int to_host, etl_rowbinary_batch** out) {
   if (!batch || !out || (n_flags && !nullable_flags)) return ETL_ERR_INVALID_ARG;
-  const uint8_t* dev_stream = etl_dec_batch_device_stream(batch);
-  etl_dec_planes P;
-  etl_dec_summary S;
-  etl_dec_schema_info sc{};
-  if (etl_dec_batch_planes(batch, 0, &P) != ETL_OK || etl_dec_batch_summary(batch, &S) != ETL_OK) return ETL_ERR_INVALID_ARG;
-  const bool copy = P.rec_kind == nullptr;
+  EmitBatch E;
+  if (open_emit_batch(batch, schema_index, &E) != ETL_OK) return ETL_ERR_INVALID_ARG;
+  const etl_dec_planes& P = E.P;
+  const etl_dec_schema_info& sc = E.sc;
   const uint8_t* pk = nullptr;
-  if (copy) {
-    if (schema_index != 0 || !etl_copy_batch_columns(batch, &sc.table_id, &sc.col_kind, &sc.n_cols)) return ETL_ERR_INVALID_ARG;
-  } else if (etl_dec_batch_schema(batch, schema_index, &sc) != ETL_OK || !etl_schema_pk_columns(batch, schema_index, &pk)) {
-    return ETL_ERR_INVALID_ARG;
-  }
+  if (!E.copy && !etl_schema_pk_columns(batch, schema_index, &pk)) return ETL_ERR_INVALID_ARG;
   if (n_flags != sc.n_cols + 2) return ETL_ERR_INVALID_ARG;
   const uint32_t W = sc.n_cols + 2;
   // column descriptors: the flags, expand_key_row's rule per column, the Json item index
@@ -363,27 +338,21 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
 
   cudaStream_t st = cudaStreamPerThread;
   etl_rowbinary_batch* B = new etl_rowbinary_batch();
-  std::vector<void*> scratch;                           // stream-ordered, released on every exit
-  auto salloc = [&](uint64_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMallocAsync(&p, bytes + 64, st) != cudaSuccess) return nullptr;
-    scratch.push_back(p);
-    return p;
-  };
+  Scratch scratch(st);
   auto fail = [&](int rc) {
-    for (void* p : scratch) cudaFreeAsync(p, st);
+    scratch.release();
     cudaStreamSynchronize(st);
     cudaGetLastError();
-    etl_dec_rowbinary_free(B);
+    delete B;
     return rc;
   };
-  const uint64_t n_valid = S.first_error.record_index == UINT64_MAX ? P.n_records : std::min<uint64_t>(P.n_records, S.first_error.record_index - S.record_index_base);
+  const uint64_t n_valid = E.n_valid;
   const uint32_t nb = (uint32_t)((n_valid + kSelThreads - 1) / kSelThreads);
-  uint32_t* d_blk = (uint32_t*)salloc((nb + 1) * 4ull);
-  uint64_t* d_cell0 = (uint64_t*)salloc((n_valid + 1) * 8);
-  uint64_t* d_rec = (uint64_t*)salloc((n_valid + 1) * 8);
-  unsigned long long* d_n = (unsigned long long*)salloc(8 * (2 + kIssueSlots));   // rows, first partial | issues
-  RbCol* d_cols = (RbCol*)salloc(sizeof(RbCol) * W + 4ull * json_col.size());
+  uint32_t* d_blk = (uint32_t*)scratch((nb + 1) * 4ull);
+  uint64_t* d_cell0 = (uint64_t*)scratch((n_valid + 1) * 8);
+  uint64_t* d_rec = (uint64_t*)scratch((n_valid + 1) * 8);
+  unsigned long long* d_n = (unsigned long long*)scratch(8 * (2 + kIssueSlots));   // rows, first partial | issues
+  RbCol* d_cols = (RbCol*)scratch(sizeof(RbCol) * W + 4ull * json_col.size());
   if (!d_blk || !d_cell0 || !d_rec || !d_n || !d_cols) return fail(ETL_ERR_ALLOC);
   unsigned long long* d_issues = d_n + 2;
   uint32_t* d_json_col = reinterpret_cast<uint32_t*>(d_cols + W);
@@ -392,67 +361,41 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
       (!json_col.empty() && cudaMemcpyAsync(d_json_col, json_col.data(), 4 * json_col.size(), cudaMemcpyHostToDevice, st) != cudaSuccess))
     return fail(ETL_ERR_CUDA);
   unsigned long long sel[2] = {0, UINT64_MAX};          // rows, first partial update
-  if (copy) {
-    sel[0] = n_valid;
-    if (n_valid) k_copy_sel<<<(uint32_t)((n_valid + 255) / 256), 256, 0, st>>>(n_valid, sc.n_cols, d_cell0, d_rec);
-  } else if (nb) {
-    SelParams Sp{P.rec_kind, P.rec_flags, P.rec_schema, P.rec_cell_base, n_valid, (int32_t)schema_index, 0u, sc.n_cols, d_blk, d_cell0, d_rec, d_n};
-    k_sel_count<ClickHouseRows><<<nb, kSelThreads, 0, st>>>(Sp);
-    k_blk_scan<<<1, kSelThreads, 0, st>>>(d_blk, nb, d_n);
-    k_sel_scatter<ClickHouseRows><<<nb, kSelThreads, 0, st>>>(Sp);
-    if (cudaMemcpyAsync(sel, d_n, 16, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-  }
+  const SelParams Sp{P.rec_kind, P.rec_flags, P.rec_schema, P.rec_cell_base, n_valid, (int32_t)schema_index, 0u, sc.n_cols, d_blk, d_cell0, d_rec, d_n};
+  if (select_rows<ClickHouseRows>(Sp, E.copy, n_valid, st, sel) != ETL_OK) return fail(ETL_ERR_CUDA);
   const uint64_t n_rows = sel[0];
   B->n_rows = n_rows;
   B->issues.first_partial_update = sel[1];
-  const uint64_t meta_bytes = (2 * n_rows + 1) * 8;
-  if (cudaMalloc(&B->meta, meta_bytes) != cudaSuccess) { B->meta = nullptr; return fail(ETL_ERR_ALLOC); }
+  if (cudaMalloc(&B->meta, B->meta_bytes()) != cudaSuccess) { B->meta = nullptr; return fail(ETL_ERR_ALLOC); }
   if (cudaMemsetAsync(B->meta, 0, 8, st) != cudaSuccess ||
       (n_rows && cudaMemcpyAsync(B->meta + (n_rows + 1) * 8, d_rec, n_rows * 8, cudaMemcpyDeviceToDevice, st) != cudaSuccess))
     return fail(ETL_ERR_CUDA);
 
-  RbParams R{P.cell_tag, P.cell_val, P.cell_aux, P.heap, dev_stream, P.rec_kind, P.rec_flags, P.rec_commit_lsn,
+  RbParams R{P.cell_tag, P.cell_val, P.cell_aux, P.heap, E.stream, P.rec_kind, P.rec_flags, P.rec_commit_lsn,
              d_cell0, d_rec, n_rows, d_cols, d_json_col, sc.n_cols, W, sc.n_identity, (uint32_t)json_col.size(),
-             nullptr, nullptr, nullptr, nullptr, nullptr, (const uint64_t*)B->meta, nullptr, d_issues};
+             nullptr, nullptr, nullptr, nullptr, (const uint64_t*)B->meta, nullptr, d_issues};
   unsigned long long tot[2] = {0, 0};                   // output bytes, issue flags
   if (n_rows) {
     // Json: input lengths → item offsets → (sync) canonical text
     const uint64_t n_items = n_rows * R.n_json;
     if (n_items) {
-      const uint32_t jb = (uint32_t)((n_items + 1023) / 1024);
-      uint32_t* jl = (uint32_t*)salloc(n_items * 4);
-      uint64_t* joff = (uint64_t*)salloc((n_items + 1) * 8);
-      unsigned long long* jblk = (unsigned long long*)salloc((jb + 1) * 8ull);
-      if (!jl || !joff || !jblk) return fail(ETL_ERR_ALLOC);
-      JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, dev_stream, n_items, joff, nullptr, nullptr,
+      JsonStage J{P.cell_tag, P.cell_val, P.cell_aux, P.heap, E.stream, n_items, nullptr, nullptr, nullptr,
                   d_issues + kIssueFlags, (unsigned long long)kFlagBadJson};
-      k_json_len<RbJsonCells><<<(uint32_t)((n_items + 255) / 256), 256, 0, st>>>(J, RbJsonCells{R}, jl);
-      k_len_blocks<<<jb, 1024, 0, st>>>(jl, n_items, jblk);
-      k_blk_scan64<<<1, 1024, 0, st>>>(jblk, jb, jblk + jb);
-      k_offsets<uint64_t><<<jb, 1024, 0, st>>>(jl, n_items, jblk, joff);
-      unsigned long long jt = 0;
-      if (cudaMemcpyAsync(&jt, jblk + jb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-      R.json_off = joff;
-      R.canon = (uint8_t*)salloc(jt);
-      R.work = (uint32_t*)salloc(16 * jt);
-      if (!R.canon || !R.work) return fail(ETL_ERR_ALLOC);
-      J.canon = R.canon;
-      J.work = R.work;
-      if (jt) k_json_canon<RbJsonCells><<<(uint32_t)((n_items + 127) / 128), 128, 0, st>>>(J, RbJsonCells{R});
+      if (int rc = stage_json(scratch, J, RbJsonCells{R}, st)) return fail(rc);
+      R.json_off = J.off;
+      R.canon = J.canon;
     }
     // sizes → in-row offsets → row offsets (sync)
     const uint64_t n_cells = n_rows * W;
-    const uint32_t rb = (uint32_t)((n_rows + 1023) / 1024);
-    R.cell_len = (uint32_t*)salloc(n_cells * 4);
-    R.row_len = (uint32_t*)salloc(n_rows * 4);
-    unsigned long long* rblk = (unsigned long long*)salloc((rb + 1) * 8ull);
+    const uint32_t rb = scan_blocks(n_rows);
+    R.cell_len = (uint32_t*)scratch(n_cells * 4);
+    R.row_len = (uint32_t*)scratch(n_rows * 4);
+    unsigned long long* rblk = (unsigned long long*)scratch((rb + 1) * 8ull);
     if (!R.cell_len || !R.row_len || !rblk) return fail(ETL_ERR_ALLOC);
     k_rb_size<<<(uint32_t)((n_cells + 255) / 256), 256, 0, st>>>(R);
     k_row_scan<<<(uint32_t)((n_rows * 32 + 255) / 256), 256, 0, st>>>(R.cell_len, W, n_rows, R.row_len, d_issues + kIssueFlags,
                                                                        (unsigned long long)kFlagRowTooLong);
-    k_len_blocks<<<rb, 1024, 0, st>>>(R.row_len, n_rows, rblk);
-    k_blk_scan64<<<1, 1024, 0, st>>>(rblk, rb, rblk + rb);
-    k_offsets<uint64_t><<<rb, 1024, 0, st>>>(R.row_len, n_rows, rblk, (uint64_t*)B->meta);
+    scan_lengths(R.row_len, n_rows, rblk, rblk + rb, (uint64_t*)B->meta, st);
     if (cudaMemcpyAsync(&tot[0], rblk + rb, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
         cudaMemcpyAsync(&tot[1], d_issues + kIssueFlags, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
         cudaStreamSynchronize(st) != cudaSuccess) return fail(ETL_ERR_CUDA);
@@ -467,14 +410,11 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
     k_rb_date_elem<<<1, 1, 0, st>>>(R);
   }
   if (to_host) {
-    if (cudaHostAlloc((void**)&B->host, meta_bytes + B->bytes + 64, cudaHostAllocDefault) != cudaSuccess) { B->host = nullptr; return fail(ETL_ERR_ALLOC); }
-    if (cudaMemcpyAsync(B->host, B->meta, meta_bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(B->host + meta_bytes, B->data, B->bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
+    if (int rc = B->copy_to_host(st)) return fail(rc);
   }
   unsigned long long iss[kIssueSlots];
   if (cudaMemcpyAsync(iss, d_issues, sizeof iss, cudaMemcpyDeviceToHost, st) != cudaSuccess) return fail(ETL_ERR_CUDA);
-  for (void* p : scratch) cudaFreeAsync(p, st);
-  scratch.clear();
+  scratch.release();
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
   auto issue = [](unsigned long long key, uint32_t elem) {
     etl_rb_issue x{UINT64_MAX, UINT32_MAX, UINT32_MAX};
@@ -486,34 +426,16 @@ int etl_dec_rowbinary_emit(const etl_dec_batch* batch, uint32_t schema_index, co
   *out = B;
   return ETL_OK;
 }
-uint64_t etl_dec_rowbinary_rows(const etl_rowbinary_batch* b) { return b ? b->n_rows : 0; }
-uint64_t etl_dec_rowbinary_bytes(const etl_rowbinary_batch* b) { return b ? b->bytes : 0; }
-const uint8_t* etl_dec_rowbinary_data(const etl_rowbinary_batch* b, int host) {
-  if (!b) return nullptr;
-  if (!host) return b->data;
-  return b->host ? b->host + (2 * b->n_rows + 1) * 8 : nullptr;
-}
-const uint64_t* etl_dec_rowbinary_row_offsets(const etl_rowbinary_batch* b, int host) {
-  if (!b) return nullptr;
-  const uint8_t* base = host ? b->host : b->meta;
-  return base ? reinterpret_cast<const uint64_t*>(base) : nullptr;
-}
-const uint64_t* etl_dec_rowbinary_row_records(const etl_rowbinary_batch* b, int host) {
-  if (!b) return nullptr;
-  const uint8_t* base = host ? b->host : b->meta;
-  return base ? reinterpret_cast<const uint64_t*>(base) + b->n_rows + 1 : nullptr;
-}
+uint64_t etl_dec_rowbinary_rows(const etl_rowbinary_batch* b) { return RowPayload::rows_of(b); }
+uint64_t etl_dec_rowbinary_bytes(const etl_rowbinary_batch* b) { return RowPayload::bytes_of(b); }
+const uint8_t* etl_dec_rowbinary_data(const etl_rowbinary_batch* b, int host) { return RowPayload::data_of(b, host); }
+const uint64_t* etl_dec_rowbinary_row_offsets(const etl_rowbinary_batch* b, int host) { return RowPayload::offsets_of(b, host); }
+const uint64_t* etl_dec_rowbinary_row_records(const etl_rowbinary_batch* b, int host) { return RowPayload::records_of(b, host); }
 int etl_dec_rowbinary_issues(const etl_rowbinary_batch* b, etl_rowbinary_issues* out) {
   if (!b || !out) return ETL_ERR_INVALID_ARG;
   *out = b->issues;
   return ETL_OK;
 }
-void etl_dec_rowbinary_free(etl_rowbinary_batch* b) {
-  if (!b) return;
-  if (b->meta) cudaFree(b->meta);
-  if (b->data) cudaFree(b->data);
-  if (b->host) cudaFreeHost(b->host);
-  delete b;
-}
+void etl_dec_rowbinary_free(etl_rowbinary_batch* b) { delete b; }
 
 }  // extern "C"

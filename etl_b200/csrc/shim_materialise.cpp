@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "etl_decode.h"
+#include "batch_internal.h"
 
 namespace {
 
@@ -218,8 +219,7 @@ int etl_shim_materialise(const etl_dec_batch* batch, const uint8_t* stream, cons
   etl_event_list* L = new etl_event_list();
   L->layout = layout ? *layout : kDefaultLayout;
   const etl_rust_layout& RL = L->layout;
-  const uint64_t n_valid = S.first_error.record_index == UINT64_MAX ? P.n_records
-                           : std::min<uint64_t>(P.n_records, S.first_error.record_index - S.record_index_base);
+  const uint64_t n_valid = etl_batch_valid_records(batch);
   L->events.reserve(S.n_events);
   auto own = [&](uint64_t i, OwnedCell& c, bool in_array) {
     c.tag = in_array ? c.tag : P.cell_tag[i];
