@@ -88,6 +88,10 @@ class ParquetMetrics(C.Structure):
                 ("min", C.c_void_p), ("min_len", C.c_uint32), ("max", C.c_void_p), ("max_len", C.c_uint32)]
 
 
+class ParquetBloom(C.Structure):
+    _fields_ = [("fpp", C.c_double), ("ndv", C.c_uint64), ("max_bytes", C.c_uint32), ("_pad", C.c_uint32)]
+
+
 class Planes(C.Structure):
     _fields_ = [("n_records", C.c_uint64), ("n_cells", C.c_uint64), ("heap_bytes", C.c_uint64),
                 ("rec_off", C.c_void_p), ("rec_kind", C.c_void_p), ("rec_flags", C.c_void_p), ("rec_rel", C.c_void_p),
@@ -129,7 +133,7 @@ EXPORTS = [
     "etl_dec_bigquery_row_offsets", "etl_dec_bigquery_row_records", "etl_dec_bigquery_issues", "etl_dec_bigquery_free",
     "etl_dec_ducklake_emit", "etl_dec_ducklake_mutations", "etl_dec_ducklake_kinds", "etl_dec_ducklake_records",
     "etl_dec_ducklake_text", "etl_dec_ducklake_issues", "etl_dec_ducklake_sub_batches", "etl_dec_ducklake_copy_fingerprint",
-    "etl_dec_ducklake_free", "etl_dec_parquet_write", "etl_dec_parquet_size", "etl_dec_parquet_bytes", "etl_dec_parquet_metrics",
+    "etl_dec_ducklake_free", "etl_dec_parquet_write", "etl_dec_parquet_write_bloom", "etl_dec_parquet_size", "etl_dec_parquet_bytes", "etl_dec_parquet_metrics",
     "etl_dec_parquet_required_null", "etl_dec_parquet_free",
     "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
@@ -246,6 +250,8 @@ def load(build: bool = True):
     L.etl_dec_ducklake_free.restype = None
     L.etl_dec_parquet_write.argtypes = [vp, C.POINTER(ParquetField), C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int,
                                         C.POINTER(vp)]
+    L.etl_dec_parquet_write_bloom.argtypes = [vp, C.POINTER(ParquetField), C.POINTER(ParquetBloom), C.c_uint32, C.c_uint64,
+                                              C.c_uint64, C.c_uint32, C.c_int, C.POINTER(vp)]
     L.etl_dec_parquet_size.argtypes = [vp]
     L.etl_dec_parquet_size.restype = C.c_uint64
     L.etl_dec_parquet_bytes.argtypes = [vp, C.c_int]

@@ -17,13 +17,16 @@
 //     the serial indices_encode below share them;
 //   * the page index pieces (ETL_PQ_PAGE_INDEX): the 64-byte truncation of byte-array ColumnIndex bounds, the
 //     PageLocation of the OffsetIndex and the header of a list field;
+//   * the bloom filter pieces (etl_dec_parquet_write_bloom): XXH64 (seed 0) of a value's PLAIN bytes, the block and bit
+//     masks of a split-block insert, the BloomFilterHeader, and (host only) the bitset size from ndv and fpp;
 //   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders, for
-//     a dictionary chunk its dictionary_page_offset and encoding_stats, and with a page index the ColumnChunk's offset
-//     and length of its OffsetIndex and ColumnIndex.
+//     a dictionary chunk its dictionary_page_offset and encoding_stats, with a page index the ColumnChunk's offset
+//     and length of its OffsetIndex and ColumnIndex, and with a bloom filter its offset and length.
 #pragma once
 #include <stdint.h>
 #include <string.h>
 
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -289,8 +292,76 @@ __host__ __device__ inline uint32_t list_field(uint8_t* out, uint8_t elem_type, 
   return (uint32_t)w.n;
 }
 
-// ------------------------------------------------------------------------------------------------ Snappy
+// ------------------------------------------------------------------------------------------------ bloom filters
+// Parquet's split-block bloom filter (BloomFilter.md): XXH64 of the value's PLAIN bytes without a length prefix; the
+// block ((h >> 32) * blocks) >> 32 of 32 bytes; in it, word i gets bit (uint32)((uint32)h * kBloomSalt[i]) >> 27.
+constexpr uint64_t kBloomMinBytes = 32, kBloomMaxBytes = 128ull << 20;
+constexpr uint64_t kBloomDefaultBytes = 1ull << 20;   // max_bytes 0 (Iceberg's write.parquet.bloom-filter-max-bytes)
+constexpr uint64_t kXxP1 = 0x9E3779B185EBCA87ull, kXxP2 = 0xC2B2AE3D27D4EB4Full, kXxP3 = 0x165667B19E3779F9ull,
+                   kXxP4 = 0x85EBCA77C2B2AE63ull, kXxP5 = 0x27D4EB2F165667C5ull;
+__host__ __device__ inline uint64_t rotl64(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
 __host__ __device__ inline uint32_t load32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
+__host__ __device__ inline uint64_t load64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
+__host__ __device__ inline uint64_t xxh64_round(uint64_t acc, uint64_t lane) { return rotl64(acc + lane * kXxP2, 31) * kXxP1; }
+__host__ __device__ inline uint64_t xxh64_merge(uint64_t h, uint64_t v) { return (h ^ xxh64_round(0, v)) * kXxP1 + kXxP4; }
+__host__ __device__ inline uint64_t xxh64_avalanche(uint64_t h) {
+  h ^= h >> 33; h *= kXxP2; h ^= h >> 29; h *= kXxP3; h ^= h >> 32;
+  return h;
+}
+// XXH64, seed 0, of p[0, len)
+__host__ __device__ inline uint64_t xxh64(const uint8_t* p, uint64_t len) {
+  uint64_t h, k = 0;
+  if (len >= 32) {
+    uint64_t v1 = kXxP1 + kXxP2, v2 = kXxP2, v3 = 0, v4 = 0 - kXxP1;
+    for (; k + 32 <= len; k += 32) {
+      v1 = xxh64_round(v1, load64(p + k)); v2 = xxh64_round(v2, load64(p + k + 8));
+      v3 = xxh64_round(v3, load64(p + k + 16)); v4 = xxh64_round(v4, load64(p + k + 24));
+    }
+    h = rotl64(v1, 1) + rotl64(v2, 7) + rotl64(v3, 12) + rotl64(v4, 18);
+    h = xxh64_merge(h, v1); h = xxh64_merge(h, v2); h = xxh64_merge(h, v3); h = xxh64_merge(h, v4);
+  } else h = kXxP5;
+  h += len;
+  for (; k + 8 <= len; k += 8) h = rotl64(h ^ xxh64_round(0, load64(p + k)), 27) * kXxP1 + kXxP4;
+  if (k + 4 <= len) { h = rotl64(h ^ (uint64_t)load32(p + k) * kXxP1, 23) * kXxP2 + kXxP3; k += 4; }
+  for (; k < len; k++) h = rotl64(h ^ (uint64_t)p[k] * kXxP5, 11) * kXxP1;
+  return xxh64_avalanche(h);
+}
+// the same hash of a 4- / 8-byte little-endian value
+__host__ __device__ inline uint64_t xxh64_u32(uint32_t v) {
+  return xxh64_avalanche(rotl64((kXxP5 + 4) ^ (uint64_t)v * kXxP1, 23) * kXxP2 + kXxP3);
+}
+__host__ __device__ inline uint64_t xxh64_u64(uint64_t v) {
+  return xxh64_avalanche(rotl64((kXxP5 + 8) ^ xxh64_round(0, v), 27) * kXxP1 + kXxP4);
+}
+// the block of hash h in a bitset of blocks 32-byte blocks, and the bit of its word i
+__host__ __device__ inline uint32_t bloom_block(uint64_t h, uint32_t blocks) { return (uint32_t)(((h >> 32) * blocks) >> 32); }
+__host__ __device__ inline uint32_t bloom_mask(uint64_t h, int i) {
+  const uint32_t salt[8] = {0x47b6137bu, 0x44974d91u, 0x8824ad5bu, 0xa2b7289du, 0x705495c7u, 0x2df1424bu, 0x9efc4947u, 0x5c6bfb31u};
+  return 1u << (((uint32_t)h * salt[i]) >> 27);
+}
+// BloomFilterHeader {1 numBytes, 2 algorithm {1 BLOCK {}}, 3 hash {1 XXHASH {}}, 4 compression {1 UNCOMPRESSED {}}};
+// out == nullptr counts.  Returns its length (at most 19 bytes).
+__host__ __device__ inline uint32_t bloom_header(uint8_t* out, uint32_t num_bytes) {
+  TWriter w(out);
+  w.i32(1, (int32_t)num_bytes);
+  for (int16_t f = 2; f <= 4; f++) { w.begin(f); w.begin(1); w.end(); w.end(); }
+  w.end();
+  return (uint32_t)w.n;
+}
+// (host) bitset bytes for ndv distinct values at false-positive probability fpp, as Arrow C++'s OptimalNumOfBits:
+// bits = -8 ndv / ln(1 - fpp^(1/8)) truncated, clamped to [8 × 32, 8 × 128 MiB], rounded up to a power of two; then
+// at most max_bytes (a power of two in [32, 128 MiB])
+inline uint64_t bloom_bytes(uint64_t ndv, double fpp, uint64_t max_bytes) {
+  const double m = -8.0 * (double)ndv / std::log(1.0 - std::pow(fpp, 1.0 / 8));
+  uint64_t bits = !(m >= 0) || m > 8.0 * kBloomMaxBytes ? 8 * kBloomMaxBytes : (uint64_t)m;
+  if (bits < 8 * kBloomMinBytes) bits = 8 * kBloomMinBytes;
+  uint64_t p = 1;
+  while (p < bits) p <<= 1;
+  const uint64_t bytes = p / 8;
+  return bytes < max_bytes ? bytes : max_bytes;
+}
+
+// ------------------------------------------------------------------------------------------------ Snappy
 __host__ __device__ inline uint32_t snappy_hash(uint32_t v) { return (v * 0x1e35a7bdu) >> (32 - kSnappyHashBits); }
 __host__ __device__ inline uint32_t snappy_literal(const uint8_t* src, uint32_t len, uint8_t* out) {
   uint32_t o = 0;
@@ -374,6 +445,8 @@ struct Chunk {
   bool page_index = false;          // ETL_PQ_PAGE_INDEX: the chunk's OffsetIndex and, when ci_len, its ColumnIndex
   uint64_t ci_offset = 0, oi_offset = 0;
   uint32_t ci_len = 0, oi_len = 0;
+  uint64_t bloom_offset = 0;        // a bloom filter: its header's file offset, header + bitset bytes (0: none)
+  uint32_t bloom_len = 0;
 };
 
 inline void schema_element(TWriter& w, const Leaf& L, bool element) {
@@ -473,6 +546,7 @@ inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::v
           w.list_struct_begin(); w.i32(1, PAGE_DICTIONARY); w.i32(2, ENC_PLAIN); w.i32(3, 1); w.end();
           w.list_struct_begin(); w.i32(1, PAGE_DATA); w.i32(2, ENC_RLE_DICTIONARY); w.i32(3, (int32_t)C.data_pages); w.end();
         }
+        if (C.bloom_len) { w.i64(14, (int64_t)C.bloom_offset); w.i32(15, (int32_t)C.bloom_len); }
         w.end();
         if (C.page_index) {                            // ColumnChunk offset_index_offset / _length, column_index_*
           w.i64(4, (int64_t)C.oi_offset);

@@ -37,6 +37,12 @@
 //      one k_blk_scan over the 2 × chunks lengths places them behind 4 + data_end (read on the device);
 //      k_index<true> writes them and their offsets into the chunk records.  k_row_max (before SYNC 1) bounds an
 //      untruncated byte-array maximum by the leaf's longest row.
+//   4c. Bloom filters (etl_dec_parquet_write_bloom).  k_chunk_nn (before SYNC 1) gives each chunk's non-null values, from
+//      which the host sizes every bitset and places the filters (row-group major) in a region behind 4 + data_end, in
+//      front of the page index.  One memset zeroes the bitsets' scratch; k_bloom, per filtered leaf and grid-stride
+//      over its items, hashes each non-null value (XXH64 of its PLAIN bytes, a byte array serially by its thread) and
+//      sets its 8 bits by atomicOr; k_bloom_write copies each header and bitset into the file.  A dictionary chunk's
+//      filter is built from its values like any other, so it equals its PLAIN form's.
 //      SYNC 2 copies the chunk and leaf records back.
 //   5. Footer, on the host from those records (parquet_format.cuh), copied behind the pages with its length and "PAR1".
 //      SYNC 3 ends the call (and the copy to pinned host memory with to_host).
@@ -47,7 +53,9 @@
 // heads (+ 12 B per page), the chunks' tables (4 B × pow2 >= 2 × non-null values: at most 16 B per value), a dictionary
 // slot per chunk (at most 1 MiB, at most the chunk's PLAIN bytes) and 32 B more per data page slot.  ETL_PQ_PAGE_INDEX
 // adds 4 B per leaf, 40 B of IndexChunk + 16 B of lengths per chunk, and in the file's buffer 189 B per page + 64 B per
-// chunk (+ for a byte-array leaf with a row over 64 bytes, its longest row per page, at most its value bytes).
+// chunk (+ for a byte-array leaf with a row over 64 bytes, its longest row per page, at most its value bytes).  Bloom
+// filters add 8 B of non-null count + 24 B of BloomChunk per chunk, each filtered chunk's bitset in scratch, and in the
+// file's buffer its header (at most 19 B) and bitset.
 // ptxas -v (sm_90a, CUDA 12.9): see the comment at the end of this file.
 #include <cuda_runtime.h>
 
@@ -854,12 +862,13 @@ constexpr uint32_t kIdxWarps = 4;
 // listed).  kWrite false: each page's entry sizes, the boundary order (each non-null page against the previous one, on
 // the untruncated bounds) and the lengths of the chunk's ColumnIndex (lens[c], 0 when it has none) and OffsetIndex
 // (lens[n_chunks + c]); lens[2 n_chunks] = 0, so that their exclusive scan places them behind the pages.  kWrite true:
-// both structures at 4 + data_end + lens[...], and their offsets and lengths into the chunk's record.
+// both structures at 4 + data_end + skip (the bloom filters' bytes) + lens[...], and their offsets and lengths into
+// the chunk's record.
 template <bool kWrite>
 __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves, const Page* pages, const uint64_t* page_base,
                                                          uint32_t n_chunks, uint32_t n_leaves, const uint64_t* foff, IndexChunk* X,
                                                          unsigned long long* lens, const unsigned long long* data_end,
-                                                         uint8_t* file, ChunkOut* out) {
+                                                         uint64_t skip, uint8_t* file, ChunkOut* out) {
   const uint32_t c = blockIdx.x * kIdxWarps + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (c >= n_chunks) {
@@ -877,7 +886,7 @@ __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves,
   uint64_t o_min = 0, o_max = 0, o_nc = 0;                // kWrite: where the sections' entries start
   if (kWrite) {
     I = X[c];
-    const uint64_t base = 4 + *data_end;                  // lens: the exclusive scan of the lengths
+    const uint64_t base = 4 + *data_end + skip;           // behind the bloom filters; lens: the exclusive scan
     ci = file + base + lens[c];
     oi = file + base + lens[n_chunks + c];
     o_min = lk + k + lk; o_max = o_min + I.s_min + lk; o_nc = o_max + I.s_max + 2 + lk;
@@ -956,6 +965,64 @@ __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves,
   }
 }
 
+// bloom filters (etl_dec_parquet_write_bloom): one record per chunk (row-group major); bytes 0: no filter
+struct BloomChunk {
+  uint64_t word;             // first u32 word of the chunk's bitset in the bloom scratch (32-byte aligned)
+  uint64_t off;              // the filter's offset (its header) in the bloom region behind 4 + data_end
+  uint32_t bytes, hlen;      // bitset bytes, header bytes
+};
+// a thread per chunk: the non-null values of the chunk (NN prefix sums at its row-group bounds), which size its bitset
+__global__ void k_chunk_nn(uint32_t n_leaves, uint32_t n_chunks, uint64_t n, const uint64_t* NN, unsigned long long* cnn) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  const uint64_t* nv = NN + (uint64_t)(c % n_leaves) * (n + 1);
+  const uint64_t g0 = (uint64_t)(c / n_leaves) * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
+  cnn[c] = nv[g1] - nv[g0];
+}
+// XXH64 of present item it's PLAIN bytes (byte arrays without the length prefix, hashed serially by this thread)
+__device__ __forceinline__ uint64_t item_hash(const LeafDev& L, uint64_t it) {
+  if (is_bytes(L)) { const uint64_t a = byte_off(L, it); return xxh64(L.data + a, byte_off(L, it + 1) - a); }
+  switch (L.fixed) {
+    case 4: return xxh64_u32(((const uint32_t*)L.values)[it]);
+    case 8: return xxh64_u64(((const uint64_t*)L.values)[it]);
+    default: return xxh64(L.values + 16 * it, 16);
+  }
+}
+// the first item of row group g of a leaf (g == n_rg: the end of its items)
+__device__ __forceinline__ uint64_t group_item(const LeafDev& L, uint64_t rb, uint64_t n, uint32_t g) {
+  const uint64_t r = rb + min(n, (uint64_t)g * kRowGroupRows);
+  return L.is_list ? (uint64_t)L.loffs[r] : r;
+}
+// 4c. bloom filters, one filtered leaf, grid-stride over its items: each non-null item's hash sets 8 bits of one block
+// of its chunk's bitset (atomicOr into the zeroed scratch; the bits are a set, so any order gives the same bitset)
+__global__ void __launch_bounds__(kInsThreads) k_bloom(const LeafDev* leaves, uint32_t l, uint32_t n_leaves, uint32_t n_rg,
+                                                       uint64_t rb, uint64_t n, const BloomChunk* B, uint32_t* words) {
+  const LeafDev L = leaves[l];
+  const uint64_t i0 = group_item(L, rb, n, 0), i1 = group_item(L, rb, n, n_rg);
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t it = i0 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; it < i1; it += stride) {
+    if (!bit(L.valid, it)) continue;
+    uint32_t g = 0;
+    while (g + 1 < n_rg && it >= group_item(L, rb, n, g + 1)) g++;
+    const BloomChunk K = B[g * n_leaves + l];
+    const uint64_t h = item_hash(L, it);
+    uint32_t* w = words + K.word + 8ull * bloom_block(h, K.bytes / 32);
+#pragma unroll
+    for (int i = 0; i < 8; i++) atomicOr(w + i, bloom_mask(h, i));
+  }
+}
+// 4d. CTAs (chunk, slice): the chunk's header and bitset at 4 + data_end + its offset (ETL_PQ_PAGE_INDEX comes after)
+__global__ void __launch_bounds__(256) k_bloom_write(const BloomChunk* B, const uint32_t* words, const unsigned long long* data_end,
+                                                     uint8_t* file) {
+  const BloomChunk K = B[blockIdx.x];
+  if (!K.bytes) return;
+  uint8_t* dst = file + 4 + *data_end + K.off;
+  if (blockIdx.y == 0 && threadIdx.x == 0) bloom_header(dst, K.bytes);
+  const uint8_t* src = (const uint8_t*)(words + K.word);
+  dst += K.hlen;
+  for (uint64_t k = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; k < K.bytes; k += (uint64_t)gridDim.y * blockDim.x) dst[k] = src[k];
+}
+
 uint32_t parquet_type(uint32_t at) {
   switch (at) {
     case ETL_ARROW_BOOLEAN: return PT_BOOLEAN;
@@ -992,6 +1059,12 @@ extern "C" {
 
 int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fields, uint32_t n_fields, uint64_t row_begin,
                           uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out) {
+  return etl_dec_parquet_write_bloom(a, fields, nullptr, n_fields, row_begin, row_end, codec, to_host, out);
+}
+
+int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom,
+                                uint32_t n_fields, uint64_t row_begin, uint64_t row_end, uint32_t codec, int to_host,
+                                etl_parquet_file** out) {
   // a file needs at least one column (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS has none)
   if (!a || !out || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
   const uint32_t cc = codec & 0xFFu;                  // the compression codec; the flag bits are ETL_PQ_DICTIONARY and
@@ -1027,6 +1100,13 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     L.fixed = plain_width(L.atype);
     L.off64 = L.atype == ETL_ARROW_LARGE_BINARY;
     L.valid = col.validity; L.values = (const uint8_t*)col.values; L.offs = col.offsets; L.data = col.data;
+    if (bloom) {
+      const etl_parquet_bloom& Bf = bloom[c];
+      const uint32_t mb = Bf.max_bytes;
+      if (!(Bf.fpp >= 0.0 && Bf.fpp < 1.0) || (mb && (mb < kBloomMinBytes || mb > kBloomMaxBytes || (mb & (mb - 1)))) ||
+          (Bf.fpp > 0.0 && L.atype == ETL_ARROW_BOOLEAN))
+        return ETL_ERR_INVALID_ARG;
+    }
     Leaf& M = meta[c];
     M.name.assign(F.name, nl);
     M.field_id = F.field_id; M.element_field_id = F.element_field_id;
@@ -1048,6 +1128,9 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   const uint32_t n_rg = (uint32_t)((n + kRowGroupRows - 1) / kRowGroupRows);
   const uint32_t n_chunks = n_rg * nL;
   const int snappy = cc == ETL_PQ_SNAPPY;
+  auto bloomed = [&](uint32_t l) { return bloom && bloom[l].fpp > 0.0; };
+  bool any_bloom = false;
+  for (uint32_t l = 0; l < nL; l++) any_bloom |= bloomed(l);
   cudaStream_t st = cudaStreamPerThread;
   etl_parquet_file* Fo = new etl_parquet_file();
   std::vector<void*> pool;
@@ -1064,7 +1147,8 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   unsigned long long* d_tot = (unsigned long long*)dalloc(3ull * nL * 8);
   unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull + 4ull * nL);   // | ETL_PQ_PAGE_INDEX: k_row_max
   uint32_t* d_np = (uint32_t*)dalloc(n_chunks * 4ull);
-  if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np) return fail(ETL_ERR_ALLOC);
+  unsigned long long* d_cnn = any_bloom ? (unsigned long long*)dalloc(n_chunks * 8ull) : nullptr;   // bloom: per chunk
+  if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np || (any_bloom && !d_cnn)) return fail(ETL_ERR_ALLOC);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_req, 0xff, nL * 8ull, st));
   unsigned int* d_vmax = (unsigned int*)(d_req + nL);
@@ -1083,9 +1167,12 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
       }
     k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
     if (pidx) k_row_max<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, n, vb, d_vmax);
+    if (any_bloom) k_chunk_nn<<<(n_chunks + 255) / 256, 256, 0, st>>>(nL, n_chunks, n, NN, d_cnn);
   }
-  // SYNC 1: page counts, totals, required-column nulls
+  // SYNC 1: page counts, totals, required-column nulls (bloom filters: the chunks' non-null values)
   std::vector<uint32_t> np(n_chunks);
+  std::vector<unsigned long long> cnn(n_chunks);
+  if (any_bloom && n_chunks) CK(cudaMemcpyAsync(cnn.data(), d_cnn, n_chunks * 8ull, cudaMemcpyDeviceToHost, st));
   std::vector<unsigned long long> tot(3ull * nL), req(nL);
   std::vector<unsigned int> vmax(nL);
   if (n_chunks) CK(cudaMemcpyAsync(np.data(), d_np, n_chunks * 4ull, cudaMemcpyDeviceToHost, st));
@@ -1154,6 +1241,22 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     if (has_dict(c % nL)) { k.dict = true; k.data_offset = 1ull << 62; k.data_pages = INT32_MAX; }
     if (pidx) { k.page_index = true; k.ci_offset = k.oi_offset = 1ull << 62; k.ci_len = k.oi_len = INT32_MAX; }
   }
+  // bloom filters: each filtered chunk's bitset size from its ndv (or non-null count), its header, its place in the
+  // region behind the pages (row-group major, column minor) and its bitset's place in the zeroed scratch
+  std::vector<BloomChunk> hb(n_chunks, BloomChunk{0, 0, 0, 0});
+  uint64_t bloom_total = 0, bloom_words = 0;
+  for (uint32_t c = 0; c < n_chunks; c++) {
+    const uint32_t l = c % nL;
+    if (!bloomed(l)) continue;
+    const etl_parquet_bloom& Bf = bloom[l];
+    const uint64_t ndv = Bf.ndv ? Bf.ndv : std::max<uint64_t>(1, cnn[c]);
+    BloomChunk& K = hb[c];
+    K.bytes = (uint32_t)bloom_bytes(ndv, Bf.fpp, Bf.max_bytes ? Bf.max_bytes : kBloomDefaultBytes);
+    K.hlen = bloom_header(nullptr, K.bytes);
+    K.off = bloom_total; K.word = bloom_words;
+    bloom_total += K.hlen + K.bytes; bloom_words += K.bytes / 4;
+    wide[c].bloom_offset = 1ull << 62; wide[c].bloom_len = INT32_MAX;
+  }
   const char* created_by = "etl-b200 parquet writer";
   const uint64_t footer_bound = footer(meta, rg_rows, wide, cc, created_by).size() + 8;
   const uint64_t data_bound = 4 + P * kPageHeaderMax + (snappy ? C_bound : U);
@@ -1206,7 +1309,14 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     d_ixlen = (unsigned long long*)dalloc(8 * (2ull * n_chunks + 1));
     if (!d_ix || !d_ixlen) return fail(ETL_ERR_ALLOC);
   }
-  if (cudaMalloc(&Fo->dev, data_bound + index_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
+  BloomChunk* d_bch = nullptr;
+  uint32_t* d_bwords = nullptr;
+  if (bloom_total) {
+    d_bch = (BloomChunk*)dalloc(sizeof(BloomChunk) * n_chunks);
+    d_bwords = (uint32_t*)dalloc(4 * bloom_words);
+    if (!d_bch || !d_bwords) return fail(ETL_ERR_ALLOC);
+  }
+  if (cudaMalloc(&Fo->dev, data_bound + bloom_total + index_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
   uint64_t* uslot = d_scan; uint64_t* cslot = d_scan + (P + 1); uint64_t* fbase = d_scan + 2 * (P + 1); uint64_t* foff = d_scan + 3 * (P + 1);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_pbase, page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
@@ -1215,6 +1325,10 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
   CK(cudaMemcpyAsync(Fo->dev, "PAR1", 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_bool, 0, bool_words * 4 + 8, st));
   CK(cudaMemsetAsync(d_lscr, 0, lscr_base[nL] + 16, st));
+  if (bloom_total) {
+    CK(cudaMemcpyAsync(d_bch, hb.data(), sizeof(BloomChunk) * n_chunks, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_bwords, 0, 4 * bloom_words, st));
+  }
   if (P) {
     k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages, dict);
     // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
@@ -1258,12 +1372,20 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
     k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, snappy, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
     k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout, d_dch);
+    if (bloom_total) {
+      // bloom filters: the bitsets in scratch, then headers and bitsets behind the pages
+      for (uint32_t l = 0; l < nL; l++)
+        if (bloomed(l))
+          k_bloom<<<std::min<uint32_t>(kInsBlocks, (uint32_t)((tot[l] + kInsThreads - 1) / kInsThreads) + 1), kInsThreads, 0, st>>>(
+              d_leaves, l, nL, n_rg, row_begin, n, d_bch, d_bwords);
+      k_bloom_write<<<dim3(n_chunks, 16), 256, 0, st>>>(d_bch, d_bwords, d_stot + 3, Fo->dev);
+    }
     if (d_ix) {
       // page index: sizes and boundary orders, their places behind the pages, the bytes
       const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
-      k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, Fo->dev, d_cout);
+      k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, bloom_total, Fo->dev, d_cout);
       k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
-      k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, Fo->dev, d_cout);
+      k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, bloom_total, Fo->dev, d_cout);
     }
   }
   if (nL) k_leaf<<<(nL + 63) / 64, 64, 0, st>>>(d_leaves, nL, P ? n_rg : 0, d_cout, d_lout);
@@ -1285,13 +1407,14 @@ int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fie
     chunks[c] = Chunk{K.offset, K.num_values, K.usize, K.csize, K.null_count, K.has != 0,
                       std::string((const char*)K.min, K.min_len), std::string((const char*)K.max, K.max_len),
                       K.dict != 0, K.data_offset, K.data_pages, pidx != 0, K.ci_offset, K.oi_offset, K.ci_len, K.oi_len};
+    if (hb[c].bytes) { chunks[c].bloom_offset = 4 + data_end + hb[c].off; chunks[c].bloom_len = hb[c].hlen + hb[c].bytes; }
   }
   std::vector<uint8_t> foot = footer(meta, rg_rows, chunks, cc, created_by);
   const uint32_t flen = (uint32_t)foot.size();
   for (int b = 0; b < 4; b++) foot.push_back((uint8_t)(flen >> (8 * b)));
   for (char ch : std::string("PAR1")) foot.push_back((uint8_t)ch);
-  Fo->size = 4 + data_end + index_end + foot.size();
-  CK(cudaMemcpyAsync(Fo->dev + 4 + data_end + index_end, foot.data(), foot.size(), cudaMemcpyHostToDevice, st));
+  Fo->size = 4 + data_end + bloom_total + index_end + foot.size();
+  CK(cudaMemcpyAsync(Fo->dev + 4 + data_end + bloom_total + index_end, foot.data(), foot.size(), cudaMemcpyHostToDevice, st));
   if (to_host) {
     if (cudaHostAlloc((void**)&Fo->host, Fo->size, cudaHostAllocDefault) != cudaSuccess) { Fo->host = nullptr; return fail(ETL_ERR_ALLOC); }
     CK(cudaMemcpyAsync(Fo->host, Fo->dev, Fo->size, cudaMemcpyDeviceToHost, st));
@@ -1348,6 +1471,8 @@ void etl_dec_parquet_free(etl_parquet_file* f) {
 //   k_dict_setup 24 / 0 / 0   k_dict_place 10 / 0 / 0   k_dict_insert 46 / 0 / 0   k_dict_mark 24 / 0 / 0
 //   k_dict_finish 22 / 0 / 0  k_dict_page 32 / 0 / 0
 //   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)
-//   k_row_max 12 / 0 / 0   k_index<false> 72 / 0 / 40 B and k_index<true> 64 / 0 / 80 B (a fixed-width bound's bytes)
+//   k_row_max 12 / 0 / 0   k_index<false> 72 / 0 / 40 B and k_index<true> 64 / 0 / 80 B (a fixed-width bound's bytes;
+//   28 B of it spills, as before the bloom filters)
+//   k_chunk_nn 16 / 0 / 0   k_bloom 54 / 0 / 0   k_bloom_write 29 / 0 / 40 B (the header's Thrift writer)
 //   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan<unsigned long long> 32 / 8192 B,
 //   k_offsets<uint64_t> 18 / 8192 B

@@ -775,7 +775,9 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * another n_fields or none (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS), an ETL_ARROW_UNSUPPORTED
  * column (the emit lacked ETL_ARROW_ALL_COLUMNS), row_begin > row_end or row_end > etl_dec_arrow_rows, an unknown
  * codec (codec & 0xFF other than ETL_PQ_UNCOMPRESSED / ETL_PQ_SNAPPY) or a codec bit other than ETL_PQ_DICTIONARY and
- * ETL_PQ_PAGE_INDEX, a NULL or empty name or one longer than 1 KiB.
+ * ETL_PQ_PAGE_INDEX, a NULL or empty name or one longer than 1 KiB; with bloom, an fpp that is NaN, negative or >= 1,
+ * a max_bytes that is neither 0 nor a power of two in [32, 2^27], or fpp > 0 on a Boolean leaf (Arrow C++ has no
+ * filters for BOOLEAN either).
  * A null in a required column (a null list of a required List column, or a null value) is data: ETL_OK with size 0 and
  * no bytes, and etl_dec_parquet_required_null gives the smallest such column and its first null row (emit row numbers)
  * — RecordBatch::try_new in rows_to_record_batch fails there before anything is written (a ConversionError in the shim).
@@ -856,14 +858,35 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  *          unless one is above, else UNORDERED (0) (one page, a constant chunk or an all-null chunk: ASCENDING).
  *          null_counts: level entries minus non-null values of each page.  A chunk with a page whose non-null values
  *          are all NaN (no bounds) has no ColumnIndex, only its OffsetIndex.  Not written: level histograms and
- *          SizeStatistics, page-header statistics, bloom filters.  The metrics' compressed_bytes stay the chunks' page
- *          bytes (Iceberg's column_sizes); etl_dec_parquet_size counts the whole file.
+ *          SizeStatistics, page-header statistics.  The metrics' compressed_bytes stay the chunks' page bytes (Iceberg's
+ *          column_sizes); etl_dec_parquet_size counts the whole file.
+ *   bloom filters (etl_dec_parquet_write_bloom, a column with fpp > 0; without one no chunk has a filter, and bytes
+ *          [0, 4 + data end) of a file with filters are the file written without them, the same codec and flags): the
+ *          split-block filters Arrow C++ writes (pyarrow's bloom_filter_options), for readers that skip row groups on
+ *          equality predicates; readers that ignore filters read the file as before.
+ *          Which chunks: every chunk (one leaf in one row group) of such a column, an all-null chunk too (its bitset all
+ *          zero); a List column's leaf is its element, its filter holds the non-null elements.  Zero rows: no filter.
+ *          Size: ndv = the field's ndv, or the chunk's non-null values when 0 (at least 1); bits = -8 ndv / ln(1 -
+ *          fpp^(1/8)) in double, truncated, clamped to [256, 2^30], rounded up to a power of two; bytes = bits / 8, then
+ *          min(bytes, max_bytes).
+ *          Hash: XXH64, seed 0, of the value's PLAIN bytes without a length prefix: INT32 / INT64 / FLOAT / DOUBLE the
+ *          little-endian value (floats by their bits: +0.0 and -0.0 differ, a NaN hashes as its bits), BYTE_ARRAY the
+ *          bytes, UUID the 16 bytes.  Insert: blocks = bytes / 32, block ((h >> 32) × blocks) >> 32, key (uint32)h; word
+ *          8 × block + i (i < 8) gets bit (uint32)(key × SALT[i]) >> 27, SALT = {0x47b6137b, 0x44974d91, 0x8824ad5b,
+ *          0xa2b7289d, 0x705495c7, 0x2df1424b, 0x9efc4947, 0x5c6bfb31}; the bitset is those u32 words little-endian.
+ *          Each filter: Thrift compact BloomFilterHeader {1 numBytes: i32, 2 algorithm {1 BLOCK {}}, 3 hash {1 XXHASH
+ *          {}}, 4 compression {1 UNCOMPRESSED {}}} (15 bytes for 32 B of bitset, 16 for 128, 17 for 8192), then the bitset.
+ *          Layout: after the last column chunk every filter, row-group major and column minor; then the page index
+ *          (the same structs, behind the filters); then the footer.  ColumnMetaData adds bloom_filter_offset (14, i64,
+ *          the header's file offset) and bloom_filter_length (15, i32, header + bitset) after encoding_stats.  The
+ *          metrics are those of the file without filters (compressed_bytes: the chunk's pages); etl_dec_parquet_size
+ *          counts the filters.
  *   footer: Thrift compact, ascending field ids: FileMetaData {version 1, schema, num_rows, row_groups, created_by,
  *          column_orders}, SchemaElement {type, type_length, repetition_type, name, num_children, converted_type,
  *          field_id, logicalType}, RowGroup {columns, total_byte_size, num_rows, file_offset, total_compressed_size,
  *          ordinal}, ColumnChunk {file_offset, meta_data[, page index fields]}, ColumnMetaData {type, encodings (PLAIN, + RLE with levels),
  *          path_in_schema, codec, num_values, total_uncompressed_size, total_compressed_size, data_page_offset,
- *          [dictionary_page_offset,] statistics[, encoding_stats]}.
+ *          [dictionary_page_offset,] statistics[, encoding_stats][, bloom_filter_offset, bloom_filter_length]}.
  * Metrics: one record per leaf (a List column's leaf is its element), over every row group of the file; min / max are
  * the PLAIN statistic bytes, which equal Iceberg's single-value serialization of these types (before truncation).
  * to_host: also copy the file to pinned host memory (etl_dec_parquet_bytes(f, 1); else NULL).  Scratch, beside the
@@ -872,7 +895,8 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * eligible leaf (bounded by its level entries) + 0.5 B per item of run heads, a dictionary slot per chunk of at most
  * 1 MiB, 32 B per data page, and hash tables of at most 16 B per non-null value; with ETL_PQ_PAGE_INDEX 40 B per chunk
  * and, in the file's buffer, 189 B per page + 64 B per chunk (+ the longest row per page of a byte-array leaf with a
- * value over 64 bytes, at most its value bytes). */
+ * value over 64 bytes, at most its value bytes); with bloom filters 8 B per chunk, 24 B per chunk record and each
+ * filtered chunk's bitset in scratch, and in the file's buffer its bitset + header (at most 19 B). */
 enum { ETL_PQ_UNCOMPRESSED = 0, ETL_PQ_SNAPPY = 1 };
 #define ETL_PQ_DICTIONARY 0x100u   /* OR-ed into codec: dictionary-encode the eligible column chunks (codec & 0xFF: compression) */
 #define ETL_PQ_PAGE_INDEX 0x400u   /* OR-ed into codec: write a ColumnIndex and an OffsetIndex per column chunk */
@@ -896,8 +920,19 @@ typedef struct etl_parquet_metrics {   /* one per leaf (= per column; a List col
   const uint8_t* max; uint32_t max_len;
 } etl_parquet_metrics;
 typedef struct etl_parquet_file etl_parquet_file;
+typedef struct etl_parquet_bloom {   /* one per emitted column, parallel to fields */
+  double fpp;                 /* false-positive probability, 0 < fpp < 1; exactly 0: no filter for this column */
+  uint64_t ndv;               /* expected distinct values per column chunk; 0: the chunk's non-null values (at least 1) */
+  uint32_t max_bytes;         /* cap on one bitset: a power of two in [32, 128 MiB]; 0: 1 MiB */
+  uint32_t _pad;
+} etl_parquet_bloom;
 int etl_dec_parquet_write(const etl_arrow_batch*, const etl_parquet_field* fields, uint32_t n_fields,
                           uint64_t row_begin, uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out);
+/* the same file with a split-block bloom filter on every column chunk of a column whose bloom[c].fpp > 0 (bloom NULL,
+ * or every fpp 0: the file etl_dec_parquet_write writes) */
+int etl_dec_parquet_write_bloom(const etl_arrow_batch*, const etl_parquet_field* fields, const etl_parquet_bloom* bloom,
+                                uint32_t n_fields, uint64_t row_begin, uint64_t row_end, uint32_t codec, int to_host,
+                                etl_parquet_file** out);
 uint64_t etl_dec_parquet_size(const etl_parquet_file*);
 const uint8_t* etl_dec_parquet_bytes(const etl_parquet_file*, int host);   /* the whole file, "PAR1" … "PAR1" */
 int etl_dec_parquet_metrics(const etl_parquet_file*, uint32_t leaf, etl_parquet_metrics* out);

@@ -4,6 +4,7 @@
   python tools/parquet_measure.py [--copy-rows 1000000] [--c3-scale 1] [--c4-scale 0.1] [--reps 7] [--warmup 2]
                                   [--plain-only] [--no-pyarrow] [--tag NAME]
   python tools/parquet_measure.py --page-index [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
+  python tools/parquet_measure.py --bloom [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
 
 Workloads: bench.py's 10-column COPY table, C3 (one schema version) and C4 (every schema version: times and sizes are
 sums over the versions), each emitted once with 7 | ETL_ARROW_ALL_COLUMNS | ETL_ARROW_CDC_COLUMNS and kept in HBM.
@@ -20,6 +21,8 @@ ETL_PQ_DICTIONARY can be timed by the same script (ETL_LIB_SUFFIX selects it); -
 --page-index instead writes each emit of the COPY table, C5 and C4 with and without ETL_PQ_PAGE_INDEX, alternating the
 two in every repetition, with Snappy and with Snappy | ETL_PQ_DICTIONARY: the CUDA-event time of the call (median over
 the repetitions, summed over the emits) and the index bytes as a share of the file.
+--bloom does the same with and without bloom filters (etl_dec_parquet_write_bloom) on every eligible column (fpp 0.01,
+ndv 0: the chunk's non-null count, max_bytes 0: 1 MiB): the call's CUDA-event time and the filter bytes' share.
 Prints the card name and power limit in the same run.
 """
 import argparse
@@ -71,7 +74,66 @@ def to_arrow(col):
     return pa.Array.from_buffers(PA_TYPE[t], n, [mask, pa.py_buffer(np.ascontiguousarray(col["values"]).tobytes())])
 
 
-OPTS = dict(plain_only=False, pyarrow=True, page_index=False)
+OPTS = dict(plain_only=False, pyarrow=True, page_index=False, bloom=False)
+
+
+def write_bloom(lib, a, fields, bloom, n, codec):
+    """etl_dec_parquet_write_bloom of rows [0, n), file in HBM; bloom None: a NULL array"""
+    arr = (abi.ParquetField * len(fields))()
+    names = [f[0].encode() for f in fields]
+    for i, (f, nm) in enumerate(zip(fields, names)):
+        arr[i].name, arr[i].field_id, arr[i].element_field_id, arr[i].required = nm, f[1], f[2], f[3]
+    barr = None
+    if bloom is not None:
+        barr = (abi.ParquetBloom * len(bloom))()
+        for i, (fpp, ndv, mb) in enumerate(bloom):
+            barr[i].fpp, barr[i].ndv, barr[i].max_bytes = fpp, ndv, mb
+    h = C.c_void_p()
+    rc = lib.etl_dec_parquet_write_bloom(a, arr, barr, len(fields), 0, n, codec, 0, C.byref(h))
+    return rc, h
+
+
+def bloom_emits(lib, emits, reps, warmup):
+    """bloom filters: per codec, the call's CUDA-event time without / with them, alternated, and their bytes"""
+    out = {}
+    for codec, name in ((abi.PQ_SNAPPY, "snappy"), (abi.PQ_SNAPPY | abi.PQ_DICTIONARY, "snappy_dict")):
+        ms, size = {0: [], 1: []}, {0: 0, 1: 0}
+        for a in emits:
+            cols = emit_columns(lib, a)
+            fields = fields_for(cols)
+            leaf_type = [c["child"]["type"] if c["type"] == R.LIST else c["type"] for c in cols]
+            bloom = [(0.0 if t == R.BOOLEAN else 0.01, 0, 0) for t in leaf_type]
+            n = lib.etl_dec_arrow_rows(a)
+            t = {0: [], 1: []}
+            for r in range(warmup + reps):
+                for on in (0, 1):
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    rc, h = write_bloom(lib, a, fields, bloom if on else None, n, codec)
+                    e1.record()
+                    e1.synchronize()
+                    assert rc == 0
+                    if r == 0:
+                        size[on] += lib.etl_dec_parquet_size(h)
+                    lib.etl_dec_parquet_free(h)
+                    if r >= warmup:
+                        t[on].append(e0.elapsed_time(e1))
+            for on in t:
+                ms[on].append(float(np.median(t[on])))
+        base, with_b = sum(ms[0]), sum(ms[1])
+        out[name] = dict(write_ms=round(base, 3), write_ms_bloom=round(with_b, 3),
+                         cost_pct=round(100 * (with_b - base) / base, 1) if base else None,
+                         file_bytes=int(size[0]), file_bytes_bloom=int(size[1]),
+                         bloom_share_pct=round(100 * (size[1] - size[0]) / size[1], 3) if size[1] else None)
+    return out
+
+
+def leg(lib, emits, reps, warmup):
+    if OPTS["bloom"]:
+        return bloom_emits(lib, emits, reps, warmup)
+    if OPTS["page_index"]:
+        return page_index_emits(lib, emits, reps, warmup)
+    return measure_emits(lib, emits, reps, warmup)
 
 
 def measure_emits(lib, emits, reps, warmup):
@@ -192,7 +254,7 @@ def copy_table(n_rows, reps, warmup, tag, low_card=False):
         assert lib.etl_dec_arrow_emit(bh._h, 0, KINDS, 1, C.byref(a)) == 0
         res = dict(tag=tag, workload="low-cardinality COPY table (int4, text, int4, date, uuid, text[])" if low_card
                    else "bench.py COPY table (5 x int4, 5 x text)", input_bytes=len(blob))
-        res.update(page_index_emits(lib, [a], reps, warmup) if OPTS["page_index"] else measure_emits(lib, [a], reps, warmup))
+        res.update(leg(lib, [a], reps, warmup))
         lib.etl_dec_arrow_free(a)
         print(json.dumps(res), flush=True)
     dec.close()
@@ -214,8 +276,7 @@ def streaming(name, scale, reps, warmup, tag):
             a = C.c_void_p()
             assert lib.etl_dec_arrow_emit(bh._h, si, KINDS, 1, C.byref(a)) == 0
             emits.append(a)
-        res.update(page_index_emits(lib, emits, reps, warmup) if OPTS["page_index"] else measure_emits(lib, emits, reps, warmup),
-                   versions=len(emits))
+        res.update(leg(lib, emits, reps, warmup), versions=len(emits))
         for a in emits:
             lib.etl_dec_arrow_free(a)
     st.close()
@@ -234,15 +295,16 @@ def main():
     ap.add_argument("--no-pyarrow", action="store_true")
     ap.add_argument("--tag", default="")
     ap.add_argument("--page-index", action="store_true")
+    ap.add_argument("--bloom", action="store_true")
     ap.add_argument("--c5-scale", type=float, default=0.02)
     a = ap.parse_args()
-    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index)
+    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index, bloom=a.bloom)
     if not torch.cuda.is_available():
         raise SystemExit("parquet_measure needs a CUDA device")
     t = time.time()
     print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
     copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
-    if a.page_index:
+    if a.page_index or a.bloom:
         for name, scale in (("c5", a.c5_scale), ("c4", a.c4_scale)):
             streaming(name, scale, a.reps, a.warmup, a.tag)
         print(json.dumps(dict(wall_s=round(time.time() - t, 1))), flush=True)
