@@ -296,7 +296,7 @@ DL_TEXT_ROW, DL_TEXT_PREDICATE, DL_TEXT_ASSIGNMENTS = 0, 1, 2
 DL_REJECT_UPDATE_NO_IDENTITY, DL_REJECT_DELETE_NO_IDENTITY, DL_REJECT_DELETE_NO_OLD_ROW, DL_REJECT_PARTIAL_KEY_MISSING = 1, 2, 3, 4
 
 # etl_dec_parquet_write codecs (ETL_PQ_*) and etl_parquet_metrics.flags
-PQ_UNCOMPRESSED, PQ_SNAPPY = 0, 1
+PQ_UNCOMPRESSED, PQ_SNAPPY, PQ_ZSTD = 0, 1, 6
 PQ_HAS_MIN_MAX = 1
 # codec bit: dictionary-encode the eligible column chunks (ETL_PQ_DICTIONARY)
 PQ_DICTIONARY = 0x100

@@ -41,7 +41,7 @@ enum { PAGE_DATA = 0, PAGE_DICTIONARY = 2 };
 constexpr uint32_t kPageRows = 20000;                 // a page ends after the row that brings it to this many rows
 constexpr uint64_t kPageBytes = 1ull << 20;           // … or to this many PLAIN value bytes
 constexpr uint64_t kRowGroupRows = 1ull << 20;
-constexpr uint32_t kFragment = 65536;                 // Snappy fragment
+constexpr uint32_t kFragment = 65536;                 // compressed independently (Snappy, Zstandard)
 constexpr uint32_t kSnappyHashBits = 12;
 constexpr uint32_t kStatMax = 64;                     // a longer byte-array min / max is not written
 constexpr uint32_t kPageHeaderMax = 48;               // 4 fields + a 4-field struct of i32 varints: at most 41 bytes

@@ -26,9 +26,14 @@
 //      arrays as length + bytes with every value copied by the whole warp.  The same pass reduces the page's statistics
 //      (min / max as item indices, NaN count).  The payload goes to a slot sized by the bound of the page.
 //   3. Compress (ETL_PQ_SNAPPY).  k_snappy, a CTA per 64 KiB fragment slot of every page, runs the fragment compressor
-//      of parquet_format.cuh on one thread, its hash table in shared memory, into a slot of snappy_bound bytes; k_page writes the length preamble and the page header
-//      (its varint widths depend on the sizes) and the page's file bytes; a scan gives the file offsets; k_gather, a CTA
-//      per page, copies header + payload (+ fragments) into the file buffer, whose size is the sum of the bounds.
+//      of parquet_format.cuh on one thread, its hash table in shared memory, into a slot of snappy_bound bytes.
+//      (ETL_PQ_ZSTD) k_zstd, in the same place and shape, runs the block compressor of zstd_format.cuh: each fragment
+//      one self-contained Zstandard block (header included) in a slot of zstd_bound bytes, its work space in shared
+//      memory, its literals and sequences in scratch placed by the fragment's payload position.  k_page writes the
+//      preamble (Snappy's length varint, or the 9-byte Zstandard frame header) and the page header (its varint widths
+//      depend on the sizes) and the page's file bytes; a scan gives the file offsets; k_gather, a CTA per page, copies
+//      header + payload (+ preamble and fragments) into the file buffer, whose size is the sum of the bounds.  The
+//      dictionary slot, the page index and the bloom filters follow csize / hlen, so they need nothing per codec.
 //   4. Statistics.  k_chunk, a thread per (leaf, row group), folds the page candidates and sizes of its chunk, k_leaf the
 //      chunks of a leaf; both write the PLAIN bytes of min / max (−0.0 / +0.0 for a zero float, none above 64 bytes).
 //   4b. Page index (ETL_PQ_PAGE_INDEX).  k_index<false>, a warp per chunk with lanes over its data pages: each page's
@@ -48,7 +53,8 @@
 //      SYNC 3 ends the call (and the copy to pinned host memory with to_host).
 // Scratch: per (row, leaf) 3 × 4 B lengths + 3 × 8 B prefix sums; per level entry 2 B (+ 64 B per page of the leaf);
 // Boolean leaves 1 bit per item (+ 4 B per page of the leaf); per page a bounded payload slot (the PLAIN value bytes + levels_bound per section) and,
-// with Snappy, a compressed slot of snappy_bound per fragment.  ETL_PQ_DICTIONARY adds, per item of an eligible leaf
+// with Snappy, a compressed slot of snappy_bound per fragment; with ETL_PQ_ZSTD, one of zstd_bound (64 KiB + 3 B) per
+// fragment, and 1 B of literal + 2 B of sequence scratch per payload byte (+ 8 B per fragment).  ETL_PQ_DICTIONARY adds, per item of an eligible leaf
 // (bounded by its level entries), 4 B slot + 4 B flag + 4 B entry size / index + 2 × 8 B prefix sums and 0.5 B of run
 // heads (+ 12 B per page), the chunks' tables (4 B × pow2 >= 2 × non-null values: at most 16 B per value), a dictionary
 // slot per chunk (at most 1 MiB, at most the chunk's PLAIN bytes) and 32 B more per data page slot.  ETL_PQ_PAGE_INDEX
@@ -67,6 +73,7 @@
 #include "etl_decode.h"
 #include "emit_scan.cuh"
 #include "parquet_format.cuh"
+#include "zstd_format.cuh"
 
 namespace {
 
@@ -94,11 +101,11 @@ struct Page {
   uint64_t it0, it1;         // items of the value column
   uint64_t nn, vbytes, ubound, lscr;   // non-null values, PLAIN value bytes, payload bound, level scratch offset
   uint64_t usize, csize;
-  uint32_t hlen, plen;       // page header / Snappy preamble bytes
+  uint32_t hlen, plen;       // page header / preamble bytes (Snappy's length varint, Zstandard's frame header)
   uint64_t min_it, max_it, nan;
   uint32_t kind, _pad;       // 0 data page; 1 the dictionary slot in front of a chunk's data pages (ETL_PQ_DICTIONARY)
   uint8_t hdr[kPageHeaderMax];
-  uint8_t pre[8];
+  uint8_t pre[12];           // at most 10 (a varint of a 32-bit size) or 9 (etl_zstd::kFrameHeader) bytes
 };
 struct ChunkOut {
   uint64_t offset, num_values, usize, csize, null_count, nan_count;
@@ -708,27 +715,53 @@ __global__ void __launch_bounds__(32) k_snappy(const Page* pages, uint32_t n_pag
   fsize[f] = snappy_fragment(uslot_base + uslot[lo] + off, len, cslot_base + cslot[lo] + 8 + k * snappy_bound(kFragment), table);
 }
 
+// 3'. ETL_PQ_ZSTD: a CTA per fragment slot, as k_snappy; one thread writes the fragment's block (a page of no bytes
+// gets one empty block), the work space in shared memory.  Its literals and sequences go to scratch placed by the
+// fragment's bytes in the payload slots: literal byte i of payload position u at lit[u], the sequences of fragment f
+// from seq[u0 / 4 + f] (u0 its first position), so no two fragments overlap.
+__global__ void __launch_bounds__(32) k_zstd(const Page* pages, uint32_t n_pages, const uint64_t* fbase, const uint8_t* uslot_base,
+                                             const uint64_t* uslot, uint8_t* cslot_base, const uint64_t* cslot, uint32_t* fsize,
+                                             uint8_t* lit, uint64_t* seq) {
+  __shared__ etl_zstd::Work W;
+  const uint64_t f = blockIdx.x;
+  if (threadIdx.x) return;
+  uint32_t lo = 0, hi = n_pages - 1;                      // the page: last fbase <= f
+  while (lo < hi) { const uint32_t m = (lo + hi + 1) / 2; if (fbase[m] <= f) lo = m; else hi = m - 1; }
+  const Page& P = pages[lo];
+  const uint64_t k = f - fbase[lo], off = k * kFragment;
+  if (off >= P.usize && off) { fsize[f] = 0; return; }
+  const uint32_t len = (uint32_t)(P.usize - off < kFragment ? P.usize - off : kFragment);
+  const uint64_t u = uslot[lo] + off;
+  fsize[f] = etl_zstd::zstd_block(uslot_base + u, len, off + len >= P.usize, cslot_base + cslot[lo] + 8 + k * etl_zstd::zstd_bound(kFragment),
+                                  W, lit + u, seq + u / 4 + f);
+}
+
+// the compressed slot of one fragment (comp: the codec, ETL_PQ_SNAPPY or ETL_PQ_ZSTD)
+__host__ __device__ inline uint32_t frag_slot(uint32_t comp) {
+  return comp == ETL_PQ_ZSTD ? etl_zstd::zstd_bound(kFragment) : snappy_bound(kFragment);
+}
+
 // a thread per page + 1: what the slot scans add up (0 payload bound, 1 compressed slot, 2 fragment slots); entry
 // n_pages is 0, so that the exclusive scan leaves the total there
-__global__ void k_fill(const Page* pages, uint32_t n_pages, int which, uint64_t* dst) {
+__global__ void k_fill(const Page* pages, uint32_t n_pages, int which, uint32_t comp, uint64_t* dst) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p > n_pages) return;
   if (p == n_pages) { dst[p] = 0; return; }
   const uint64_t nf = pages[p].ubound ? (pages[p].ubound + kFragment - 1) / kFragment : 1;
-  dst[p] = which == 0 ? pages[p].ubound : which == 1 ? 8 + nf * snappy_bound(kFragment) : nf;
+  dst[p] = which == 0 ? pages[p].ubound : which == 1 ? 8 + nf * frag_slot(comp) : nf;
 }
 
-// a thread per page: compressed size, preamble, header, file bytes of the page (D: ETL_PQ_DICTIONARY; the dictionary
-// slot of a chunk that is not dictionary-encoded has no bytes)
-__global__ void k_page(Page* pages, uint32_t n_pages, int snappy, const uint64_t* fbase, const uint32_t* fsize, uint64_t* fbytes,
+// a thread per page: compressed size, preamble, header, file bytes of the page (comp: the codec; D: ETL_PQ_DICTIONARY;
+// the dictionary slot of a chunk that is not dictionary-encoded has no bytes)
+__global__ void k_page(Page* pages, uint32_t n_pages, uint32_t comp, const uint64_t* fbase, const uint32_t* fsize, uint64_t* fbytes,
                        const DictChunk* D) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n_pages) return;
   Page& P = pages[p];
   const bool dict = D && D[P.chunk].dict;
   if (P.kind && !dict) { P.hlen = P.plen = 0; P.csize = 0; fbytes[p] = 0; return; }
-  if (snappy) {
-    P.plen = varint(P.usize, P.pre);
+  if (comp != ETL_PQ_UNCOMPRESSED) {
+    P.plen = comp == ETL_PQ_ZSTD ? etl_zstd::frame_header((uint32_t)P.usize, P.pre) : varint(P.usize, P.pre);
     uint64_t c = P.plen;
     for (uint64_t f = fbase[p]; f < fbase[p + 1]; f++) c += fsize[f];
     P.csize = c;
@@ -739,15 +772,16 @@ __global__ void k_page(Page* pages, uint32_t n_pages, int snappy, const uint64_t
 }
 
 // a CTA per page: header, preamble and payload (or its fragments) at the page's file offset
-__global__ void __launch_bounds__(256) k_gather(const Page* pages, int snappy, const uint64_t* foff, const uint8_t* uslot_base,
+__global__ void __launch_bounds__(256) k_gather(const Page* pages, uint32_t comp, const uint64_t* foff, const uint8_t* uslot_base,
                                                 const uint64_t* uslot, const uint8_t* cslot_base, const uint64_t* cslot,
                                                 const uint64_t* fbase, const uint32_t* fsize, uint8_t* file) {
   const uint32_t p = blockIdx.x;
   const Page& P = pages[p];
-  uint8_t* dst = file + 4 + foff[p];
+  if (!P.hlen) return;                                   // a dictionary slot without a dictionary has no bytes (k_zstd
+  uint8_t* dst = file + 4 + foff[p];                     // still wrote an empty block for it)
   for (uint32_t k = threadIdx.x; k < P.hlen; k += blockDim.x) dst[k] = P.hdr[k];
   dst += P.hlen;
-  if (!snappy) {
+  if (comp == ETL_PQ_UNCOMPRESSED) {
     const uint8_t* src = uslot_base + uslot[p];
     for (uint64_t k = threadIdx.x; k < P.usize; k += blockDim.x) dst[k] = src[k];
     return;
@@ -755,7 +789,7 @@ __global__ void __launch_bounds__(256) k_gather(const Page* pages, int snappy, c
   for (uint32_t k = threadIdx.x; k < P.plen; k += blockDim.x) dst[k] = P.pre[k];
   dst += P.plen;
   for (uint64_t f = fbase[p]; f < fbase[p + 1]; f++) {
-    const uint8_t* src = cslot_base + cslot[p] + 8 + (f - fbase[p]) * snappy_bound(kFragment);
+    const uint8_t* src = cslot_base + cslot[p] + 8 + (f - fbase[p]) * frag_slot(comp);
     for (uint32_t k = threadIdx.x; k < fsize[f]; k += blockDim.x) dst[k] = src[k];
     dst += fsize[f];
   }
@@ -1069,7 +1103,7 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   if (!a || !out || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
   const uint32_t cc = codec & 0xFFu;                  // the compression codec; the flag bits are ETL_PQ_DICTIONARY and
   if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) ||   // ETL_PQ_PAGE_INDEX
-      (codec & ~(0xFFu | ETL_PQ_DICTIONARY | ETL_PQ_PAGE_INDEX)) || (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY))
+      (codec & ~(0xFFu | ETL_PQ_DICTIONARY | ETL_PQ_PAGE_INDEX)) || (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY && cc != ETL_PQ_ZSTD))
     return ETL_ERR_INVALID_ARG;
   const int dict = (codec & ETL_PQ_DICTIONARY) != 0;
   const int pidx = (codec & ETL_PQ_PAGE_INDEX) != 0;
@@ -1127,7 +1161,8 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   const uint32_t nL = n_fields;
   const uint32_t n_rg = (uint32_t)((n + kRowGroupRows - 1) / kRowGroupRows);
   const uint32_t n_chunks = n_rg * nL;
-  const int snappy = cc == ETL_PQ_SNAPPY;
+  const int snappy = cc != ETL_PQ_UNCOMPRESSED;        // Snappy or Zstandard: compressed fragments
+  const int zstd = cc == ETL_PQ_ZSTD;
   auto bloomed = [&](uint32_t l) { return bloom && bloom[l].fpp > 0.0; };
   bool any_bloom = false;
   for (uint32_t l = 0; l < nL; l++) any_bloom |= bloomed(l);
@@ -1221,7 +1256,7 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   std::vector<uint64_t> leaf_page_base(n_chunks + 1, 0);   // pages of the chunk's leaf in the row groups before it
   for (uint32_t c = nL; c < n_chunks; c++) leaf_page_base[c] = leaf_page_base[c - nL] + np[c - nL];
   const uint64_t n_frag_bound = snappy ? U / kFragment + P + 1 : 0;
-  const uint64_t C_bound = snappy ? 8 * P + n_frag_bound * snappy_bound(kFragment) : 0;
+  const uint64_t C_bound = snappy ? 8 * P + n_frag_bound * frag_slot(cc) : 0;
   // bit scratch: page lp of a Boolean leaf starts at word bscr + it0 / 32 + lp
   uint64_t bool_words = 0;
   for (uint32_t l = 0; l < nL; l++)
@@ -1279,9 +1314,12 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   uint32_t* d_bool = (uint32_t*)dalloc(bool_words * 4 + 8);
   uint8_t* d_c = snappy ? (uint8_t*)dalloc(C_bound + 16) : nullptr;
   uint32_t* d_fsz = snappy ? (uint32_t*)dalloc(n_frag_bound * 4 + 4) : nullptr;
+  uint8_t* d_zlit = zstd ? (uint8_t*)dalloc(U + 16) : nullptr;                            // ETL_PQ_ZSTD: literals and
+  uint64_t* d_zseq = zstd ? (uint64_t*)dalloc(8 * (U / 4 + n_frag_bound + 1)) : nullptr;  // sequences of k_zstd
   ChunkOut* d_cout = (ChunkOut*)dalloc(sizeof(ChunkOut) * (n_chunks + nL) + 16ull * n_chunks);
   ChunkOut* d_lout = d_cout ? (ChunkOut*)((uint8_t*)d_cout + sizeof(ChunkOut) * n_chunks + 16ull * n_chunks) : nullptr;
-  if (!d_pages || !d_pbase || !d_lbase || !d_lscr || !d_scan || !d_stot || !d_u || !d_bool || !d_cout || (snappy && (!d_c || !d_fsz)))
+  if (!d_pages || !d_pbase || !d_lbase || !d_lscr || !d_scan || !d_stot || !d_u || !d_bool || !d_cout || (snappy && (!d_c || !d_fsz)) ||
+      (zstd && (!d_zlit || !d_zseq)))
     return fail(ETL_ERR_ALLOC);
   DictChunk* d_dch = nullptr;
   unsigned long long* d_tabn = nullptr;
@@ -1333,7 +1371,7 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
     k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages, dict);
     // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
     auto fill_scan = [&](int which, uint64_t* dst) {
-      k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, dst);
+      k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, cc, dst);
       k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)dst, (uint32_t)(P + 1), d_stot + which);
     };
     fill_scan(0, uslot);
@@ -1365,12 +1403,13 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
     if (snappy) {
       fill_scan(1, cslot);
       fill_scan(2, fbase);
-      k_snappy<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz);
+      if (zstd) k_zstd<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz, d_zlit, d_zseq);
+      else k_snappy<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz);
     }
-    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, snappy, fbase, d_fsz, foff, d_dch);
+    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, cc, fbase, d_fsz, foff, d_dch);
     CK(cudaMemsetAsync(foff + P, 0, 8, st));
     k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
-    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, snappy, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
+    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, cc, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
     k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout, d_dch);
     if (bloom_total) {
       // bloom filters: the bitsets in scratch, then headers and bitsets behind the pages
@@ -1465,9 +1504,10 @@ void etl_dec_parquet_free(etl_parquet_file* f) {
 }  // extern "C"
 
 // ptxas -v, sm_90a, CUDA 12.9 (registers / shared memory / stack):
-//   k_plan 32 / 0 / 0      k_cut 53 / 0 / 0       k_encode<false> 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 12 / 0 / 0
+//   k_plan 32 / 0 / 0      k_cut 53 / 0 / 0       k_encode<false> 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 10 / 0 / 0
 //   k_encode<true> 64 / 4200 B / 16 B (two 8-byte spills)
-//   k_snappy 50 / 8192 B / 0                      k_page 29 / 0 / 40 B (the header bytes)   k_gather 23 / 0 / 0
+//   k_snappy 50 / 8192 B / 0                      k_page 29 / 0 / 40 B (the header bytes)   k_gather 22 / 0 / 0
+//   k_zstd 88 / 27772 B / 104 B, no spills (the stack is the canonical-code rank counters of the Huffman table)
 //   k_dict_setup 24 / 0 / 0   k_dict_place 10 / 0 / 0   k_dict_insert 46 / 0 / 0   k_dict_mark 24 / 0 / 0
 //   k_dict_finish 22 / 0 / 0  k_dict_page 32 / 0 / 0
 //   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)

@@ -774,7 +774,7 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * fields: one per emitted column, in order (n_fields == etl_dec_arrow_cols).  ETL_ERR_INVALID_ARG, before any launch:
  * another n_fields or none (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS), an ETL_ARROW_UNSUPPORTED
  * column (the emit lacked ETL_ARROW_ALL_COLUMNS), row_begin > row_end or row_end > etl_dec_arrow_rows, an unknown
- * codec (codec & 0xFF other than ETL_PQ_UNCOMPRESSED / ETL_PQ_SNAPPY) or a codec bit other than ETL_PQ_DICTIONARY and
+ * codec (codec & 0xFF other than ETL_PQ_UNCOMPRESSED / ETL_PQ_SNAPPY / ETL_PQ_ZSTD) or a codec bit other than ETL_PQ_DICTIONARY and
  * ETL_PQ_PAGE_INDEX, a NULL or empty name or one longer than 1 KiB; with bloom, an fpp that is NaN, negative or >= 1,
  * a max_bytes that is neither 0 nor a power of two in [32, 2^27], or fpp > 0 on a Boolean leaf (Arrow C++ has no
  * filters for BOOLEAN either).
@@ -804,6 +804,16 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  *          max definition level 3 (optional list) or 2 (required), max repetition level 1.
  *   codec: ETL_PQ_SNAPPY compresses each page's levels + values as one Snappy stream: the varint length, then the
  *          elements of independent 64 KiB fragments (no copy crosses a fragment).  Page headers are not compressed.
+ *          ETL_PQ_ZSTD (Parquet's ZSTD) compresses each page's levels + values, and each dictionary page's entries, as
+ *          one Zstandard frame (RFC 8878).  Frame header, 9 bytes: the magic 28 B5 2F FD, Frame_Header_Descriptor 0xA0
+ *          (Single_Segment, a 4-byte Frame_Content_Size, no checksum, no dictionary id), then the Frame_Content_Size =
+ *          the uncompressed page size (LE).  Blocks: exactly one per 64 KiB fragment of the payload, Last_Block set on
+ *          the last one only; an empty payload is one empty last Raw block.  Every block is self-contained: no match
+ *          reaches before its fragment's start, no offset is a repeat-offset code, Huffman literals always carry their
+ *          own table (never Treeless), sequence modes are Predefined, RLE or FSE_Compressed (never Repeat).  A
+ *          Compressed block is used only when strictly smaller than its fragment; otherwise the block is RLE when all its
+ *          bytes are equal, else Raw.  The encoder has one fixed strategy (no level).  uncompressed_page_size is
+ *          unchanged; compressed_page_size is the frame's length.
  *   statistics: per column chunk null_count, max_value, min_value in the type's order (signed ints / dates / times,
  *          unsigned bytewise BYTE_ARRAY / UUID, false < true), NaN excluded, a zero minimum written as -0.0 and a zero
  *          maximum as +0.0; none when the chunk has no non-NaN value or a byte-array min / max is longer than 64 bytes.
@@ -891,13 +901,14 @@ void etl_dec_ducklake_free(etl_ducklake_batch*);
  * the PLAIN statistic bytes, which equal Iceberg's single-value serialization of these types (before truncation).
  * to_host: also copy the file to pinned host memory (etl_dec_parquet_bytes(f, 1); else NULL).  Scratch, beside the
  * file: 36 B per (row, column), 2 B per level entry + 64 B per page, 1 bit per Boolean value, a payload slot per page (values +
- * level bound) and with Snappy a compressed slot per 64 KiB of payload; with ETL_PQ_DICTIONARY also 28 B per item of an
+ * level bound) and with Snappy a compressed slot per 64 KiB of payload (with ETL_PQ_ZSTD a slot of 64 KiB + 3 B, and 3 B
+ * of literal / sequence scratch per payload byte + 8 B per fragment); with ETL_PQ_DICTIONARY also 28 B per item of an
  * eligible leaf (bounded by its level entries) + 0.5 B per item of run heads, a dictionary slot per chunk of at most
  * 1 MiB, 32 B per data page, and hash tables of at most 16 B per non-null value; with ETL_PQ_PAGE_INDEX 40 B per chunk
  * and, in the file's buffer, 189 B per page + 64 B per chunk (+ the longest row per page of a byte-array leaf with a
  * value over 64 bytes, at most its value bytes); with bloom filters 8 B per chunk, 24 B per chunk record and each
  * filtered chunk's bitset in scratch, and in the file's buffer its bitset + header (at most 19 B). */
-enum { ETL_PQ_UNCOMPRESSED = 0, ETL_PQ_SNAPPY = 1 };
+enum { ETL_PQ_UNCOMPRESSED = 0, ETL_PQ_SNAPPY = 1, ETL_PQ_ZSTD = 6 };   /* Parquet's CompressionCodec values */
 #define ETL_PQ_DICTIONARY 0x100u   /* OR-ed into codec: dictionary-encode the eligible column chunks (codec & 0xFF: compression) */
 #define ETL_PQ_PAGE_INDEX 0x400u   /* OR-ed into codec: write a ColumnIndex and an OffsetIndex per column chunk */
 #define ETL_PQ_HAS_MIN_MAX 1u   /* etl_parquet_metrics.flags: min / max are set */

@@ -5,6 +5,7 @@
                                   [--plain-only] [--no-pyarrow] [--tag NAME]
   python tools/parquet_measure.py --page-index [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
   python tools/parquet_measure.py --bloom [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
+  python tools/parquet_measure.py --zstd [--copy-rows 1000000] [--c2-scale 0.05] [--c3-scale 1] [--c5-scale 0.02] [--reps 7]
 
 Workloads: bench.py's 10-column COPY table, C3 (one schema version) and C4 (every schema version: times and sizes are
 sums over the versions), each emitted once with 7 | ETL_ARROW_ALL_COLUMNS | ETL_ARROW_CDC_COLUMNS and kept in HBM.
@@ -23,6 +24,10 @@ two in every repetition, with Snappy and with Snappy | ETL_PQ_DICTIONARY: the CU
 the repetitions, summed over the emits) and the index bytes as a share of the file.
 --bloom does the same with and without bloom filters (etl_dec_parquet_write_bloom) on every eligible column (fpp 0.01,
 ndv 0: the chunk's non-null count, max_bytes 0: 1 MiB): the call's CUDA-event time and the filter bytes' share.
+--zstd writes each emit of the COPY table, C2, C3 and C5 uncompressed, with Snappy and with ETL_PQ_ZSTD, each with and
+without ETL_PQ_DICTIONARY, the six calls alternated in every repetition: the call's CUDA-event time (median, summed over
+the emits), the file bytes, and from one torch.profiler pass per codec the device time of the compression kernel
+(k_snappy / k_zstd) against the call's other kernels.
 Prints the card name and power limit in the same run.
 """
 import argparse
@@ -74,7 +79,7 @@ def to_arrow(col):
     return pa.Array.from_buffers(PA_TYPE[t], n, [mask, pa.py_buffer(np.ascontiguousarray(col["values"]).tobytes())])
 
 
-OPTS = dict(plain_only=False, pyarrow=True, page_index=False, bloom=False)
+OPTS = dict(plain_only=False, pyarrow=True, page_index=False, bloom=False, zstd=False)
 
 
 def write_bloom(lib, a, fields, bloom, n, codec):
@@ -128,7 +133,65 @@ def bloom_emits(lib, emits, reps, warmup):
     return out
 
 
+ZSTD_LEGS = [(c | d, n + ("_dict" if d else "")) for d in (0, abi.PQ_DICTIONARY)
+             for c, n in ((abi.PQ_UNCOMPRESSED, "uncompressed"), (abi.PQ_SNAPPY, "snappy"), (abi.PQ_ZSTD, "zstd"))]
+
+
+def _kernel_ms(lib, emits, codec):
+    """device time of one call per emit under torch.profiler: (compression kernel, every other kernel), ms"""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for a in emits:
+            cols = emit_columns(lib, a)
+            rc, h = write_bloom(lib, a, fields_for(cols), None, lib.etl_dec_arrow_rows(a), codec)
+            assert rc == 0
+            lib.etl_dec_parquet_free(h)
+        torch.cuda.synchronize()
+    comp = other = 0.0
+    for e in prof.key_averages():
+        us = getattr(e, "device_time_total", None)
+        if us is None:
+            us = e.cuda_time_total
+        if e.device_type is not None and str(e.device_type).endswith("CUDA") and us:
+            if "k_zstd" in e.key or "k_snappy" in e.key:
+                comp += us
+            elif "k_" in e.key:
+                other += us
+    return round(comp / 1e3, 3), round(other / 1e3, 3)
+
+
+def zstd_emits(lib, emits, reps, warmup):
+    """ETL_PQ_ZSTD: per codec and dictionary flag, the call's CUDA-event time (six calls alternated) and file bytes"""
+    ms = {n: [] for _, n in ZSTD_LEGS}
+    size = {n: 0 for _, n in ZSTD_LEGS}
+    for a in emits:
+        fields = fields_for(emit_columns(lib, a))
+        n = lib.etl_dec_arrow_rows(a)
+        t = {name: [] for _, name in ZSTD_LEGS}
+        for r in range(warmup + reps):
+            for codec, name in ZSTD_LEGS:
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                rc, h = write_bloom(lib, a, fields, None, n, codec)
+                e1.record()
+                e1.synchronize()
+                assert rc == 0
+                if r == 0:
+                    size[name] += lib.etl_dec_parquet_size(h)
+                lib.etl_dec_parquet_free(h)
+                if r >= warmup:
+                    t[name].append(e0.elapsed_time(e1))
+        for name in t:
+            ms[name].append(float(np.median(t[name])))
+    out = {name: dict(write_ms=round(sum(ms[name]), 3), file_bytes=int(size[name])) for _, name in ZSTD_LEGS}
+    for codec, name in ((abi.PQ_SNAPPY, "snappy"), (abi.PQ_ZSTD, "zstd")):
+        out[name]["compress_kernel_ms"], out[name]["other_kernels_ms"] = _kernel_ms(lib, emits, codec)
+    return out
+
+
 def leg(lib, emits, reps, warmup):
+    if OPTS["zstd"]:
+        return zstd_emits(lib, emits, reps, warmup)
     if OPTS["bloom"]:
         return bloom_emits(lib, emits, reps, warmup)
     if OPTS["page_index"]:
@@ -297,13 +360,20 @@ def main():
     ap.add_argument("--page-index", action="store_true")
     ap.add_argument("--bloom", action="store_true")
     ap.add_argument("--c5-scale", type=float, default=0.02)
+    ap.add_argument("--zstd", action="store_true")
+    ap.add_argument("--c2-scale", type=float, default=0.05)
     a = ap.parse_args()
-    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index, bloom=a.bloom)
+    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index, bloom=a.bloom, zstd=a.zstd)
     if not torch.cuda.is_available():
         raise SystemExit("parquet_measure needs a CUDA device")
     t = time.time()
     print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
     copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
+    if a.zstd:
+        for name, scale in (("c2", a.c2_scale), ("c3", a.c3_scale), ("c5", a.c5_scale)):
+            streaming(name, scale, a.reps, a.warmup, a.tag)
+        print(json.dumps(dict(wall_s=round(time.time() - t, 1))), flush=True)
+        return
     if a.page_index or a.bloom:
         for name, scale in (("c5", a.c5_scale), ("c4", a.c4_scale)):
             streaming(name, scale, a.reps, a.warmup, a.tag)
