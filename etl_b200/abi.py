@@ -92,6 +92,14 @@ class ParquetBloom(C.Structure):
     _fields_ = [("fpp", C.c_double), ("ndv", C.c_uint64), ("max_bytes", C.c_uint32), ("_pad", C.c_uint32)]
 
 
+class IcebergPartitionField(C.Structure):
+    _fields_ = [("source_column", C.c_uint32), ("transform", C.c_uint32), ("param", C.c_uint32), ("_pad", C.c_uint32)]
+
+
+class IcebergPartitionValue(C.Structure):
+    _fields_ = [("is_null", C.c_uint32), ("len", C.c_uint32), ("value", C.c_int64), ("data", C.c_void_p)]
+
+
 class Planes(C.Structure):
     _fields_ = [("n_records", C.c_uint64), ("n_cells", C.c_uint64), ("heap_bytes", C.c_uint64),
                 ("rec_off", C.c_void_p), ("rec_kind", C.c_void_p), ("rec_flags", C.c_void_p), ("rec_rel", C.c_void_p),
@@ -135,6 +143,8 @@ EXPORTS = [
     "etl_dec_ducklake_text", "etl_dec_ducklake_issues", "etl_dec_ducklake_sub_batches", "etl_dec_ducklake_copy_fingerprint",
     "etl_dec_ducklake_free", "etl_dec_parquet_write", "etl_dec_parquet_write_bloom", "etl_dec_parquet_size", "etl_dec_parquet_bytes", "etl_dec_parquet_metrics",
     "etl_dec_parquet_required_null", "etl_dec_parquet_free",
+    "etl_dec_iceberg_partition", "etl_dec_iceberg_partitions", "etl_dec_iceberg_partition_rows", "etl_dec_iceberg_partition_value",
+    "etl_dec_iceberg_partitioned_arrow", "etl_dec_iceberg_partition_free",
     "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
     "etl_shim_json_text", "etl_shim_event_list_free",
 ]
@@ -260,6 +270,17 @@ def load(build: bool = True):
     L.etl_dec_parquet_required_null.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     L.etl_dec_parquet_free.argtypes = [vp]
     L.etl_dec_parquet_free.restype = None
+    L.etl_dec_iceberg_partition.argtypes = [vp, C.POINTER(IcebergPartitionField), C.c_uint32, C.c_uint64, C.c_uint64, C.c_int,
+                                            C.POINTER(vp)]
+    L.etl_dec_iceberg_partitions.argtypes = [vp]
+    L.etl_dec_iceberg_partitions.restype = C.c_uint64
+    L.etl_dec_iceberg_partition_rows.argtypes = [vp, C.c_int]
+    L.etl_dec_iceberg_partition_rows.restype = C.c_void_p
+    L.etl_dec_iceberg_partition_value.argtypes = [vp, C.c_uint64, C.c_uint32, C.POINTER(IcebergPartitionValue)]
+    L.etl_dec_iceberg_partitioned_arrow.argtypes = [vp]
+    L.etl_dec_iceberg_partitioned_arrow.restype = C.c_void_p
+    L.etl_dec_iceberg_partition_free.argtypes = [vp]
+    L.etl_dec_iceberg_partition_free.restype = None
     L.etl_dec_batch_device_stream.argtypes = [vp]
     L.etl_dec_batch_device_stream.restype = C.c_void_p
     L.etl_shim_materialise.argtypes = [vp, vp, vp, C.POINTER(vp)]
@@ -302,6 +323,10 @@ PQ_HAS_MIN_MAX = 1
 PQ_DICTIONARY = 0x100
 # codec bit: write a ColumnIndex and an OffsetIndex per column chunk (ETL_PQ_PAGE_INDEX)
 PQ_PAGE_INDEX = 0x400
+
+# etl_iceberg_partition_field.transform (ETL_ICE_*) and the most fields of one spec (ETL_ICE_MAX_FIELDS)
+ICE_IDENTITY, ICE_BUCKET, ICE_TRUNCATE, ICE_YEAR, ICE_MONTH, ICE_DAY, ICE_HOUR, ICE_VOID = range(8)
+ICE_MAX_FIELDS = 16
 
 # etl_dec_summary.sizing bits (ETL_SIZING_*)
 SIZING_EXACT = 0x01

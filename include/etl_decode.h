@@ -952,6 +952,82 @@ int etl_dec_parquet_metrics(const etl_parquet_file*, uint32_t leaf, etl_parquet_
 int etl_dec_parquet_required_null(const etl_parquet_file*, uint32_t* column, uint64_t* row);
 void etl_dec_parquet_free(etl_parquet_file*);
 
+/* ---------------------------------------------------------------- Iceberg partitioning
+ * Rows [row_begin, row_end) of an Arrow emit grouped by the partition tuple of an Iceberg partition spec, on the device:
+ * a permuted copy of the emit in which every partition is one contiguous row range, so that each partition's data file
+ * is one etl_dec_parquet_write(_bloom) call over that range.  The reference writes unpartitioned tables only
+ * (iceberg/client.rs:355-356 builds every DataFile with no partition key); this is what a partitioned table needs.
+ * spec: n_fields (1 .. 16) partition fields, each a source column of the emit (table columns and both CDC columns), an
+ * ETL_ICE_* transform and its parameter (bucket: N, truncate: W, both in 1 .. INT32_MAX; 0 for every other transform).
+ * Transforms (Iceberg spec "Partition Transforms"; the source types are the emit's):
+ *   identity     Boolean, Int32, Int64, Date32, Time64, Timestamp(tz), Utf8, LargeBinary, UUID: the value itself
+ *   bucket[N]    Int32, Int64, Date32, Time64, Timestamp(tz), Utf8, LargeBinary, UUID: (murmur3_x86_32(bytes, seed 0) &
+ *                INT32_MAX) % N, where bytes are (Appendix B) the value widened to a little-endian int64 for the integer
+ *                types (days for Date32, micros for Time64 and timestamps), the UTF-8 bytes of Utf8, the bytes of
+ *                LargeBinary and the 16 bytes of a UUID in RFC 4122 order (the order FixedSizeBinary(16) holds)
+ *   truncate[W]  Int32, Int64: v - (((v % W) + W) % W) in the source's width, wrapping like two's-complement Java / Rust
+ *                (truncate[10] of INT32_MIN is 2147483646); Utf8: the first W code points; LargeBinary: the first W bytes
+ *   year, month  Date32, Timestamp(tz): year(d) - 1970 and (year(d) - 1970) * 12 + month(d) - 1 of the proleptic
+ *                Gregorian date (iceberg-rust's and PyIceberg's formulas: 1969-12-31 is year -1 and month -1)
+ *   day          Date32: the day count; Timestamp(tz): floor(micros / 86 400 000 000)
+ *   hour         Timestamp(tz): floor(micros / 3 600 000 000)
+ *   void         any column that is neither a List nor ETL_ARROW_UNSUPPORTED: always null
+ * A Timestamptz is in UTC; a naive Timestamp is taken on its stored micros.  A null source gives a null result.  Float
+ * sources are rejected for every transform but void (engines disagree on -0.0 / 0.0 and on NaN grouping).
+ * Grouping: two rows share a partition when every field's null flag and result are equal (integers by value, bytes by
+ * content).  Partitions come in the order of their first row; inside a partition rows keep emit order, so
+ * sequence_number stays ascending inside every file.  The order depends on the input alone, not on scheduling.
+ * Result:
+ *   etl_dec_iceberg_partitions             P, the number of partitions (0 for zero rows);
+ *   etl_dec_iceberg_partition_rows         P + 1 row offsets: partition k is rows [rows[k], rows[k + 1]) of the
+ *                                          partitioned emit (host = 1: host memory, 0: device memory);
+ *   etl_dec_iceberg_partition_value        partition k's result of field f: is_null, value (every integer result,
+ *                                          sign-extended; Boolean 0 / 1) or len / data (Utf8, LargeBinary and UUID
+ *                                          results; data in host memory owned by the result);
+ *   etl_dec_iceberg_partitioned_arrow      the partitioned emit: row_end - row_begin rows, the source's columns, types,
+ *                                          List children and CDC columns with the rows permuted; its
+ *                                          etl_dec_arrow_row_records permuted the same way and its
+ *                                          etl_dec_arrow_first_skipped the source's.  A genuine etl_arrow_batch for
+ *                                          etl_dec_arrow_column / _list_child / etl_dec_parquet_write(_bloom), owned by
+ *                                          the result (never etl_dec_arrow_free it); with to_host it has a host image.
+ * The result owns everything it returns: the source emit may be freed right after the call.
+ * ETL_ERR_INVALID_ARG, before any launch: a NULL emit, spec or out; n_fields 0 (an unpartitioned table writes the emit
+ * directly) or above 16; a source column out of range, a List or ETL_ARROW_UNSUPPORTED column; a transform / type pair
+ * not in the table (a float source included); an unknown transform; N or W of 0 or above INT32_MAX, or a non-zero param
+ * on another transform; row_begin > row_end or row_end > etl_dec_arrow_rows; 2^32 rows or more.  A CUDA failure is
+ * ETL_ERR_CUDA and leaks nothing.
+ * Work: one thread per row computes every field's result and a tuple hash; a device hash table keyed by the tuple (full
+ * compare on a hash match, atomicMin of the first row) finds the partitions; a scan of the first-row flags ranks them; a
+ * stable radix sort of (rank, row) gives the permutation; every column, List children included, is gathered through it
+ * (bits by ballot, fixed-width values, offsets from the permuted lengths, bytes a warp per row).  Host syncs: one for the
+ * partition count and the representative values' sizes, then the final one.  Scratch: 13 B per (row, field), 12 B per
+ * (row, field with a byte-valued result), 64–84 B per row (the hash table, ranks, the sort's keys, rows and temporary
+ * storage), 4 B per row of each variable-width column and 4 B per element of each List; the output is the size of the
+ * source rows it holds. */
+enum { ETL_ICE_IDENTITY = 0, ETL_ICE_BUCKET = 1, ETL_ICE_TRUNCATE = 2, ETL_ICE_YEAR = 3, ETL_ICE_MONTH = 4, ETL_ICE_DAY = 5,
+       ETL_ICE_HOUR = 6, ETL_ICE_VOID = 7 };
+#define ETL_ICE_MAX_FIELDS 16u
+typedef struct etl_iceberg_partition_field {
+  uint32_t source_column;   /* column of the emit (table columns and CDC columns; not a List) */
+  uint32_t transform;       /* ETL_ICE_* */
+  uint32_t param;           /* bucket: N, truncate: W (1 .. INT32_MAX); 0 for every other transform */
+  uint32_t _pad;
+} etl_iceberg_partition_field;
+typedef struct etl_iceberg_partition_value {
+  uint32_t is_null, len;    /* len: bytes at data (Utf8 / LargeBinary / UUID results), else 0 */
+  int64_t value;            /* every integer-valued result, sign-extended; Boolean 0 / 1 */
+  const uint8_t* data;      /* host memory owned by the result, valid until free; NULL for integer results */
+} etl_iceberg_partition_value;
+typedef struct etl_iceberg_partitioned etl_iceberg_partitioned;
+int etl_dec_iceberg_partition(const etl_arrow_batch*, const etl_iceberg_partition_field* spec, uint32_t n_fields,
+                              uint64_t row_begin, uint64_t row_end, int to_host, etl_iceberg_partitioned** out);
+uint64_t etl_dec_iceberg_partitions(const etl_iceberg_partitioned*);
+const uint64_t* etl_dec_iceberg_partition_rows(const etl_iceberg_partitioned*, int host);   /* P + 1 entries */
+int etl_dec_iceberg_partition_value(const etl_iceberg_partitioned*, uint64_t partition, uint32_t field,
+                                    etl_iceberg_partition_value* out);
+const etl_arrow_batch* etl_dec_iceberg_partitioned_arrow(const etl_iceberg_partitioned*);
+void etl_dec_iceberg_partition_free(etl_iceberg_partitioned*);
+
 /* device address of the staged stream a batch was decoded from (string / json cells are offsets into it); valid until
  * the next decode on the same context (library-owned copy) or as long as the caller's dev_buf lives */
 const uint8_t* etl_dec_batch_device_stream(const etl_dec_batch*);

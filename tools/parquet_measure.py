@@ -6,6 +6,7 @@
   python tools/parquet_measure.py --page-index [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
   python tools/parquet_measure.py --bloom [--copy-rows 1000000] [--c5-scale 0.02] [--c4-scale 0.1] [--reps 7]
   python tools/parquet_measure.py --zstd [--copy-rows 1000000] [--c2-scale 0.05] [--c3-scale 1] [--c5-scale 0.02] [--reps 7]
+  python tools/parquet_measure.py --partition [--copy-rows 1000000] [--c1-scale 10] [--c2-scale 0.05] [--c5-scale 0.02]
 
 Workloads: bench.py's 10-column COPY table, C3 (one schema version) and C4 (every schema version: times and sizes are
 sums over the versions), each emitted once with 7 | ETL_ARROW_ALL_COLUMNS | ETL_ARROW_CDC_COLUMNS and kept in HBM.
@@ -28,6 +29,15 @@ ndv 0: the chunk's non-null count, max_bytes 0: 1 MiB): the call's CUDA-event ti
 without ETL_PQ_DICTIONARY, the six calls alternated in every repetition: the call's CUDA-event time (median, summed over
 the emits), the file bytes, and from one torch.profiler pass per codec the device time of the compression kernel
 (k_snappy / k_zstd) against the call's other kernels.
+--partition partitions each emit with etl_dec_iceberg_partition (C1 day(created), C2 bucket[16](id), the COPY table
+bucket[16](c0) + truncate[1](c5), C5 bucket[16](id)) and writes every partition's Snappy file from the partitioned emit;
+the unpartitioned Snappy write of the same rows is alternated with it in every repetition.  Reported: the partition
+call's CUDA-event time, its device time from one torch.profiler pass split into transform + group (k_ice_transform …
+k_ice_reps and the radix sort), the length scans and the gather (k_ice_gather_*), the gather's bytes moved (the
+partitioned emit read from the source and written once: 2 × its column bytes) per second as a kernel share of the
+3.35 TB/s data sheet figure, P, and the whole partitioned write (partition + P file writes) against the unpartitioned
+write.  Before timing, the partition offsets, values and every column of the partitioned emit are compared with
+tests/iceberg_partition_ref.py; every timed file must have the bytes of the first repetition's.
 Prints the card name and power limit in the same run.
 """
 import argparse
@@ -79,7 +89,7 @@ def to_arrow(col):
     return pa.Array.from_buffers(PA_TYPE[t], n, [mask, pa.py_buffer(np.ascontiguousarray(col["values"]).tobytes())])
 
 
-OPTS = dict(plain_only=False, pyarrow=True, page_index=False, bloom=False, zstd=False)
+OPTS = dict(plain_only=False, pyarrow=True, page_index=False, bloom=False, zstd=False, partition=False, spec=None)
 
 
 def write_bloom(lib, a, fields, bloom, n, codec):
@@ -189,7 +199,146 @@ def zstd_emits(lib, emits, reps, warmup):
     return out
 
 
+def _emit_bytes(lib, a):
+    """bytes of an emit's column buffers: validity, values, offsets and data, List children included"""
+    n = lib.etl_dec_arrow_rows(a)
+
+    def flat(col, items):
+        b = (items + 7) // 8
+        t = col.arrow_type
+        if t == R.BOOLEAN:
+            return 2 * b
+        if t in R.WIDTH:
+            return b + items * R.WIDTH[t]
+        return b + (items + 1) * (8 if t == R.LARGE_BINARY else 4) + col.data_bytes
+    total = 8 * n                                          # row records
+    for c in range(lib.etl_dec_arrow_cols(a)):
+        col = abi.ArrowColumn()
+        lib.etl_dec_arrow_column(a, c, 0, C.byref(col))
+        total += flat(col, n)
+        if col.arrow_type == R.LIST:
+            kid, ne = abi.ArrowColumn(), C.c_uint64()
+            lib.etl_dec_arrow_list_child(a, c, 0, C.byref(kid), C.byref(ne))
+            total += flat(kid, ne.value)
+    return total
+
+
+def _partition(lib, a, spec, n, to_host=0):
+    arr = (abi.IcebergPartitionField * len(spec))()
+    for i, (c, tr, p) in enumerate(spec):
+        arr[i].source_column, arr[i].transform, arr[i].param = c, tr, p
+    h = C.c_void_p()
+    assert lib.etl_dec_iceberg_partition(a, arr, len(spec), 0, n, to_host, C.byref(h)) == 0
+    return h
+
+
+def _check_partition(lib, a, spec):
+    """the partition of the whole emit against tests/iceberg_partition_ref.py; returns the partition count"""
+    import iceberg_partition_ref as IP
+    from test_gpu_parquet import _norm_ref
+    cols = emit_columns(lib, a)
+    n = lib.etl_dec_arrow_rows(a)
+    perm, offs, values = IP.partition(cols, spec, 0, n)
+    h = _partition(lib, a, spec, n, 1)
+    P = lib.etl_dec_iceberg_partitions(h)
+    rows = np.frombuffer((C.c_uint64 * (P + 1)).from_address(lib.etl_dec_iceberg_partition_rows(h, 1)), dtype=np.uint64)
+    assert rows.tolist() == offs
+    v = abi.IcebergPartitionValue()
+    for k in range(P):
+        for f in range(len(spec)):
+            assert lib.etl_dec_iceberg_partition_value(h, k, f, C.byref(v)) == 0
+            got = None if v.is_null else bytes((C.c_uint8 * v.len).from_address(v.data)) if v.data else v.value
+            assert got == values[k][f], (k, f)
+    got = emit_columns(lib, lib.etl_dec_iceberg_partitioned_arrow(h))
+    for g, c in zip(got, cols):
+        assert _norm_ref(g) == _norm_ref(IP.take(c, perm))
+    lib.etl_dec_iceberg_partition_free(h)
+    return P
+
+
+def _partition_kernel_ms(lib, a, spec, n):
+    """device time of one partition call under torch.profiler: (transform + group, scans, gather), ms"""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        lib.etl_dec_iceberg_partition_free(_partition(lib, a, spec, n))
+        torch.cuda.synchronize()
+    group = scan = gather = 0.0
+    for e in prof.key_averages():
+        us = getattr(e, "device_time_total", None)
+        if us is None:
+            us = e.cuda_time_total
+        if e.device_type is None or not str(e.device_type).endswith("CUDA") or not us:
+            continue
+        if "k_ice_gather" in e.key:
+            gather += us
+        elif "k_ice_" in e.key or "RadixSort" in e.key:
+            group += us
+        elif "k_len_blocks" in e.key or "k_blk_scan" in e.key or "k_offsets" in e.key:
+            scan += us
+    return group / 1e3, scan / 1e3, gather / 1e3
+
+
+def partition_emits(lib, emits, reps, warmup):
+    """--partition: see the module docstring; sums over the emits"""
+    spec = OPTS["spec"]
+    codec = abi.PQ_SNAPPY
+    call, whole, plain, files, parts, moved, group, scan, gather = [], [], [], 0, 0, 0, 0.0, 0.0, 0.0
+    for a in emits:
+        fields = fields_for(emit_columns(lib, a))
+        n = lib.etl_dec_arrow_rows(a)
+        parts += _check_partition(lib, a, spec)
+        g, s, k = _partition_kernel_ms(lib, a, spec, n)
+        group, scan, gather = group + g, scan + s, gather + k
+        moved += 2 * _emit_bytes(lib, a)
+        first, t_call, t_whole, t_plain = None, [], [], []
+        for r in range(warmup + reps):
+            e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+            e[0].record()
+            h = _partition(lib, a, spec, n)
+            e[1].record()
+            pa_ = lib.etl_dec_iceberg_partitioned_arrow(h)
+            P = lib.etl_dec_iceberg_partitions(h)
+            rows = np.frombuffer((C.c_uint64 * (P + 1)).from_address(lib.etl_dec_iceberg_partition_rows(h, 1)), dtype=np.uint64).copy()
+            sizes = []
+            for k in range(P):
+                rc, fh = pq_write(lib, pa_, fields, int(rows[k]), int(rows[k + 1]), codec, 0)
+                assert rc == 0
+                sizes.append(lib.etl_dec_parquet_size(fh))
+                lib.etl_dec_parquet_free(fh)
+            e[2].record()
+            e[2].synchronize()
+            lib.etl_dec_iceberg_partition_free(h)
+            if first is None:
+                first = sizes
+                files += P
+            assert sizes == first
+            p0, p1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            p0.record()
+            rc, fh = pq_write(lib, a, fields, 0, n, codec, 0)
+            p1.record()
+            p1.synchronize()
+            assert rc == 0
+            lib.etl_dec_parquet_free(fh)
+            if r >= warmup:
+                t_call.append(e[0].elapsed_time(e[1]))
+                t_whole.append(e[0].elapsed_time(e[2]))
+                t_plain.append(p0.elapsed_time(p1))
+        call.append(float(np.median(t_call)))
+        whole.append(float(np.median(t_whole)))
+        plain.append(float(np.median(t_plain)))
+    c, w, p = sum(call), sum(whole), sum(plain)
+    gbps = moved / (gather * 1e-3) / 1e9 if gather else None
+    return dict(spec=spec, partitions=int(parts), files=int(files), partition_call_ms=round(c, 3),
+                device_ms=dict(transform_group=round(group, 3), scans=round(scan, 3), gather=round(gather, 3)),
+                gather_bytes_moved=int(moved), gather_GBps=round(gbps, 1) if gbps else None,
+                gather_kernel_share_of_3_35TBps_pct=round(100 * gbps / 3350, 1) if gbps else None,
+                partitioned_write_ms=round(w, 3), unpartitioned_snappy_write_ms=round(p, 3),
+                ratio=round(w / p, 2) if p else None, ms_per_file=round((w - c) / files, 3) if files else None)
+
+
 def leg(lib, emits, reps, warmup):
+    if OPTS["partition"]:
+        return partition_emits(lib, emits, reps, warmup)
     if OPTS["zstd"]:
         return zstd_emits(lib, emits, reps, warmup)
     if OPTS["bloom"]:
@@ -362,12 +511,26 @@ def main():
     ap.add_argument("--c5-scale", type=float, default=0.02)
     ap.add_argument("--zstd", action="store_true")
     ap.add_argument("--c2-scale", type=float, default=0.05)
+    ap.add_argument("--partition", action="store_true")
+    ap.add_argument("--c1-scale", type=float, default=10.0)
     a = ap.parse_args()
-    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index, bloom=a.bloom, zstd=a.zstd)
+    OPTS.update(plain_only=a.plain_only, pyarrow=not a.no_pyarrow, page_index=a.page_index, bloom=a.bloom, zstd=a.zstd,
+                partition=a.partition)
     if not torch.cuda.is_available():
         raise SystemExit("parquet_measure needs a CUDA device")
     t = time.time()
     print(json.dumps(dict(card=card(), torch_device=torch.cuda.get_device_name(0))), flush=True)
+    if a.partition:
+        for name, scale, spec in (("c1", a.c1_scale, [(4, abi.ICE_DAY, 0)]), ("c2", a.c2_scale, [(0, abi.ICE_BUCKET, 16)]),
+                                  ("copy", 0, [(0, abi.ICE_BUCKET, 16), (5, abi.ICE_TRUNCATE, 1)]),
+                                  ("c5", a.c5_scale, [(0, abi.ICE_BUCKET, 16)])):
+            OPTS["spec"] = spec
+            if name == "copy":
+                copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
+            else:
+                streaming(name, scale, a.reps, a.warmup, a.tag)
+        print(json.dumps(dict(wall_s=round(time.time() - t, 1))), flush=True)
+        return
     copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
     if a.zstd:
         for name, scale in (("c2", a.c2_scale), ("c3", a.c3_scale), ("c5", a.c5_scale)):
