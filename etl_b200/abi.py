@@ -143,6 +143,8 @@ EXPORTS = [
     "etl_dec_ducklake_text", "etl_dec_ducklake_issues", "etl_dec_ducklake_sub_batches", "etl_dec_ducklake_copy_fingerprint",
     "etl_dec_ducklake_free", "etl_dec_parquet_write", "etl_dec_parquet_write_bloom", "etl_dec_parquet_size", "etl_dec_parquet_bytes", "etl_dec_parquet_metrics",
     "etl_dec_parquet_required_null", "etl_dec_parquet_free",
+    "etl_dec_parquet_write_files", "etl_dec_parquet_files_count", "etl_dec_parquet_files_offsets", "etl_dec_parquet_files_bytes",
+    "etl_dec_parquet_files_metrics", "etl_dec_parquet_files_required_null", "etl_dec_parquet_files_free",
     "etl_dec_iceberg_partition", "etl_dec_iceberg_partitions", "etl_dec_iceberg_partition_rows", "etl_dec_iceberg_partition_value",
     "etl_dec_iceberg_partitioned_arrow", "etl_dec_iceberg_partition_free",
     "etl_dec_batch_device_stream", "etl_shim_materialise", "etl_shim_event_count", "etl_shim_size_hint", "etl_shim_total_size_hint", "etl_shim_owned_bytes",
@@ -270,6 +272,18 @@ def load(build: bool = True):
     L.etl_dec_parquet_required_null.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     L.etl_dec_parquet_free.argtypes = [vp]
     L.etl_dec_parquet_free.restype = None
+    L.etl_dec_parquet_write_files.argtypes = [vp, C.POINTER(ParquetField), C.POINTER(ParquetBloom), C.c_uint32,
+                                              C.POINTER(C.c_uint64), C.c_uint64, C.c_uint32, C.c_int, C.POINTER(vp)]
+    L.etl_dec_parquet_files_count.argtypes = [vp]
+    L.etl_dec_parquet_files_count.restype = C.c_uint64
+    L.etl_dec_parquet_files_offsets.argtypes = [vp]
+    L.etl_dec_parquet_files_offsets.restype = C.c_void_p
+    L.etl_dec_parquet_files_bytes.argtypes = [vp, C.c_int]
+    L.etl_dec_parquet_files_bytes.restype = C.c_void_p
+    L.etl_dec_parquet_files_metrics.argtypes = [vp, C.c_uint64, C.c_uint32, C.POINTER(ParquetMetrics)]
+    L.etl_dec_parquet_files_required_null.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
+    L.etl_dec_parquet_files_free.argtypes = [vp]
+    L.etl_dec_parquet_files_free.restype = None
     L.etl_dec_iceberg_partition.argtypes = [vp, C.POINTER(IcebergPartitionField), C.c_uint32, C.c_uint64, C.c_uint64, C.c_int,
                                             C.POINTER(vp)]
     L.etl_dec_iceberg_partitions.argtypes = [vp]

@@ -19,9 +19,12 @@
 //     PageLocation of the OffsetIndex and the header of a list field;
 //   * the bloom filter pieces (etl_dec_parquet_write_bloom): XXH64 (seed 0) of a value's PLAIN bytes, the block and bit
 //     masks of a split-block insert, the BloomFilterHeader, and (host only) the bitset size from ndv and fpp;
-//   * (host only) the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders, for
-//     a dictionary chunk its dictionary_page_offset and encoding_stats, with a page index the ColumnChunk's offset
-//     and length of its OffsetIndex and ColumnIndex, and with a bloom filter its offset and length.
+//   * the footer: FileMetaData with the schema, row groups, column chunks, statistics and column orders, for a
+//     dictionary chunk its dictionary_page_offset and encoding_stats, with a page index the ColumnChunk's offset and
+//     length of its OffsetIndex and ColumnIndex, and with a bloom filter its offset and length.  The schema prefix is
+//     host only (the same for every file); the tail behind it (num_rows, row groups, created_by, column orders) is host
+//     and device, so that etl_dec_parquet_write_files serialises every file's tail on the device;
+//   * (host only) the row-group table of a multi-file write.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -471,109 +474,207 @@ inline void schema_element(TWriter& w, const Leaf& L, bool element) {
   w.end();
 }
 
-// FileMetaData {1 version, 2 schema, 3 num_rows, 4 row_groups, 6 created_by, 7 column_orders}; chunks row-group major
-inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::vector<uint64_t>& rg_rows,
-                                   const std::vector<Chunk>& chunks, uint32_t codec, const char* created_by) {
-  std::vector<uint8_t> buf;
-  for (int pass = 0; pass < 2; pass++) {
-    TWriter w(pass ? buf.data() : nullptr);
-    uint32_t n_elems = 1;
-    for (const Leaf& L : leaves) n_elems += L.is_list ? 3 : 1;
-    uint64_t num_rows = 0;
-    for (uint64_t r : rg_rows) num_rows += r;
-    w.i32(1, 1);
-    w.list(2, TT_STRUCT, n_elems);
-    w.list_struct_begin();
-    w.bin(4, (const uint8_t*)"schema", 6);
-    w.i32(5, (int32_t)leaves.size());
+// the footer fields of one column chunk, as the tail serialiser below reads them (the device's chunk records and the
+// host's Chunk both give one); min / max point at their statistic bytes
+struct ChunkMeta {
+  uint64_t offset, num_values, usize, csize, null_count, data_offset, data_pages, ci_offset, oi_offset, bloom_offset;
+  uint32_t ci_len, oi_len, bloom_len, min_len, max_len;
+  bool has_minmax, dict, page_index;
+  const uint8_t* min;
+  const uint8_t* max;
+};
+// what the tail needs of a leaf: its Parquet type, whether it has levels or is a list, its column name
+struct LeafMeta {
+  const uint8_t* name;
+  uint32_t name_len, ptype;
+  bool levels, is_list;
+};
+
+// FileMetaData fields 1 (version) and 2 (schema): the same for every file of one schema, serialised once on the host.
+// The writer is left where the tail continues (field 2 was the last of the top-level struct).
+inline void footer_prefix(TWriter& w, const std::vector<Leaf>& leaves) {
+  uint32_t n_elems = 1;
+  for (const Leaf& L : leaves) n_elems += L.is_list ? 3 : 1;
+  w.i32(1, 1);
+  w.list(2, TT_STRUCT, n_elems);
+  w.list_struct_begin();
+  w.bin(4, (const uint8_t*)"schema", 6);
+  w.i32(5, (int32_t)leaves.size());
+  w.end();
+  for (const Leaf& L : leaves) {
+    if (!L.is_list) { schema_element(w, L, false); continue; }
+    w.list_struct_begin();                           // <rep> group name (LIST)
+    w.i32(3, L.required ? REP_REQUIRED : REP_OPTIONAL);
+    w.bin(4, (const uint8_t*)L.name.data(), (uint32_t)L.name.size());
+    w.i32(5, 1);
+    w.i32(6, CT_LIST);
+    w.i32(9, L.field_id);
+    w.begin(10); w.begin(3); w.end(); w.end();
     w.end();
-    for (const Leaf& L : leaves) {
-      if (!L.is_list) { schema_element(w, L, false); continue; }
-      w.list_struct_begin();                           // <rep> group name (LIST)
-      w.i32(3, L.required ? REP_REQUIRED : REP_OPTIONAL);
-      w.bin(4, (const uint8_t*)L.name.data(), (uint32_t)L.name.size());
-      w.i32(5, 1);
-      w.i32(6, CT_LIST);
-      w.i32(9, L.field_id);
-      w.begin(10); w.begin(3); w.end(); w.end();
-      w.end();
-      w.list_struct_begin();                           // repeated group list
-      w.i32(3, REP_REPEATED);
-      w.bin(4, (const uint8_t*)"list", 4);
-      w.i32(5, 1);
-      w.end();
-      schema_element(w, L, true);
-    }
-    w.i64(3, (int64_t)num_rows);
-    w.list(4, TT_STRUCT, (uint32_t)rg_rows.size());
-    for (size_t g = 0; g < rg_rows.size(); g++) {
-      w.list_struct_begin();
-      uint64_t tu = 0, tc = 0;
-      for (size_t l = 0; l < leaves.size(); l++) { tu += chunks[g * leaves.size() + l].usize; tc += chunks[g * leaves.size() + l].csize; }
-      w.list(1, TT_STRUCT, (uint32_t)leaves.size());
-      for (size_t l = 0; l < leaves.size(); l++) {
-        const Leaf& L = leaves[l];
-        const Chunk& C = chunks[g * leaves.size() + l];
-        w.list_struct_begin();
-        w.i64(2, (int64_t)C.offset);
-        w.begin(3);
-        w.i32(1, (int32_t)L.ptype);
-        const bool levels = L.is_list || !L.required;
-        w.list(2, TT_I32, (levels ? 2 : 1) + (C.dict ? 1 : 0));
-        w.var(zigzag(ENC_PLAIN));
-        if (levels) w.var(zigzag(ENC_RLE));
-        if (C.dict) w.var(zigzag(ENC_RLE_DICTIONARY));
-        const std::string& leaf_name = L.name;
-        w.list(3, TT_BINARY, L.is_list ? 3 : 1);
-        w.var(leaf_name.size());
-        for (char ch : leaf_name) w.byte((uint8_t)ch);
-        if (L.is_list) { w.var(4); for (char ch : std::string("list")) w.byte((uint8_t)ch); w.var(7); for (char ch : std::string("element")) w.byte((uint8_t)ch); }
-        w.i32(4, (int32_t)(codec & 0xFFu));        // the compression codec, without the ETL_PQ_DICTIONARY bit
-        w.i64(5, (int64_t)C.num_values);
-        w.i64(6, (int64_t)C.usize);
-        w.i64(7, (int64_t)C.csize);
-        w.i64(9, (int64_t)(C.dict ? C.data_offset : C.offset));
-        if (C.dict) w.i64(11, (int64_t)C.offset);
-        w.begin(12);
-        w.i64(3, (int64_t)C.null_count);
-        if (C.has_minmax) {
-          w.bin(5, (const uint8_t*)C.max.data(), (uint32_t)C.max.size());
-          w.bin(6, (const uint8_t*)C.min.data(), (uint32_t)C.min.size());
-        }
-        w.end();
-        if (C.dict) {                                  // PageEncodingStats {page_type, encoding, count}
-          w.list(13, TT_STRUCT, 2);
-          w.list_struct_begin(); w.i32(1, PAGE_DICTIONARY); w.i32(2, ENC_PLAIN); w.i32(3, 1); w.end();
-          w.list_struct_begin(); w.i32(1, PAGE_DATA); w.i32(2, ENC_RLE_DICTIONARY); w.i32(3, (int32_t)C.data_pages); w.end();
-        }
-        if (C.bloom_len) { w.i64(14, (int64_t)C.bloom_offset); w.i32(15, (int32_t)C.bloom_len); }
-        w.end();
-        if (C.page_index) {                            // ColumnChunk offset_index_offset / _length, column_index_*
-          w.i64(4, (int64_t)C.oi_offset);
-          w.i32(5, (int32_t)C.oi_len);
-          if (C.ci_len) { w.i64(6, (int64_t)C.ci_offset); w.i32(7, (int32_t)C.ci_len); }
-        }
-        w.end();
-      }
-      w.i64(2, (int64_t)tu);
-      w.i64(3, (int64_t)rg_rows[g]);
-      w.i64(5, (int64_t)chunks[g * leaves.size()].offset);
-      w.i64(6, (int64_t)tc);
-      w.field(7, TT_I16); w.var(zigzag((int64_t)g));
-      w.end();
-    }
-    const uint32_t cb = (uint32_t)strlen(created_by);
-    w.bin(6, (const uint8_t*)created_by, cb);
-    w.list(7, TT_STRUCT, (uint32_t)leaves.size());
-    for (size_t l = 0; l < leaves.size(); l++) {       // ColumnOrder { 1: TypeDefinedOrder {} }
+    w.list_struct_begin();                           // repeated group list
+    w.i32(3, REP_REPEATED);
+    w.bin(4, (const uint8_t*)"list", 4);
+    w.i32(5, 1);
+    w.end();
+    schema_element(w, L, true);
+  }
+}
+// one ColumnChunk of a RowGroup's columns list (the writer inside that list: depth 1)
+__host__ __device__ inline void column_chunk(TWriter& w, const LeafMeta& L, const ChunkMeta& C, uint32_t codec) {
+  w.list_struct_begin();
+  w.i64(2, (int64_t)C.offset);
+  w.begin(3);
+  w.i32(1, (int32_t)L.ptype);
+  w.list(2, TT_I32, (L.levels ? 2 : 1) + (C.dict ? 1 : 0));
+  w.var(zigzag(ENC_PLAIN));
+  if (L.levels) w.var(zigzag(ENC_RLE));
+  if (C.dict) w.var(zigzag(ENC_RLE_DICTIONARY));
+  w.list(3, TT_BINARY, L.is_list ? 3 : 1);
+  w.var(L.name_len);
+  for (uint32_t k = 0; k < L.name_len; k++) w.byte(L.name[k]);
+  if (L.is_list) { w.var(4); for (const char* s = "list"; *s; s++) w.byte((uint8_t)*s); w.var(7); for (const char* s = "element"; *s; s++) w.byte((uint8_t)*s); }
+  w.i32(4, (int32_t)(codec & 0xFFu));            // the compression codec, without the ETL_PQ_DICTIONARY bit
+  w.i64(5, (int64_t)C.num_values);
+  w.i64(6, (int64_t)C.usize);
+  w.i64(7, (int64_t)C.csize);
+  w.i64(9, (int64_t)(C.dict ? C.data_offset : C.offset));
+  if (C.dict) w.i64(11, (int64_t)C.offset);
+  w.begin(12);
+  w.i64(3, (int64_t)C.null_count);
+  if (C.has_minmax) {
+    w.bin(5, C.max, C.max_len);
+    w.bin(6, C.min, C.min_len);
+  }
+  w.end();
+  if (C.dict) {                                      // PageEncodingStats {page_type, encoding, count}
+    w.list(13, TT_STRUCT, 2);
+    w.list_struct_begin(); w.i32(1, PAGE_DICTIONARY); w.i32(2, ENC_PLAIN); w.i32(3, 1); w.end();
+    w.list_struct_begin(); w.i32(1, PAGE_DATA); w.i32(2, ENC_RLE_DICTIONARY); w.i32(3, (int32_t)C.data_pages); w.end();
+  }
+  if (C.bloom_len) { w.i64(14, (int64_t)C.bloom_offset); w.i32(15, (int32_t)C.bloom_len); }
+  w.end();
+  if (C.page_index) {                                // ColumnChunk offset_index_offset / _length, column_index_*
+    w.i64(4, (int64_t)C.oi_offset);
+    w.i32(5, (int32_t)C.oi_len);
+    if (C.ci_len) { w.i64(6, (int64_t)C.ci_offset); w.i32(7, (int32_t)C.ci_len); }
+  }
+  w.end();
+}
+
+// FileMetaData fields 3 (num_rows), 4 (row_groups), 6 (created_by), 7 (column_orders) and the struct's end, the part
+// of a footer behind footer_prefix, cut into independent units: with n_rg row groups of n_leaves chunks (row group g
+// is rows [rg_start[g], rg_start[g + 1]), any origin; its chunks chunk(g * n_leaves + l)), unit 0 is num_rows and the
+// row_groups list header, unit 1 + c is chunk c's ColumnChunk (the first of a row group with the RowGroup's opening
+// and its columns list header, the last with the RowGroup's closing fields), unit n_rg * n_leaves + 1 is created_by,
+// column_orders and the end.  Each unit starts from a writer in the state the whole tail has there, so the units
+// written back to back are the tail; the device sizes and writes them a lane per unit.  Returns its bytes (out ==
+// nullptr counts).
+template <class GetChunk>
+__host__ __device__ inline uint64_t tail_unit(uint8_t* out, uint64_t u, const LeafMeta* leaves, uint32_t n_leaves, const uint64_t* rg_start,
+                                              uint32_t n_rg, GetChunk chunk, uint32_t codec, const uint8_t* created_by, uint32_t cb_len) {
+  TWriter w(out);
+  const uint64_t nc = (uint64_t)n_rg * n_leaves;
+  if (u == 0) {
+    w.last[0] = 2;                                   // behind field 2 (schema)
+    w.i64(3, (int64_t)(n_rg ? rg_start[n_rg] - rg_start[0] : 0));
+    w.list(4, TT_STRUCT, n_rg);
+    return w.n;
+  }
+  if (u == nc + 1) {
+    w.last[0] = 4;                                   // behind field 4 (row_groups)
+    w.bin(6, created_by, cb_len);
+    w.list(7, TT_STRUCT, n_leaves);
+    for (uint32_t l = 0; l < n_leaves; l++) {        // ColumnOrder { 1: TypeDefinedOrder {} }
       w.list_struct_begin();
       w.begin(1); w.end();
       w.end();
     }
     w.end();
-    if (!pass) buf.resize(w.n);
+    return w.n;
   }
+  const uint64_t c = u - 1, g = c / n_leaves;
+  const uint32_t l = (uint32_t)(c % n_leaves);
+  if (l == 0) {                                      // the RowGroup's struct and its columns list (field 1)
+    w.list_struct_begin();
+    w.list(1, TT_STRUCT, n_leaves);
+  } else {
+    w.depth = 1; w.last[1] = 1;
+  }
+  column_chunk(w, leaves[l], chunk(c), codec);
+  if (l + 1 == n_leaves) {                           // the RowGroup's totals, rows, file_offset, ordinal
+    uint64_t tu = 0, tc = 0;
+    for (uint32_t k = 0; k < n_leaves; k++) { const ChunkMeta C = chunk(g * n_leaves + k); tu += C.usize; tc += C.csize; }
+    w.i64(2, (int64_t)tu);
+    w.i64(3, (int64_t)(rg_start[g + 1] - rg_start[g]));
+    w.i64(5, (int64_t)chunk(g * n_leaves).offset);
+    w.i64(6, (int64_t)tc);
+    w.field(7, TT_I16); w.var(zigzag((int64_t)g));
+    w.end();
+  }
+  return w.n;
+}
+// the whole tail, its units in order (the host's footer; out == nullptr counts)
+template <class GetChunk>
+__host__ __device__ inline uint64_t footer_tail(uint8_t* out, const LeafMeta* leaves, uint32_t n_leaves, const uint64_t* rg_start,
+                                                uint32_t n_rg, GetChunk chunk, uint32_t codec, const uint8_t* created_by,
+                                                uint32_t cb_len) {
+  uint64_t n = 0;
+  for (uint64_t u = 0; u < (uint64_t)n_rg * n_leaves + 2; u++)
+    n += tail_unit(out ? out + n : nullptr, u, leaves, n_leaves, rg_start, n_rg, chunk, codec, created_by, cb_len);
+  return n;
+}
+
+// (host) the tail's leaves: names point into leaves
+inline std::vector<LeafMeta> leaf_meta(const std::vector<Leaf>& leaves) {
+  std::vector<LeafMeta> m(leaves.size());
+  for (size_t l = 0; l < leaves.size(); l++)
+    m[l] = LeafMeta{(const uint8_t*)leaves[l].name.data(), (uint32_t)leaves[l].name.size(), leaves[l].ptype,
+                    leaves[l].is_list || !leaves[l].required, leaves[l].is_list};
+  return m;
+}
+inline ChunkMeta chunk_meta(const Chunk& C) {
+  return ChunkMeta{C.offset, C.num_values, C.usize, C.csize, C.null_count, C.data_offset, C.data_pages, C.ci_offset, C.oi_offset,
+                   C.bloom_offset, C.ci_len, C.oi_len, C.bloom_len, (uint32_t)C.min.size(), (uint32_t)C.max.size(), C.has_minmax,
+                   C.dict, C.page_index, (const uint8_t*)C.min.data(), (const uint8_t*)C.max.data()};
+}
+
+// FileMetaData {1 version, 2 schema, 3 num_rows, 4 row_groups, 6 created_by, 7 column_orders}; chunks row-group major.
+// The schema prefix, then the tail.
+inline std::vector<uint8_t> footer(const std::vector<Leaf>& leaves, const std::vector<uint64_t>& rg_rows,
+                                   const std::vector<Chunk>& chunks, uint32_t codec, const char* created_by) {
+  TWriter pw(nullptr);
+  footer_prefix(pw, leaves);
+  std::vector<uint8_t> buf(pw.n);
+  TWriter w(buf.data());
+  footer_prefix(w, leaves);
+  std::vector<uint64_t> rg_start(rg_rows.size() + 1, 0);
+  for (size_t g = 0; g < rg_rows.size(); g++) rg_start[g + 1] = rg_start[g] + rg_rows[g];
+  const std::vector<LeafMeta> lm = leaf_meta(leaves);
+  auto get = [&](uint64_t c) { return chunk_meta(chunks[c]); };
+  const uint32_t cb = (uint32_t)strlen(created_by);
+  const uint64_t t = footer_tail(nullptr, lm.data(), (uint32_t)lm.size(), rg_start.data(), (uint32_t)rg_rows.size(), get, codec,
+                                 (const uint8_t*)created_by, cb);
+  buf.resize(w.n + t);
+  footer_tail(buf.data() + w.n, lm.data(), (uint32_t)lm.size(), rg_start.data(), (uint32_t)rg_rows.size(), get, codec,
+              (const uint8_t*)created_by, cb);
   return buf;
+}
+
+// ------------------------------------------------------------------------------------------------ files (host)
+// etl_dec_parquet_write_files: the row groups of K files, file k rows [ro[k], ro[k + 1]).  Row groups restart in every
+// file (at most kRowGroupRows rows each, an empty file has none) and are numbered across the files in order; row0 is
+// relative to ro[0], so the row groups tile [0, ro[K] - ro[0]).  first[k] is file k's first row group (first[K]: all).
+struct RowGroup { uint64_t row0, rows; uint64_t file; };
+inline std::vector<RowGroup> row_group_table(const uint64_t* ro, uint64_t K, std::vector<uint64_t>& first) {
+  std::vector<RowGroup> t;
+  first.assign(K + 1, 0);
+  for (uint64_t k = 0; k < K; k++) {
+    first[k] = t.size();
+    for (uint64_t r = ro[k]; r < ro[k + 1]; r += kRowGroupRows)
+      t.push_back(RowGroup{r - ro[0], ro[k + 1] - r < kRowGroupRows ? ro[k + 1] - r : kRowGroupRows, k});
+  }
+  first[K] = t.size();
+  return t;
 }
 
 }  // namespace etl_pq

@@ -4,6 +4,10 @@
 // encode every value again, build the levels, Snappy-compress the pages and compute the column statistics behind the
 // DataFile metrics.  The format rules are in include/etl_decode.h; the byte-level pieces are in parquet_format.cuh.
 //
+// One engine writes K files, file k the rows [ro[k], ro[k + 1]) (etl_dec_parquet_write_files; the single-file calls are
+// K = 1).  The plan runs once over [ro[0], ro[K]); the row-group table (row_group_table of parquet_format.cuh: row groups
+// restart in every file) replaces uniform cuts, so a chunk is (row group, leaf) of the whole call and each file's chunks,
+// pages and filters are contiguous ranges of the call's (FileRec).  Every offset a file holds is relative to the file.
 // Stages (one leaf per column: a flat column, or the element of a List column):
 //   1. Plan.  k_plan, a thread per (row, leaf): level entries (1, or max(1, list length)), non-null values and PLAIN
 //      value bytes (Boolean: bits) of the row, and a required column's first null row (atomicMin).  Three scans per leaf
@@ -31,26 +35,36 @@
 //      one self-contained Zstandard block (header included) in a slot of zstd_bound bytes, its work space in shared
 //      memory, its literals and sequences in scratch placed by the fragment's payload position.  k_page writes the
 //      preamble (Snappy's length varint, or the 9-byte Zstandard frame header) and the page header (its varint widths
-//      depend on the sizes) and the page's file bytes; a scan gives the file offsets; k_gather, a CTA per page, copies
-//      header + payload (+ preamble and fragments) into the file buffer, whose size is the sum of the bounds.  The
-//      dictionary slot, the page index and the bloom filters follow csize / hlen, so they need nothing per codec.
+//      depend on the sizes) and the page's file bytes; a scan gives the pages' offsets (a file's: minus its first
+//      page's); k_gather (stage 6), a CTA per page, copies header + payload (+ preamble and fragments) to its place in
+//      the output, whose size is the sum of the bounds.  The dictionary slot, the page index and the bloom filters
+//      follow csize / hlen, so they need nothing per codec.
 //   4. Statistics.  k_chunk, a thread per (leaf, row group), folds the page candidates and sizes of its chunk, k_leaf the
 //      chunks of a leaf; both write the PLAIN bytes of min / max (−0.0 / +0.0 for a zero float, none above 64 bytes).
 //   4b. Page index (ETL_PQ_PAGE_INDEX).  k_index<false>, a warp per chunk with lanes over its data pages: each page's
 //      ColumnIndex entry (null flag, bounds truncated by index_min / index_max, null count) and PageLocation sizes, the
 //      boundary order from adjacent non-null pages' untruncated bounds, the chunk's ColumnIndex / OffsetIndex lengths;
-//      one k_blk_scan over the 2 × chunks lengths places them behind 4 + data_end (read on the device);
-//      k_index<true> writes them and their offsets into the chunk records.  k_row_max (before SYNC 1) bounds an
-//      untruncated byte-array maximum by the leaf's longest row.
+//      one k_blk_scan over the 2 × chunks lengths (laid out per file: its ColumnIndexes, then its OffsetIndexes) places
+//      them; k_index_place puts each file-relative offset and length into the chunk record, behind the file's pages and
+//      filters; k_index<true> (stage 6) writes them.  k_row_max (before SYNC 1) bounds an untruncated byte-array
+//      maximum by the leaf's longest row.
 //   4c. Bloom filters (etl_dec_parquet_write_bloom).  k_chunk_nn (before SYNC 1) gives each chunk's non-null values, from
-//      which the host sizes every bitset and places the filters (row-group major) in a region behind 4 + data_end, in
-//      front of the page index.  One memset zeroes the bitsets' scratch; k_bloom, per filtered leaf and grid-stride
-//      over its items, hashes each non-null value (XXH64 of its PLAIN bytes, a byte array serially by its thread) and
-//      sets its 8 bits by atomicOr; k_bloom_write copies each header and bitset into the file.  A dictionary chunk's
-//      filter is built from its values like any other, so it equals its PLAIN form's.
-//      SYNC 2 copies the chunk and leaf records back.
-//   5. Footer, on the host from those records (parquet_format.cuh), copied behind the pages with its length and "PAR1".
-//      SYNC 3 ends the call (and the copy to pinned host memory with to_host).
+//      which the host sizes every bitset and places the filters (row-group major) in each file's region behind its
+//      pages, in front of its page index (k_chunk puts the file-relative offset into the chunk record).  One memset
+//      zeroes the bitsets' scratch; k_bloom, per filtered leaf and grid-stride over its items, hashes each non-null value
+//      (XXH64 of its PLAIN bytes, a byte array serially by its thread) and sets its 8 bits by atomicOr; k_bloom_write
+//      (stage 6) copies each header and bitset into its file.  A dictionary chunk's filter is built from its values like
+//      any other, so it equals its PLAIN form's.
+//   5. Footers, on the device: the schema prefix (the same for every file) is serialised once on the host; k_footer<false>,
+//      a warp per file, lanes over its tail's units (tail_unit of parquet_format.cuh: a ColumnChunk each), sizes the
+//      tail and the file (4 + pages + filters + index + footer + 8); a scan over the sizes places the files.
+//   6. Bytes, each written once at base[file] + its relative offset: k_gather, k_bloom_write, k_index<true>, and
+//      k_footer<true> (both magics, prefix, tail, length).  k_leaf, a thread per (file, leaf), folds the metrics.
+//      SYNC 2 copies the files' offsets and the (file, leaf) records back; SYNC 3 only with to_host (the pinned copy).
+// Per file, beside the scratch of one call over the whole range: a 72 B FileRec, 8 B of size / place and a ChunkOut
+// (248 B) per leaf; per row group 12 B of table; once the schema prefix, names and created_by.  Per page (a file has
+// at least one per leaf): a 216 B Page, 32 B of slot scans, 64 B of level scratch, a compressed slot sized by its own
+// payload (8 B + the bound of each fragment, 32 B + 7/6 of its bytes), and 48 B of header room in the output.
 // Scratch: per (row, leaf) 3 × 4 B lengths + 3 × 8 B prefix sums; per level entry 2 B (+ 64 B per page of the leaf);
 // Boolean leaves 1 bit per item (+ 4 B per page of the leaf); per page a bounded payload slot (the PLAIN value bytes + levels_bound per section) and,
 // with Snappy, a compressed slot of snappy_bound per fragment; with ETL_PQ_ZSTD, one of zstd_bound (64 KiB + 3 B) per
@@ -114,6 +128,21 @@ struct ChunkOut {
   uint8_t min[kStatMax], max[kStatMax];
   uint64_t ci_offset, oi_offset;      // ETL_PQ_PAGE_INDEX: file offsets of the chunk's ColumnIndex (ci_len 0: none) and
   uint32_t ci_len, oi_len;            // OffsetIndex
+  uint64_t bloom_offset;              // bloom filter: file offset of its header, header + bitset bytes (0: none)
+  uint32_t bloom_len, page_index;     // page_index: the call has ETL_PQ_PAGE_INDEX
+};
+// bloom filters (etl_dec_parquet_write_bloom): one record per chunk (row-group major); bytes 0: no filter
+struct BloomChunk {
+  uint64_t word;             // first u32 word of the chunk's bitset in the bloom scratch (32-byte aligned)
+  uint64_t off;              // the filter's offset (its header) among the call's filters (FileRec.bloom0: its file's first)
+  uint32_t bytes, hlen;      // bitset bytes, header bytes
+};
+// one file of the call (etl_dec_parquet_write_files; the single-file calls are one of it).  Host: its row groups, pages
+// and bloom-filter bytes as ranges of the call's (chunks row-group major, so each file's are contiguous); device: the
+// sizes of its parts.  Every offset inside a file is relative to the file.
+struct FileRec {
+  uint64_t rg0, rg1, page0, page1, bloom0, bloom1;
+  uint64_t data, index, footer;       // the pages' bytes, the page index's, the footer's (without length and magic)
 };
 constexpr uint64_t kNone = ~0ull;
 // ETL_PQ_DICTIONARY: one record per chunk (Boolean chunks have none: dict stays 0)
@@ -206,8 +235,8 @@ __global__ void __launch_bounds__(256) k_row_max(const LeafDev* leaves, uint64_t
   if ((threadIdx.x & 31) == 0 && m) atomicMax(vmax + blockIdx.y, m);
 }
 
-// 1b. a thread per (leaf, row group): greedy page cuts.  pages == nullptr: count into n_pages[chunk]
-__global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, uint64_t rb, uint64_t n, const uint64_t* E,
+// 1b. a thread per (leaf, row group; rgb: the n_rg + 1 row-group starts): greedy page cuts.  pages == nullptr: count into n_pages[chunk]
+__global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, uint64_t rb, const uint64_t* rgb, uint64_t n, const uint64_t* E,
                       const uint64_t* NN, const uint64_t* V, uint32_t* n_pages, const uint64_t* page_base, const uint64_t* leaf_page_base,
                       const uint64_t* lscr_base,
                       Page* pages, int dict) {
@@ -216,7 +245,7 @@ __global__ void k_cut(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, u
   const uint32_t g = t / n_leaves, l = t % n_leaves;
   const LeafDev L = leaves[l];
   const uint64_t* e = E + (uint64_t)l * (n + 1); const uint64_t* nv = NN + (uint64_t)l * (n + 1); const uint64_t* v = V + (uint64_t)l * (n + 1);
-  const uint64_t g0 = (uint64_t)g * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
+  const uint64_t g0 = rgb[g], g1 = rgb[g + 1];             // the row group's local rows (row_group_table)
   const bool boolean = L.atype == ETL_ARROW_BOOLEAN;
   const uint64_t thresh = boolean ? 8 * kPageBytes - 7 : kPageBytes;   // ceil(bits / 8) >= 1 MiB
   const uint32_t slot = dict && !boolean ? 1 : 0;          // the dictionary slot in front of the data pages
@@ -477,14 +506,14 @@ __global__ void __launch_bounds__(kEncThreads) k_encode(const LeafDev* leaves, P
 
 // 1c. ETL_PQ_DICTIONARY, a thread per chunk: its items, and its table sized from its non-null values (pow2 >= 2 ×
 // min(nn, kDictCap); Boolean chunks none) into tab_n, whose exclusive scan places the tables
-__global__ void k_dict_setup(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_chunks, uint64_t rb, uint64_t n, const uint64_t* NN,
+__global__ void k_dict_setup(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_chunks, uint64_t rb, const uint64_t* rgb, uint64_t n, const uint64_t* NN,
                              const uint64_t* page_base, DictChunk* D, unsigned long long* tab_n) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t > n_chunks) return;
   if (t == n_chunks) { tab_n[t] = 0; return; }
   const uint32_t g = t / n_leaves, l = t % n_leaves;
   const LeafDev L = leaves[l];
-  const uint64_t g0 = (uint64_t)g * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
+  const uint64_t g0 = rgb[g], g1 = rgb[g + 1];
   DictChunk K;
   memset(&K, 0, sizeof K);
   K.it0 = L.is_list ? (uint64_t)L.loffs[rb + g0] : rb + g0;
@@ -530,10 +559,12 @@ __device__ bool same_value(const LeafDev& L, uint64_t a, uint64_t b) {
 __device__ __forceinline__ uint64_t plain_size(const LeafDev& L, uint64_t it) {
   return is_bytes(L) ? 4 + byte_off(L, it + 1) - byte_off(L, it) : L.fixed;
 }
+// the chunk of leaf l that holds item it: the last row group whose first item is <= it (a binary search, since one call
+// can have thousands of row groups)
 __device__ __forceinline__ uint32_t chunk_of(const DictChunk* D, uint32_t l, uint32_t n_leaves, uint32_t n_rg, uint64_t it) {
-  uint32_t g = 0;
-  while (g + 1 < n_rg && it >= D[(g + 1) * n_leaves + l].it0) g++;
-  return g * n_leaves + l;
+  uint32_t lo = 0, hi = n_rg - 1;
+  while (lo < hi) { const uint32_t m = (lo + hi + 1) / 2; if (D[(uint64_t)m * n_leaves + l].it0 <= it) lo = m; else hi = m - 1; }
+  return lo * n_leaves + l;
 }
 // a slot claimed for a new entry: its PLAIN size joins the chunk's total; past kDictBytes the chunk falls back
 __device__ __forceinline__ void claimed(DictChunk& K, uint64_t sz) {
@@ -736,19 +767,29 @@ __global__ void __launch_bounds__(32) k_zstd(const Page* pages, uint32_t n_pages
                                   W, lit + u, seq + u / 4 + f);
 }
 
-// the compressed slot of one fragment (comp: the codec, ETL_PQ_SNAPPY or ETL_PQ_ZSTD)
-__host__ __device__ inline uint32_t frag_slot(uint32_t comp) {
-  return comp == ETL_PQ_ZSTD ? etl_zstd::zstd_bound(kFragment) : snappy_bound(kFragment);
+// the compressed bound of a fragment of n bytes (comp: the codec, ETL_PQ_SNAPPY or ETL_PQ_ZSTD): at most 32 + 7n / 6
+__host__ __device__ inline uint32_t frag_bound(uint32_t comp, uint32_t n) {
+  return comp == ETL_PQ_ZSTD ? etl_zstd::zstd_bound(n) : snappy_bound(n);
 }
+// the stride of the fragments in a page's compressed slot: every fragment but the last is a whole kFragment
+__host__ __device__ inline uint32_t frag_slot(uint32_t comp) { return frag_bound(comp, kFragment); }
 
 // a thread per page + 1: what the slot scans add up (0 payload bound, 1 compressed slot, 2 fragment slots); entry
-// n_pages is 0, so that the exclusive scan leaves the total there
+// n_pages is 0, so that the exclusive scan leaves the total there.  The compressed slot (after k_encode) is sized by
+// the page's payload: 8 B, whole fragments at the stride, then the bound of its last fragment, so a page of a few
+// bytes takes a few dozen, not a whole 64 KiB fragment's bound
 __global__ void k_fill(const Page* pages, uint32_t n_pages, int which, uint32_t comp, uint64_t* dst) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p > n_pages) return;
   if (p == n_pages) { dst[p] = 0; return; }
-  const uint64_t nf = pages[p].ubound ? (pages[p].ubound + kFragment - 1) / kFragment : 1;
-  dst[p] = which == 0 ? pages[p].ubound : which == 1 ? 8 + nf * frag_slot(comp) : nf;
+  const Page& P = pages[p];
+  if (which == 1) {
+    const uint64_t nu = P.usize ? (P.usize + kFragment - 1) / kFragment : 1;
+    dst[p] = 8 + (nu - 1) * frag_slot(comp) + frag_bound(comp, (uint32_t)(P.usize - (nu - 1) * kFragment));
+    return;
+  }
+  const uint64_t nf = P.ubound ? (P.ubound + kFragment - 1) / kFragment : 1;
+  dst[p] = which == 0 ? P.ubound : nf;
 }
 
 // a thread per page: compressed size, preamble, header, file bytes of the page (comp: the codec; D: ETL_PQ_DICTIONARY;
@@ -771,14 +812,17 @@ __global__ void k_page(Page* pages, uint32_t n_pages, uint32_t comp, const uint6
   fbytes[p] = P.hlen + P.csize;
 }
 
-// a CTA per page: header, preamble and payload (or its fragments) at the page's file offset
+// a CTA per page: header, preamble and payload (or its fragments) at the page's place in its file (base: the files'
+// places in the output; rgf: the file of each row group)
 __global__ void __launch_bounds__(256) k_gather(const Page* pages, uint32_t comp, const uint64_t* foff, const uint8_t* uslot_base,
                                                 const uint64_t* uslot, const uint8_t* cslot_base, const uint64_t* cslot,
-                                                const uint64_t* fbase, const uint32_t* fsize, uint8_t* file) {
+                                                const uint64_t* fbase, const uint32_t* fsize, uint32_t n_leaves, const uint32_t* rgf,
+                                                const FileRec* files, const uint64_t* base, uint8_t* out) {
   const uint32_t p = blockIdx.x;
   const Page& P = pages[p];
   if (!P.hlen) return;                                   // a dictionary slot without a dictionary has no bytes (k_zstd
-  uint8_t* dst = file + 4 + foff[p];                     // still wrote an empty block for it)
+  const uint32_t f = rgf[P.chunk / n_leaves];            // still wrote an empty block for it)
+  uint8_t* dst = out + base[f] + 4 + foff[p] - foff[files[f].page0];
   for (uint32_t k = threadIdx.x; k < P.hlen; k += blockDim.x) dst[k] = P.hdr[k];
   dst += P.hlen;
   if (comp == ETL_PQ_UNCOMPRESSED) {
@@ -821,18 +865,27 @@ __device__ void write_stats(const LeafDev& L, uint64_t mn, uint64_t mx, ChunkOut
   else C.min_len = C.max_len = 0;
 }
 
-// 4. a thread per chunk (row-group major): sizes, counts, statistics of its pages
-__global__ void k_chunk(const LeafDev* leaves, const Page* pages, const uint64_t* page_base, uint32_t n_chunks, const uint64_t* foff,
+// 4. a thread per chunk (row-group major): sizes, counts, statistics of its pages; its offsets relative to its file (the
+// bloom filter's: the file's filters follow its pages, B nullable)
+__global__ void k_chunk(const LeafDev* leaves, const Page* pages, const uint64_t* page_base, uint32_t n_chunks, uint32_t n_leaves,
+                        const uint64_t* foff, const uint32_t* rgf, const FileRec* files, const BloomChunk* B, uint32_t pidx,
                         ChunkOut* out, const DictChunk* D) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= n_chunks) return;
   const Page& P0 = pages[page_base[c]];
   const LeafDev L = leaves[P0.leaf];
+  const FileRec& F = files[rgf[c / n_leaves]];
+  const uint64_t f0 = foff[F.page0];                    // the file's first page
   ChunkOut C{};
-  C.offset = 4 + foff[page_base[c]];
+  C.offset = 4 + foff[page_base[c]] - f0;
   const uint64_t p0 = page_base[c] + P0.kind;          // the first data page
-  C.data_offset = 4 + foff[p0]; C.data_pages = page_base[c + 1] - p0;
+  C.data_offset = 4 + foff[p0] - f0; C.data_pages = page_base[c + 1] - p0;
   C.dict = D ? D[c].dict : 0;
+  C.page_index = pidx;
+  if (B && B[c].bytes) {
+    C.bloom_offset = 4 + (foff[F.page1] - f0) + B[c].off - F.bloom0;
+    C.bloom_len = B[c].hlen + B[c].bytes;
+  }
   uint64_t mn = kNone, mx = kNone;
   for (uint64_t p = page_base[c]; p < page_base[c + 1]; p++) {
     const Page& P = pages[p];
@@ -846,23 +899,25 @@ __global__ void k_chunk(const LeafDev* leaves, const Page* pages, const uint64_t
   reinterpret_cast<uint64_t*>(out + n_chunks)[2 * c] = mn;
   reinterpret_cast<uint64_t*>(out + n_chunks)[2 * c + 1] = mx;
 }
-// a thread per leaf: the file's statistics over its chunks
-__global__ void k_leaf(const LeafDev* leaves, uint32_t n_leaves, uint32_t n_rg, ChunkOut* chunks, ChunkOut* out) {
-  const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
-  if (l >= n_leaves) return;
+// a thread per (file, leaf): the file's statistics of the leaf over its chunks, into out[file * n_leaves + leaf]
+__global__ void k_leaf(const LeafDev* leaves, uint32_t n_leaves, uint64_t n_files, uint32_t n_chunks, const FileRec* files,
+                       ChunkOut* chunks, ChunkOut* out) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_files * n_leaves) return;
+  const uint32_t l = (uint32_t)(t % n_leaves);
+  const FileRec& F = files[t / n_leaves];
   const LeafDev L = leaves[l];
-  const uint32_t n_chunks = n_leaves * n_rg;
   const uint64_t* cand = reinterpret_cast<const uint64_t*>(chunks + n_chunks);
   ChunkOut C{};
   uint64_t mn = kNone, mx = kNone;
-  for (uint32_t g = 0; g < n_rg; g++) {
+  for (uint64_t g = F.rg0; g < F.rg1; g++) {
     const ChunkOut& K = chunks[g * n_leaves + l];
     C.num_values += K.num_values; C.null_count += K.null_count; C.nan_count += K.nan_count;
     C.usize += K.usize; C.csize += K.csize;
     fold(L, cand[2 * (g * n_leaves + l)], cand[2 * (g * n_leaves + l) + 1], mn, mx);
   }
   write_stats(L, mn, mx, C);
-  out[l] = C;
+  out[t] = C;
 }
 
 // ETL_PQ_PAGE_INDEX: the ColumnIndex bound of present, non-NaN item it: its statistic bytes, a byte array's truncated
@@ -895,14 +950,14 @@ constexpr uint32_t kIdxWarps = 4;
 // 4b. ETL_PQ_PAGE_INDEX, a warp per chunk (row-group major), lanes over its data pages (the dictionary page is not
 // listed).  kWrite false: each page's entry sizes, the boundary order (each non-null page against the previous one, on
 // the untruncated bounds) and the lengths of the chunk's ColumnIndex (lens[c], 0 when it has none) and OffsetIndex
-// (lens[n_chunks + c]); lens[2 n_chunks] = 0, so that their exclusive scan places them behind the pages.  kWrite true:
-// both structures at 4 + data_end + skip (the bloom filters' bytes) + lens[...], and their offsets and lengths into
-// the chunk's record.
+// (lens[c1 + c]), where the chunk's file has chunks [c0, c1): a file's ColumnIndexes, then its OffsetIndexes, files in
+// order; lens[2 n_chunks] = 0, so that their exclusive scan places every file's index as one run (k_index_place).
+// kWrite true: both structures at the offsets k_index_place put into the chunk's record, in its file at base.
 template <bool kWrite>
-__global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves, const Page* pages, const uint64_t* page_base,
-                                                         uint32_t n_chunks, uint32_t n_leaves, const uint64_t* foff, IndexChunk* X,
-                                                         unsigned long long* lens, const unsigned long long* data_end,
-                                                         uint64_t skip, uint8_t* file, ChunkOut* out) {
+__global__ void __maxnreg__(96) k_index(const LeafDev* leaves, const Page* pages, const uint64_t* page_base,
+                                                         uint32_t n_chunks, uint32_t n_leaves, const uint64_t* rgb, const uint32_t* rgf,
+                                                         const FileRec* files, const uint64_t* base, const uint64_t* foff,
+                                                         IndexChunk* X, unsigned long long* lens, uint8_t* out_file, ChunkOut* out) {
   const uint32_t c = blockIdx.x * kIdxWarps + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (c >= n_chunks) {
@@ -912,7 +967,8 @@ __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves,
   const uint64_t pb = page_base[c];
   const LeafDev L = leaves[pages[pb].leaf];
   const uint64_t p0 = pb + pages[pb].kind, k = page_base[c + 1] - p0;
-  const uint64_t g0 = (uint64_t)(c / n_leaves) * kRowGroupRows;
+  const uint32_t f = rgf[c / n_leaves];
+  const uint64_t g0 = rgb[c / n_leaves], f0 = foff[files[f].page0];
   const uint32_t lk = list_field(nullptr, TT_BINARY, (uint32_t)k);   // a list field's header
   IndexChunk I{};
   uint8_t* ci = nullptr;
@@ -920,16 +976,11 @@ __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves,
   uint64_t o_min = 0, o_max = 0, o_nc = 0;                // kWrite: where the sections' entries start
   if (kWrite) {
     I = X[c];
-    const uint64_t base = 4 + *data_end + skip;           // behind the bloom filters; lens: the exclusive scan
-    ci = file + base + lens[c];
-    oi = file + base + lens[n_chunks + c];
+    const ChunkOut& C = out[c];
+    ci = out_file + base[f] + C.ci_offset;
+    oi = out_file + base[f] + C.oi_offset;
     o_min = lk + k + lk; o_max = o_min + I.s_min + lk; o_nc = o_max + I.s_max + 2 + lk;
     if (lane == 0) {
-      ChunkOut& C = out[c];
-      C.ci_len = I.has_ci ? (uint32_t)(o_nc + I.s_nc + 1) : 0;
-      C.ci_offset = I.has_ci ? base + lens[c] : 0;
-      C.oi_offset = base + lens[n_chunks + c];
-      C.oi_len = (uint32_t)(lk + I.s_loc + 1);
       if (I.has_ci) {
         list_field(ci, TT_TRUE, (uint32_t)k);             // null_pages: list<bool>, one byte per element
         list_field(ci + lk + k, TT_BINARY, (uint32_t)k);  // min_values
@@ -965,7 +1016,7 @@ __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves,
     const uint64_t mnl = bounded ? index_bound(L, P.min_it, false, nullptr) : 0;
     const uint64_t mxl = bounded ? index_bound(L, P.max_it, true, nullptr) : 0;
     const uint64_t nc = in ? (P.e1 - P.e0) - P.nn : 0;
-    const uint64_t off = 4 + foff[p], first = P.row0 - g0;
+    const uint64_t off = 4 + foff[p] - f0, first = P.row0 - g0;
     const uint32_t fsz = (uint32_t)(foff[p + 1] - foff[p]);
     uint64_t t_min, t_max, t_nc, t_loc;
     const uint64_t x_min = warp_excl(in ? varint(mnl, nullptr) + mnl : 0, &t_min);
@@ -994,23 +1045,34 @@ __global__ void __launch_bounds__(32 * kIdxWarps) k_index(const LeafDev* leaves,
     I.order = asc ? 1 : desc ? 2 : 0;                       // ASCENDING, DESCENDING, UNORDERED
     I.has_ci = !nan_only;
     X[c] = I;
-    lens[c] = I.has_ci ? (lk + k) + (lk + s_min) + (lk + s_max) + 2 + (lk + s_nc) + 1 : 0;
-    lens[n_chunks + c] = lk + s_loc + 1;
+    const FileRec& F = files[f];
+    lens[F.rg0 * n_leaves + c] = I.has_ci ? (lk + k) + (lk + s_min) + (lk + s_max) + 2 + (lk + s_nc) + 1 : 0;
+    lens[F.rg1 * n_leaves + c] = lk + s_loc + 1;
   }
 }
+// ETL_PQ_PAGE_INDEX, a thread per chunk, after the scan of k_index<false>'s lengths: the offsets and lengths of the
+// chunk's ColumnIndex and OffsetIndex in its file, whose index follows its pages and bloom filters
+__global__ void k_index_place(uint32_t n_chunks, uint32_t n_leaves, const uint32_t* rgf, const FileRec* files, const uint64_t* foff,
+                              const IndexChunk* X, const unsigned long long* lens, ChunkOut* out) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  const FileRec& F = files[rgf[c / n_leaves]];
+  const uint64_t c0 = F.rg0 * n_leaves, c1 = F.rg1 * n_leaves;
+  const uint64_t at = 4 + foff[F.page1] - foff[F.page0] + (F.bloom1 - F.bloom0) - lens[2 * c0];
+  ChunkOut& C = out[c];
+  const bool has_ci = X[c].has_ci;
+  C.ci_len = has_ci ? (uint32_t)(lens[c0 + c + 1] - lens[c0 + c]) : 0;
+  C.ci_offset = has_ci ? at + lens[c0 + c] : 0;
+  C.oi_offset = at + lens[c1 + c];
+  C.oi_len = (uint32_t)(lens[c1 + c + 1] - lens[c1 + c]);
+}
 
-// bloom filters (etl_dec_parquet_write_bloom): one record per chunk (row-group major); bytes 0: no filter
-struct BloomChunk {
-  uint64_t word;             // first u32 word of the chunk's bitset in the bloom scratch (32-byte aligned)
-  uint64_t off;              // the filter's offset (its header) in the bloom region behind 4 + data_end
-  uint32_t bytes, hlen;      // bitset bytes, header bytes
-};
 // a thread per chunk: the non-null values of the chunk (NN prefix sums at its row-group bounds), which size its bitset
-__global__ void k_chunk_nn(uint32_t n_leaves, uint32_t n_chunks, uint64_t n, const uint64_t* NN, unsigned long long* cnn) {
+__global__ void k_chunk_nn(uint32_t n_leaves, uint32_t n_chunks, uint64_t n, const uint64_t* rgb, const uint64_t* NN, unsigned long long* cnn) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= n_chunks) return;
   const uint64_t* nv = NN + (uint64_t)(c % n_leaves) * (n + 1);
-  const uint64_t g0 = (uint64_t)(c / n_leaves) * kRowGroupRows, g1 = min(n, g0 + kRowGroupRows);
+  const uint64_t g0 = rgb[c / n_leaves], g1 = rgb[c / n_leaves + 1];
   cnn[c] = nv[g1] - nv[g0];
 }
 // XXH64 of present item it's PLAIN bytes (byte arrays without the length prefix, hashed serially by this thread)
@@ -1023,21 +1085,21 @@ __device__ __forceinline__ uint64_t item_hash(const LeafDev& L, uint64_t it) {
   }
 }
 // the first item of row group g of a leaf (g == n_rg: the end of its items)
-__device__ __forceinline__ uint64_t group_item(const LeafDev& L, uint64_t rb, uint64_t n, uint32_t g) {
-  const uint64_t r = rb + min(n, (uint64_t)g * kRowGroupRows);
+__device__ __forceinline__ uint64_t group_item(const LeafDev& L, uint64_t rb, const uint64_t* rgb, uint32_t g) {
+  const uint64_t r = rb + rgb[g];
   return L.is_list ? (uint64_t)L.loffs[r] : r;
 }
 // 4c. bloom filters, one filtered leaf, grid-stride over its items: each non-null item's hash sets 8 bits of one block
 // of its chunk's bitset (atomicOr into the zeroed scratch; the bits are a set, so any order gives the same bitset)
 __global__ void __launch_bounds__(kInsThreads) k_bloom(const LeafDev* leaves, uint32_t l, uint32_t n_leaves, uint32_t n_rg,
-                                                       uint64_t rb, uint64_t n, const BloomChunk* B, uint32_t* words) {
+                                                       uint64_t rb, const uint64_t* rgb, const BloomChunk* B, uint32_t* words) {
   const LeafDev L = leaves[l];
-  const uint64_t i0 = group_item(L, rb, n, 0), i1 = group_item(L, rb, n, n_rg);
+  const uint64_t i0 = group_item(L, rb, rgb, 0), i1 = group_item(L, rb, rgb, n_rg);
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t it = i0 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; it < i1; it += stride) {
     if (!bit(L.valid, it)) continue;
-    uint32_t g = 0;
-    while (g + 1 < n_rg && it >= group_item(L, rb, n, g + 1)) g++;
+    uint32_t g = 0, hi = n_rg - 1;                       // the last row group whose first item is <= it
+    while (g < hi) { const uint32_t m = (g + hi + 1) / 2; if (group_item(L, rb, rgb, m) <= it) g = m; else hi = m - 1; }
     const BloomChunk K = B[g * n_leaves + l];
     const uint64_t h = item_hash(L, it);
     uint32_t* w = words + K.word + 8ull * bloom_block(h, K.bytes / 32);
@@ -1045,16 +1107,81 @@ __global__ void __launch_bounds__(kInsThreads) k_bloom(const LeafDev* leaves, ui
     for (int i = 0; i < 8; i++) atomicOr(w + i, bloom_mask(h, i));
   }
 }
-// 4d. CTAs (chunk, slice): the chunk's header and bitset at 4 + data_end + its offset (ETL_PQ_PAGE_INDEX comes after)
-__global__ void __launch_bounds__(256) k_bloom_write(const BloomChunk* B, const uint32_t* words, const unsigned long long* data_end,
-                                                     uint8_t* file) {
+// 4d. CTAs (chunk, slice): the chunk's header and bitset in its file, behind the file's pages (ETL_PQ_PAGE_INDEX comes
+// after), at the offset k_chunk put into its record
+__global__ void __launch_bounds__(256) k_bloom_write(const BloomChunk* B, const uint32_t* words, uint32_t n_leaves, const uint32_t* rgf,
+                                                     const uint64_t* base, const ChunkOut* chunks, uint8_t* out) {
   const BloomChunk K = B[blockIdx.x];
   if (!K.bytes) return;
-  uint8_t* dst = file + 4 + *data_end + K.off;
+  uint8_t* dst = out + base[rgf[blockIdx.x / n_leaves]] + chunks[blockIdx.x].bloom_offset;
   if (blockIdx.y == 0 && threadIdx.x == 0) bloom_header(dst, K.bytes);
   const uint8_t* src = (const uint8_t*)(words + K.word);
   dst += K.hlen;
   for (uint64_t k = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; k < K.bytes; k += (uint64_t)gridDim.y * blockDim.x) dst[k] = src[k];
+}
+
+// 5. footers, a warp per file, its lanes over the footer's units (tail_unit of parquet_format.cuh: a ColumnChunk each,
+// so a file of many row groups or leaves is written by the whole warp).  The schema prefix (the same for every file) is
+// serialised once on the host.  kWrite false: the footer's length and the file's size (4 + pages + filters + index +
+// footer + 8) into size[f], whose exclusive scan places the files (size[K] = 0); kWrite true: both magics, the prefix,
+// the units at their scanned places, and the footer's length, at the file's place.
+struct FooterArgs {
+  const LeafMeta* leaves;
+  const uint8_t* prefix;
+  const uint8_t* created_by;
+  uint32_t n_leaves, prefix_len, cb_len, codec;
+};
+__device__ __forceinline__ ChunkMeta out_meta(const ChunkOut& K) {
+  return ChunkMeta{K.offset, K.num_values, K.usize, K.csize, K.null_count, K.data_offset, K.data_pages, K.ci_offset, K.oi_offset,
+                   K.bloom_offset, K.ci_len, K.oi_len, K.bloom_len, K.min_len, K.max_len, K.has != 0, K.dict != 0,
+                   K.page_index != 0, K.min, K.max};
+}
+constexpr uint32_t kFootWarps = 4;
+template <bool kWrite>
+__global__ void __maxnreg__(96) k_footer(FooterArgs A, uint64_t n_files, const uint64_t* rgb, FileRec* files,
+                                                           const uint64_t* foff, const unsigned long long* lens,
+                                                           const ChunkOut* chunks, uint64_t* size, uint8_t* out) {
+  const uint64_t f = (uint64_t)blockIdx.x * kFootWarps + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (f > n_files) return;
+  if (f == n_files) { if (!kWrite && lane == 0) size[f] = 0; return; }
+  FileRec& F = files[f];
+  const ChunkOut* C = chunks + F.rg0 * A.n_leaves;
+  auto get = [&](uint64_t c) { return out_meta(C[c]); };
+  const uint32_t n_rg = (uint32_t)(F.rg1 - F.rg0);
+  const uint64_t n_units = (uint64_t)n_rg * A.n_leaves + 2;
+  if (!kWrite) {
+    uint64_t t = 0;
+    for (uint64_t u = lane; u < n_units; u += 32)
+      t += tail_unit(nullptr, u, A.leaves, A.n_leaves, rgb + F.rg0, n_rg, get, A.codec, A.created_by, A.cb_len);
+    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
+    if (lane == 0) {
+      F.data = foff[F.page1] - foff[F.page0];
+      F.index = lens ? lens[2 * F.rg1 * A.n_leaves] - lens[2 * F.rg0 * A.n_leaves] : 0;
+      F.footer = A.prefix_len + t;
+      size[f] = 4 + F.data + (F.bloom1 - F.bloom0) + F.index + F.footer + 8;
+    }
+    return;
+  }
+  uint8_t* o = out + size[f];                             // the scan: the file's place
+  const uint8_t magic[4] = {'P', 'A', 'R', '1'};
+  uint8_t* t = o + 4 + F.data + (F.bloom1 - F.bloom0) + F.index;
+  for (uint32_t k = lane; k < A.prefix_len; k += 32) t[k] = A.prefix[k];
+  uint64_t at = A.prefix_len;
+  for (uint64_t u0 = 0; u0 < n_units; u0 += 32) {
+    const uint64_t u = u0 + lane;
+    const uint64_t n = u < n_units ? tail_unit(nullptr, u, A.leaves, A.n_leaves, rgb + F.rg0, n_rg, get, A.codec, A.created_by, A.cb_len) : 0;
+    uint64_t tile;
+    const uint64_t x = warp_excl(n, &tile);
+    if (u < n_units) tail_unit(t + at + x, u, A.leaves, A.n_leaves, rgb + F.rg0, n_rg, get, A.codec, A.created_by, A.cb_len);
+    at += tile;
+  }
+  if (lane == 0) {
+    for (int k = 0; k < 4; k++) o[k] = magic[k];
+    uint8_t* e = t + F.footer;
+    for (int k = 0; k < 4; k++) e[k] = (uint8_t)(F.footer >> (8 * k));
+    for (int k = 0; k < 4; k++) e[4 + k] = magic[k];
+  }
 }
 
 uint32_t parquet_type(uint32_t at) {
@@ -1084,27 +1211,38 @@ struct etl_parquet_file {
   uint8_t* host = nullptr;
   uint64_t size = 0;
   std::vector<etl_parquet_metrics> metrics;
-  std::vector<std::string> stats;                   // min / max bytes of the metrics
+  std::vector<uint8_t> stats;                       // min / max bytes of the metrics
+  uint32_t null_column = UINT32_MAX;
+  uint64_t null_row = UINT64_MAX;
+};
+struct etl_parquet_files {
+  uint8_t* dev = nullptr;
+  uint8_t* host = nullptr;
+  uint64_t n_files = 0;
+  uint32_t n_leaves = 0;
+  std::vector<uint64_t> offs;                       // n_files + 1 byte offsets of the files in dev / host
+  std::vector<etl_parquet_metrics> metrics;         // file-major, n_leaves per file (none after a required null)
+  std::vector<uint8_t> stats;                       // min / max bytes of the metrics
   uint32_t null_column = UINT32_MAX;
   uint64_t null_row = UINT64_MAX;
 };
 
-extern "C" {
+namespace {
 
-int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fields, uint32_t n_fields, uint64_t row_begin,
-                          uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out) {
-  return etl_dec_parquet_write_bloom(a, fields, nullptr, n_fields, row_begin, row_end, codec, to_host, out);
-}
-
-int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom,
-                                uint32_t n_fields, uint64_t row_begin, uint64_t row_end, uint32_t codec, int to_host,
-                                etl_parquet_file** out) {
+// The writer: files k < K, file k the rows [ro[k], ro[k + 1]) of the emit, in one device buffer (and with to_host one
+// pinned image), packed in order.  etl_dec_parquet_write(_bloom) is K = 1.  Fs is filled on ETL_OK; on an error
+// everything the call allocated is freed (Fs owns nothing yet).
+int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom, uint32_t n_fields,
+                const uint64_t* ro, uint64_t K, uint32_t codec, int to_host, etl_parquet_files* Fs) {
   // a file needs at least one column (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS has none)
-  if (!a || !out || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
+  if (!a || !ro || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
   const uint32_t cc = codec & 0xFFu;                  // the compression codec; the flag bits are ETL_PQ_DICTIONARY and
-  if (row_begin > row_end || row_end > etl_dec_arrow_rows(a) ||   // ETL_PQ_PAGE_INDEX
-      (codec & ~(0xFFu | ETL_PQ_DICTIONARY | ETL_PQ_PAGE_INDEX)) || (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY && cc != ETL_PQ_ZSTD))
+  if ((codec & ~(0xFFu | ETL_PQ_DICTIONARY | ETL_PQ_PAGE_INDEX)) ||   // ETL_PQ_PAGE_INDEX
+      (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY && cc != ETL_PQ_ZSTD))
     return ETL_ERR_INVALID_ARG;
+  if (K >= UINT32_MAX) return ETL_ERR_INVALID_ARG;
+  for (uint64_t k = 0; k < K; k++) if (ro[k + 1] < ro[k]) return ETL_ERR_INVALID_ARG;
+  if (ro[K] > etl_dec_arrow_rows(a)) return ETL_ERR_INVALID_ARG;
   const int dict = (codec & ETL_PQ_DICTIONARY) != 0;
   const int pidx = (codec & ETL_PQ_PAGE_INDEX) != 0;
   std::vector<LeafDev> hl(n_fields);
@@ -1157,20 +1295,32 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
       default: break;
     }
   }
-  const uint64_t n = row_end - row_begin;
   const uint32_t nL = n_fields;
-  const uint32_t n_rg = (uint32_t)((n + kRowGroupRows - 1) / kRowGroupRows);
+  // the row-group table: row groups restart in every file; chunk indices are 32-bit, and the page index's length scan
+  // runs over 2 × chunks + 1 entries in 32 bits, so at most 2^31 - 1 chunks
+  std::vector<uint64_t> frg;
+  const std::vector<RowGroup> rgt = row_group_table(ro, K, frg);
+  if ((uint64_t)rgt.size() * nL >= (1ull << 31)) return ETL_ERR_INVALID_ARG;
+  Fs->n_files = K; Fs->n_leaves = nL;
+  Fs->offs.assign(K + 1, 0);
+  if (!K) return ETL_OK;
+  const uint64_t row_begin = ro[0], n = ro[K] - ro[0];
+  const uint32_t n_rg = (uint32_t)rgt.size();
   const uint32_t n_chunks = n_rg * nL;
+  std::vector<uint64_t> rgb(n_rg + 1, n);             // row-group starts (local rows), then n
+  std::vector<uint32_t> rgf(n_rg + 1, 0);             // the file of each row group
+  for (uint32_t g = 0; g < n_rg; g++) { rgb[g] = rgt[g].row0; rgf[g] = (uint32_t)rgt[g].file; }
   const int snappy = cc != ETL_PQ_UNCOMPRESSED;        // Snappy or Zstandard: compressed fragments
   const int zstd = cc == ETL_PQ_ZSTD;
   auto bloomed = [&](uint32_t l) { return bloom && bloom[l].fpp > 0.0; };
   bool any_bloom = false;
   for (uint32_t l = 0; l < nL; l++) any_bloom |= bloomed(l);
   cudaStream_t st = cudaStreamPerThread;
-  etl_parquet_file* Fo = new etl_parquet_file();
+  uint8_t* dev = nullptr;
+  uint8_t* host = nullptr;
   std::vector<void*> pool;
   auto dalloc = [&](uint64_t bytes) -> void* { void* p = nullptr; if (cudaMalloc(&p, bytes + 64) != cudaSuccess) return nullptr; pool.push_back(p); return p; };
-  auto fail = [&](int rc) { cudaGetLastError(); for (void* p : pool) cudaFree(p); if (Fo->dev) cudaFree(Fo->dev); if (Fo->host) cudaFreeHost(Fo->host); delete Fo; return rc; };
+  auto fail = [&](int rc) { cudaGetLastError(); for (void* p : pool) cudaFree(p); if (dev) cudaFree(dev); if (host) cudaFreeHost(host); return rc; };
 #define CK(call) do { if ((call) != cudaSuccess) return fail(ETL_ERR_CUDA); } while (0)
   // 1. plan
   LeafDev* d_leaves = (LeafDev*)dalloc(sizeof(LeafDev) * (nL + 1));
@@ -1183,8 +1333,12 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull + 4ull * nL);   // | ETL_PQ_PAGE_INDEX: k_row_max
   uint32_t* d_np = (uint32_t*)dalloc(n_chunks * 4ull);
   unsigned long long* d_cnn = any_bloom ? (unsigned long long*)dalloc(n_chunks * 8ull) : nullptr;   // bloom: per chunk
-  if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np || (any_bloom && !d_cnn)) return fail(ETL_ERR_ALLOC);
+  uint64_t* d_rgb = (uint64_t*)dalloc(8ull * (n_rg + 1) + 4ull * (n_rg + 1));        // row-group starts | files
+  if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np || (any_bloom && !d_cnn) || !d_rgb) return fail(ETL_ERR_ALLOC);
+  uint32_t* d_rgf = (uint32_t*)(d_rgb + n_rg + 1);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_rgb, rgb.data(), 8ull * (n_rg + 1), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_rgf, rgf.data(), 4ull * (n_rg + 1), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_req, 0xff, nL * 8ull, st));
   unsigned int* d_vmax = (unsigned int*)(d_req + nL);
   if (pidx) CK(cudaMemsetAsync(d_vmax, 0, 4ull * nL, st));
@@ -1200,9 +1354,9 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
         uint32_t* lens = d_len + s * nr1 + (uint64_t)l * (n + 1);
         scan_lengths(lens, n, d_blk + at * (lb + 1), d_tot + at, d_pre + s * nr1 + (uint64_t)l * (n + 1), st);
       }
-    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, d_rgb, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
     if (pidx) k_row_max<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, n, vb, d_vmax);
-    if (any_bloom) k_chunk_nn<<<(n_chunks + 255) / 256, 256, 0, st>>>(nL, n_chunks, n, NN, d_cnn);
+    if (any_bloom) k_chunk_nn<<<(n_chunks + 255) / 256, 256, 0, st>>>(nL, n_chunks, n, d_rgb, NN, d_cnn);
   }
   // SYNC 1: page counts, totals, required-column nulls (bloom filters: the chunks' non-null values)
   std::vector<uint32_t> np(n_chunks);
@@ -1219,9 +1373,8 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   CK(cudaStreamSynchronize(st));
   for (uint32_t l = 0; l < nL; l++)
     if (req[l] != kNone) {                            // RecordBatch::try_new fails before anything is written
-      Fo->null_column = l; Fo->null_row = req[l];
+      Fs->null_column = l; Fs->null_row = req[l];
       for (void* p : pool) cudaFree(p);
-      *out = Fo;
       return ETL_OK;
     }
   // ETL_PQ_DICTIONARY: every chunk of a non-Boolean leaf has a dictionary slot in front of its data pages
@@ -1256,7 +1409,9 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
   std::vector<uint64_t> leaf_page_base(n_chunks + 1, 0);   // pages of the chunk's leaf in the row groups before it
   for (uint32_t c = nL; c < n_chunks; c++) leaf_page_base[c] = leaf_page_base[c - nL] + np[c - nL];
   const uint64_t n_frag_bound = snappy ? U / kFragment + P + 1 : 0;
-  const uint64_t C_bound = snappy ? 8 * P + n_frag_bound * frag_slot(cc) : 0;
+  // compressed slots: 8 B per page and each fragment's bound (affine in its bytes: 32 + 7 n / 6 at most), the
+  // fragments' bytes adding up to at most U
+  const uint64_t C_bound = snappy ? 8 * P + 32 * n_frag_bound + U + U / 6 : 0;
   // bit scratch: page lp of a Boolean leaf starts at word bscr + it0 / 32 + lp
   uint64_t bool_words = 0;
   for (uint32_t l = 0; l < nL; l++)
@@ -1266,35 +1421,52 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
       hl[l].bscr = bool_words;
       bool_words += ne / 32 + pages_of[l] + 2;
     }
-  // footer bound: every size at its widest varint, every statistic at its longest
-  std::vector<uint64_t> rg_rows(n_rg);
-  for (uint32_t g = 0; g < n_rg; g++) rg_rows[g] = std::min<uint64_t>(kRowGroupRows, n - (uint64_t)g * kRowGroupRows);
-  std::vector<Chunk> wide(n_chunks);
-  for (uint32_t c = 0; c < n_chunks; c++) {
-    Chunk& k = wide[c];
-    k.offset = k.num_values = k.usize = k.csize = k.null_count = 1ull << 62; k.has_minmax = true; k.min.assign(kStatMax, 'x'); k.max.assign(kStatMax, 'x');
-    if (has_dict(c % nL)) { k.dict = true; k.data_offset = 1ull << 62; k.data_pages = INT32_MAX; }
-    if (pidx) { k.page_index = true; k.ci_offset = k.oi_offset = 1ull << 62; k.ci_len = k.oi_len = INT32_MAX; }
-  }
-  // bloom filters: each filtered chunk's bitset size from its ndv (or non-null count), its header, its place in the
-  // region behind the pages (row-group major, column minor) and its bitset's place in the zeroed scratch
+  // bloom filters: each filtered chunk's bitset size from its ndv (or non-null count), its header, its place among the
+  // call's filters (row-group major, column minor: each file's run follows its pages) and its bitset's place in the
+  // zeroed scratch
   std::vector<BloomChunk> hb(n_chunks, BloomChunk{0, 0, 0, 0});
+  std::vector<uint64_t> bloom_at(n_chunks + 1, 0);
   uint64_t bloom_total = 0, bloom_words = 0;
   for (uint32_t c = 0; c < n_chunks; c++) {
     const uint32_t l = c % nL;
+    bloom_at[c] = bloom_total;
     if (!bloomed(l)) continue;
     const etl_parquet_bloom& Bf = bloom[l];
     const uint64_t ndv = Bf.ndv ? Bf.ndv : std::max<uint64_t>(1, cnn[c]);
-    BloomChunk& K = hb[c];
-    K.bytes = (uint32_t)bloom_bytes(ndv, Bf.fpp, Bf.max_bytes ? Bf.max_bytes : kBloomDefaultBytes);
-    K.hlen = bloom_header(nullptr, K.bytes);
-    K.off = bloom_total; K.word = bloom_words;
-    bloom_total += K.hlen + K.bytes; bloom_words += K.bytes / 4;
-    wide[c].bloom_offset = 1ull << 62; wide[c].bloom_len = INT32_MAX;
+    BloomChunk& Kb = hb[c];
+    Kb.bytes = (uint32_t)bloom_bytes(ndv, Bf.fpp, Bf.max_bytes ? Bf.max_bytes : kBloomDefaultBytes);
+    Kb.hlen = bloom_header(nullptr, Kb.bytes);
+    Kb.off = bloom_total; Kb.word = bloom_words;
+    bloom_total += Kb.hlen + Kb.bytes; bloom_words += Kb.bytes / 4;
   }
+  bloom_at[n_chunks] = bloom_total;
+  std::vector<FileRec> hf(K);
+  for (uint64_t k = 0; k < K; k++) {
+    const uint64_t c0 = frg[k] * nL, c1 = frg[k + 1] * nL;
+    hf[k] = FileRec{frg[k], frg[k + 1], page_base[c0], page_base[c1], bloom_at[c0], bloom_at[c1], 0, 0, 0};
+  }
+  // footers: the schema prefix once; the tail's bound from one file of no row group and one of a row group whose every
+  // field is at its widest (sizes and offsets 2^62, statistics of kStatMax bytes), with room for the varints that
+  // grow with the row count and the row-group ordinal
   const char* created_by = "etl-b200 parquet writer";
-  const uint64_t footer_bound = footer(meta, rg_rows, wide, cc, created_by).size() + 8;
-  const uint64_t data_bound = 4 + P * kPageHeaderMax + (snappy ? C_bound : U);
+  const uint32_t cb_len = (uint32_t)strlen(created_by);
+  TWriter pw(nullptr);
+  footer_prefix(pw, meta);
+  std::vector<uint8_t> prefix(pw.n);
+  { TWriter w(prefix.data()); footer_prefix(w, meta); }
+  const std::vector<LeafMeta> lm = leaf_meta(meta);
+  const std::string stat_x(kStatMax, 'x');
+  auto wide = [&](uint64_t c) {
+    const uint32_t l = (uint32_t)(c % nL);
+    const uint64_t x = 1ull << 62;
+    return ChunkMeta{x, x, x, x, x, x, INT32_MAX, x, x, x, INT32_MAX, INT32_MAX, bloomed(l) ? INT32_MAX : 0u, kStatMax, kStatMax,
+                     true, has_dict(l), pidx != 0, (const uint8_t*)stat_x.data(), (const uint8_t*)stat_x.data()};
+  };
+  const uint64_t wide_rg[2] = {0, 1ull << 62};
+  const uint64_t tail0 = footer_tail(nullptr, lm.data(), nL, wide_rg, 0, wide, cc, (const uint8_t*)created_by, cb_len);
+  const uint64_t tail1 = footer_tail(nullptr, lm.data(), nL, wide_rg, 1, wide, cc, (const uint8_t*)created_by, cb_len);
+  const uint64_t footer_bound = K * (prefix.size() + tail0 + 20 + 8) + (uint64_t)n_rg * (tail1 - tail0 + 40);
+  const uint64_t data_bound = 4 * K + P * kPageHeaderMax + (snappy ? C_bound : U);
   // ETL_PQ_PAGE_INDEX: per page a ColumnIndex entry (null flag, two bounds of at most 64 bytes + a 10-byte length, a
   // null count) and a PageLocation, per chunk the fields' and lists' headers; a byte-array maximum that cannot be
   // incremented stays whole, at most its page's longest row (bounded by the leaf's rows or its value bytes)
@@ -1304,23 +1476,30 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
     for (uint32_t l = 0; l < nL; l++)
       if (vmax[l] > kIndexTruncate) index_bound += std::min<uint64_t>(tot[2 * nL + l], (pages_of[l] + n_rg) * (uint64_t)vmax[l]);
   }
+  // the footers' leaves, names, created_by and schema prefix, in one device block
+  const uint64_t lm_bytes = sizeof(LeafMeta) * nL;
+  uint64_t meta_bytes = lm_bytes + cb_len + prefix.size();
+  for (const Leaf& M : meta) meta_bytes += M.name.size();
   Page* d_pages = (Page*)dalloc(sizeof(Page) * (P + 1));
   uint64_t* d_pbase = (uint64_t*)dalloc(16 * (n_chunks + 1ull));   // page_base | leaf_page_base
   uint64_t* d_lbase = (uint64_t*)dalloc(8 * (nL + 1ull));
   uint8_t* d_lscr = (uint8_t*)dalloc(lscr_base[nL] + 16);
   uint64_t* d_scan = (uint64_t*)dalloc(8 * 4 * (P + 1));   // uslot | cslot | fbase | file offsets, P + 1 each
-  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 6);
+  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 8);
   uint8_t* d_u = (uint8_t*)dalloc(U + 16);
   uint32_t* d_bool = (uint32_t*)dalloc(bool_words * 4 + 8);
   uint8_t* d_c = snappy ? (uint8_t*)dalloc(C_bound + 16) : nullptr;
   uint32_t* d_fsz = snappy ? (uint32_t*)dalloc(n_frag_bound * 4 + 4) : nullptr;
   uint8_t* d_zlit = zstd ? (uint8_t*)dalloc(U + 16) : nullptr;                            // ETL_PQ_ZSTD: literals and
   uint64_t* d_zseq = zstd ? (uint64_t*)dalloc(8 * (U / 4 + n_frag_bound + 1)) : nullptr;  // sequences of k_zstd
-  ChunkOut* d_cout = (ChunkOut*)dalloc(sizeof(ChunkOut) * (n_chunks + nL) + 16ull * n_chunks);
+  ChunkOut* d_cout = (ChunkOut*)dalloc(sizeof(ChunkOut) * (n_chunks + K * nL) + 16ull * n_chunks);
   ChunkOut* d_lout = d_cout ? (ChunkOut*)((uint8_t*)d_cout + sizeof(ChunkOut) * n_chunks + 16ull * n_chunks) : nullptr;
+  FileRec* d_files = (FileRec*)dalloc(sizeof(FileRec) * K + 8 * (K + 1));   // the files | their sizes, then places
+  uint8_t* d_meta = (uint8_t*)dalloc(meta_bytes);
   if (!d_pages || !d_pbase || !d_lbase || !d_lscr || !d_scan || !d_stot || !d_u || !d_bool || !d_cout || (snappy && (!d_c || !d_fsz)) ||
-      (zstd && (!d_zlit || !d_zseq)))
+      (zstd && (!d_zlit || !d_zseq)) || !d_files || !d_meta)
     return fail(ETL_ERR_ALLOC);
+  uint64_t* d_fplace = (uint64_t*)(d_files + K);
   DictChunk* d_dch = nullptr;
   unsigned long long* d_tabn = nullptr;
   unsigned long long* d_dblk = nullptr;
@@ -1354,21 +1533,39 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
     d_bwords = (uint32_t*)dalloc(4 * bloom_words);
     if (!d_bch || !d_bwords) return fail(ETL_ERR_ALLOC);
   }
-  if (cudaMalloc(&Fo->dev, data_bound + bloom_total + index_bound + footer_bound + 64) != cudaSuccess) { Fo->dev = nullptr; return fail(ETL_ERR_ALLOC); }
+  if (cudaMalloc(&dev, data_bound + bloom_total + index_bound + footer_bound + 64) != cudaSuccess) { dev = nullptr; return fail(ETL_ERR_ALLOC); }
+  std::vector<uint8_t> hmeta(meta_bytes);
+  {
+    std::vector<LeafMeta> dm = lm;
+    uint64_t o = lm_bytes;
+    for (uint32_t l = 0; l < nL; l++) {
+      memcpy(hmeta.data() + o, meta[l].name.data(), meta[l].name.size());
+      dm[l].name = d_meta + o;
+      o += meta[l].name.size();
+    }
+    memcpy(hmeta.data(), dm.data(), lm_bytes);
+    memcpy(hmeta.data() + o, created_by, cb_len);
+    memcpy(hmeta.data() + o + cb_len, prefix.data(), prefix.size());
+  }
+  const FooterArgs fa{(const LeafMeta*)d_meta, d_meta + meta_bytes - prefix.size(), d_meta + meta_bytes - prefix.size() - cb_len,
+                      nL, (uint32_t)prefix.size(), cb_len, cc};
   uint64_t* uslot = d_scan; uint64_t* cslot = d_scan + (P + 1); uint64_t* fbase = d_scan + 2 * (P + 1); uint64_t* foff = d_scan + 3 * (P + 1);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_pbase, page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_pbase + n_chunks + 1, leaf_page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_lbase, lscr_base.data(), 8 * (nL + 1ull), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(Fo->dev, "PAR1", 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_files, hf.data(), sizeof(FileRec) * K, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_meta, hmeta.data(), meta_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_bool, 0, bool_words * 4 + 8, st));
   CK(cudaMemsetAsync(d_lscr, 0, lscr_base[nL] + 16, st));
+  CK(cudaMemsetAsync(foff + P, 0, 8, st));
   if (bloom_total) {
     CK(cudaMemcpyAsync(d_bch, hb.data(), sizeof(BloomChunk) * n_chunks, cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(d_bwords, 0, 4 * bloom_words, st));
   }
+  const uint32_t kb = (uint32_t)((K + 1 + kFootWarps - 1) / kFootWarps);   // a warp per file (+ the scan's last entry)
   if (P) {
-    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages, dict);
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, d_rgb, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages, dict);
     // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
     auto fill_scan = [&](int which, uint64_t* dst) {
       k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, cc, dst);
@@ -1377,7 +1574,7 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
     fill_scan(0, uslot);
     if (d_dch) {
       // dictionaries: tables, inserts, first-occurrence flags and their scans, decisions, dictionary pages
-      k_dict_setup<<<(n_chunks + 256) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, n, NN, d_pbase, d_dch, d_tabn);
+      k_dict_setup<<<(n_chunks + 256) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, d_rgb, n, NN, d_pbase, d_dch, d_tabn);
       k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_tabn, n_chunks + 1, d_stot + 4);
       k_dict_place<<<(n_chunks + 255) / 256, 256, 0, st>>>(n_chunks, d_tabn, d_dch);
       CK(cudaMemsetAsync(d_tab, 0xff, 4 * d_slots, st));
@@ -1407,79 +1604,98 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
       else k_snappy<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz);
     }
     k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, cc, fbase, d_fsz, foff, d_dch);
-    CK(cudaMemsetAsync(foff + P, 0, 8, st));
     k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
-    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, cc, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, Fo->dev);
-    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, foff, d_cout, d_dch);
+    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_rgf, d_files, d_bch, pidx, d_cout, d_dch);
+    if (d_ix) {
+      // page index: sizes and boundary orders, their places in each file behind its pages and filters
+      const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
+      k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_rgb, d_rgf, d_files, d_fplace, foff, d_ix, d_ixlen, dev, d_cout);
+      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
+      k_index_place<<<(n_chunks + 63) / 64, 64, 0, st>>>(n_chunks, nL, d_rgf, d_files, foff, d_ix, d_ixlen, d_cout);
+    }
+  }
+  // every file's footer length and size, their scan (the files' places), then every byte at its place
+  k_footer<false><<<kb, 32 * kFootWarps, 0, st>>>(fa, K, d_rgb, d_files, foff, d_ixlen, d_cout, d_fplace, dev);
+  k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)d_fplace, (uint32_t)(K + 1), d_stot + 6);
+  if (P) {
+    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, cc, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, nL, d_rgf, d_files, d_fplace, dev);
     if (bloom_total) {
-      // bloom filters: the bitsets in scratch, then headers and bitsets behind the pages
+      // bloom filters: the bitsets in scratch, then headers and bitsets behind each file's pages
       for (uint32_t l = 0; l < nL; l++)
         if (bloomed(l))
           k_bloom<<<std::min<uint32_t>(kInsBlocks, (uint32_t)((tot[l] + kInsThreads - 1) / kInsThreads) + 1), kInsThreads, 0, st>>>(
-              d_leaves, l, nL, n_rg, row_begin, n, d_bch, d_bwords);
-      k_bloom_write<<<dim3(n_chunks, 16), 256, 0, st>>>(d_bch, d_bwords, d_stot + 3, Fo->dev);
+              d_leaves, l, nL, n_rg, row_begin, d_rgb, d_bch, d_bwords);
+      k_bloom_write<<<dim3(n_chunks, 16), 256, 0, st>>>(d_bch, d_bwords, nL, d_rgf, d_fplace, d_cout, dev);
     }
     if (d_ix) {
-      // page index: sizes and boundary orders, their places behind the pages, the bytes
       const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
-      k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, bloom_total, Fo->dev, d_cout);
-      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
-      k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_ix, d_ixlen, d_stot + 3, bloom_total, Fo->dev, d_cout);
+      k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_rgb, d_rgf, d_files, d_fplace, foff, d_ix, d_ixlen, dev, d_cout);
     }
   }
-  if (nL) k_leaf<<<(nL + 63) / 64, 64, 0, st>>>(d_leaves, nL, P ? n_rg : 0, d_cout, d_lout);
-  // SYNC 2: chunk and leaf records
-  std::vector<ChunkOut> hc(n_chunks), hlo(nL);
-  unsigned long long data_end = 0, index_end = 0;   // the pages' bytes, then the page index's (d_stot 3 and 5)
-  if (P) {
-    CK(cudaMemcpyAsync(hc.data(), d_cout, sizeof(ChunkOut) * n_chunks, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&data_end, d_stot + 3, 8, cudaMemcpyDeviceToHost, st));
-    if (d_ix) CK(cudaMemcpyAsync(&index_end, d_stot + 5, 8, cudaMemcpyDeviceToHost, st));
-  }
-  if (nL) CK(cudaMemcpyAsync(hlo.data(), d_lout, sizeof(ChunkOut) * nL, cudaMemcpyDeviceToHost, st));
+  k_footer<true><<<kb, 32 * kFootWarps, 0, st>>>(fa, K, d_rgb, d_files, foff, d_ixlen, d_cout, d_fplace, dev);
+  k_leaf<<<(uint32_t)((K * nL + 63) / 64), 64, 0, st>>>(d_leaves, nL, K, n_chunks, d_files, d_cout, d_lout);
+  // SYNC 2: the files' places and every (file, leaf) record
+  std::vector<ChunkOut> hlo(K * nL);
+  CK(cudaMemcpyAsync(Fs->offs.data(), d_fplace, 8 * (K + 1), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(hlo.data(), d_lout, sizeof(ChunkOut) * K * nL, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
-  // 5. footer
-  std::vector<Chunk> chunks(n_chunks);
-  for (uint32_t c = 0; c < n_chunks; c++) {
-    const ChunkOut& K = hc[c];
-    chunks[c] = Chunk{K.offset, K.num_values, K.usize, K.csize, K.null_count, K.has != 0,
-                      std::string((const char*)K.min, K.min_len), std::string((const char*)K.max, K.max_len),
-                      K.dict != 0, K.data_offset, K.data_pages, pidx != 0, K.ci_offset, K.oi_offset, K.ci_len, K.oi_len};
-    if (hb[c].bytes) { chunks[c].bloom_offset = 4 + data_end + hb[c].off; chunks[c].bloom_len = hb[c].hlen + hb[c].bytes; }
-  }
-  std::vector<uint8_t> foot = footer(meta, rg_rows, chunks, cc, created_by);
-  const uint32_t flen = (uint32_t)foot.size();
-  for (int b = 0; b < 4; b++) foot.push_back((uint8_t)(flen >> (8 * b)));
-  for (char ch : std::string("PAR1")) foot.push_back((uint8_t)ch);
-  Fo->size = 4 + data_end + bloom_total + index_end + foot.size();
-  CK(cudaMemcpyAsync(Fo->dev + 4 + data_end + bloom_total + index_end, foot.data(), foot.size(), cudaMemcpyHostToDevice, st));
+  const uint64_t total = Fs->offs[K];
   if (to_host) {
-    if (cudaHostAlloc((void**)&Fo->host, Fo->size, cudaHostAllocDefault) != cudaSuccess) { Fo->host = nullptr; return fail(ETL_ERR_ALLOC); }
-    CK(cudaMemcpyAsync(Fo->host, Fo->dev, Fo->size, cudaMemcpyDeviceToHost, st));
-  }
-  CK(cudaStreamSynchronize(st));                      // SYNC 3 (the footer's host buffer is read by the copy)
-  Fo->metrics.resize(nL);
-  Fo->stats.resize(2 * nL);
-  for (uint32_t l = 0; l < nL; l++) {
-    const ChunkOut& K = hlo[l];
-    etl_parquet_metrics& M = Fo->metrics[l];
-    memset(&M, 0, sizeof M);
-    M.field_id = hl[l].is_list ? fields[l].element_field_id : fields[l].field_id;
-    M.flags = K.has ? ETL_PQ_HAS_MIN_MAX : 0;
-    M.num_values = K.num_values; M.null_count = K.null_count; M.nan_count = K.nan_count;
-    M.compressed_bytes = K.csize; M.uncompressed_bytes = K.usize;
-    if (K.has) {
-      Fo->stats[2 * l].assign((const char*)K.min, K.min_len);
-      Fo->stats[2 * l + 1].assign((const char*)K.max, K.max_len);
-      M.min = (const uint8_t*)Fo->stats[2 * l].data(); M.min_len = K.min_len;
-      M.max = (const uint8_t*)Fo->stats[2 * l + 1].data(); M.max_len = K.max_len;
-    }
+    if (cudaHostAlloc((void**)&host, total + 1, cudaHostAllocDefault) != cudaSuccess) { host = nullptr; return fail(ETL_ERR_ALLOC); }
+    CK(cudaMemcpyAsync(host, dev, total, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));                    // SYNC 3
   }
   for (void* p : pool) cudaFree(p);
-  *out = Fo;
+  // metrics: one record per (file, leaf); their statistic bytes in one block
+  uint64_t sb = 0;
+  for (const ChunkOut& R : hlo) if (R.has) sb += R.min_len + R.max_len;
+  Fs->stats.resize(sb);
+  Fs->metrics.resize(K * nL);
+  uint64_t so = 0;
+  for (uint64_t t = 0; t < K * nL; t++) {
+    const ChunkOut& R = hlo[t];
+    const uint32_t l = (uint32_t)(t % nL);
+    etl_parquet_metrics& M = Fs->metrics[t];
+    memset(&M, 0, sizeof M);
+    M.field_id = hl[l].is_list ? fields[l].element_field_id : fields[l].field_id;
+    M.flags = R.has ? ETL_PQ_HAS_MIN_MAX : 0;
+    M.num_values = R.num_values; M.null_count = R.null_count; M.nan_count = R.nan_count;
+    M.compressed_bytes = R.csize; M.uncompressed_bytes = R.usize;
+    if (R.has) {
+      memcpy(Fs->stats.data() + so, R.min, R.min_len); M.min = Fs->stats.data() + so; M.min_len = R.min_len; so += R.min_len;
+      memcpy(Fs->stats.data() + so, R.max, R.max_len); M.max = Fs->stats.data() + so; M.max_len = R.max_len; so += R.max_len;
+    }
+  }
+  Fs->dev = dev; Fs->host = host;
   return ETL_OK;
 #undef CK
+}
+
+}  // namespace
+
+extern "C" {
+
+int etl_dec_parquet_write(const etl_arrow_batch* a, const etl_parquet_field* fields, uint32_t n_fields, uint64_t row_begin,
+                          uint64_t row_end, uint32_t codec, int to_host, etl_parquet_file** out) {
+  return etl_dec_parquet_write_bloom(a, fields, nullptr, n_fields, row_begin, row_end, codec, to_host, out);
+}
+
+int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom,
+                                uint32_t n_fields, uint64_t row_begin, uint64_t row_end, uint32_t codec, int to_host,
+                                etl_parquet_file** out) {
+  if (!out) return ETL_ERR_INVALID_ARG;
+  const uint64_t ro[2] = {row_begin, row_end};
+  etl_parquet_files Fs;
+  const int rc = write_files(a, fields, bloom, n_fields, ro, 1, codec, to_host, &Fs);
+  if (rc != ETL_OK) return rc;
+  etl_parquet_file* Fo = new etl_parquet_file();
+  Fo->dev = Fs.dev; Fo->host = Fs.host; Fo->size = Fs.offs[1];
+  Fo->metrics = std::move(Fs.metrics);              // their min / max point into the moved block
+  Fo->stats = std::move(Fs.stats);
+  Fo->null_column = Fs.null_column; Fo->null_row = Fs.null_row;
+  *out = Fo;
+  return ETL_OK;
 }
 uint64_t etl_dec_parquet_size(const etl_parquet_file* f) { return f ? f->size : 0; }
 const uint8_t* etl_dec_parquet_bytes(const etl_parquet_file* f, int host) { return f ? (host ? f->host : f->dev) : nullptr; }
@@ -1501,18 +1717,52 @@ void etl_dec_parquet_free(etl_parquet_file* f) {
   delete f;
 }
 
+int etl_dec_parquet_write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom,
+                                uint32_t n_fields, const uint64_t* row_offsets, uint64_t n_files, uint32_t codec, int to_host,
+                                etl_parquet_files** out) {
+  if (!out) return ETL_ERR_INVALID_ARG;
+  etl_parquet_files* Fs = new etl_parquet_files();
+  const int rc = write_files(a, fields, bloom, n_fields, row_offsets, n_files, codec, to_host, Fs);
+  if (rc != ETL_OK) { delete Fs; return rc; }
+  *out = Fs;
+  return ETL_OK;
+}
+uint64_t etl_dec_parquet_files_count(const etl_parquet_files* fs) { return fs ? fs->n_files : 0; }
+const uint64_t* etl_dec_parquet_files_offsets(const etl_parquet_files* fs) { return fs ? fs->offs.data() : nullptr; }
+const uint8_t* etl_dec_parquet_files_bytes(const etl_parquet_files* fs, int host) { return fs ? (host ? fs->host : fs->dev) : nullptr; }
+int etl_dec_parquet_files_metrics(const etl_parquet_files* fs, uint64_t file, uint32_t leaf, etl_parquet_metrics* out) {
+  if (!fs || !out || file >= fs->n_files || leaf >= fs->n_leaves || fs->metrics.empty()) return ETL_ERR_INVALID_ARG;
+  *out = fs->metrics[file * fs->n_leaves + leaf];
+  return ETL_OK;
+}
+int etl_dec_parquet_files_required_null(const etl_parquet_files* fs, uint32_t* column, uint64_t* row) {
+  if (!fs) return ETL_ERR_INVALID_ARG;
+  if (column) *column = fs->null_column;
+  if (row) *row = fs->null_row;
+  return ETL_OK;
+}
+void etl_dec_parquet_files_free(etl_parquet_files* fs) {
+  if (!fs) return;
+  if (fs->dev) cudaFree(fs->dev);
+  if (fs->host) cudaFreeHost(fs->host);
+  delete fs;
+}
+
 }  // extern "C"
 
 // ptxas -v, sm_90a, CUDA 12.9 (registers / shared memory / stack):
 //   k_plan 32 / 0 / 0      k_cut 53 / 0 / 0       k_encode<false> 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 10 / 0 / 0
 //   k_encode<true> 64 / 4200 B / 16 B (two 8-byte spills)
-//   k_snappy 50 / 8192 B / 0                      k_page 29 / 0 / 40 B (the header bytes)   k_gather 22 / 0 / 0
+//   k_snappy 50 / 8192 B / 0                      k_page 29 / 0 / 40 B (the header bytes)   k_gather 22 / 0 / 0 (+ a load
+//   of its file's place)
 //   k_zstd 88 / 27772 B / 104 B, no spills (the stack is the canonical-code rank counters of the Huffman table)
-//   k_dict_setup 24 / 0 / 0   k_dict_place 10 / 0 / 0   k_dict_insert 46 / 0 / 0   k_dict_mark 24 / 0 / 0
+//   k_dict_setup 23 / 0 / 0   k_dict_place 10 / 0 / 0   k_dict_insert 46 / 0 / 0   k_dict_mark 24 / 0 / 0
 //   k_dict_finish 22 / 0 / 0  k_dict_page 32 / 0 / 0
-//   k_chunk 56 / 0 / 192 B and k_leaf 56 / 0 / 192 B (the ChunkOut record built in local memory, written once)
-//   k_row_max 12 / 0 / 0   k_index<false> 72 / 0 / 40 B and k_index<true> 64 / 0 / 80 B (a fixed-width bound's bytes;
-//   28 B of it spills, as before the bloom filters)
-//   k_chunk_nn 16 / 0 / 0   k_bloom 54 / 0 / 0   k_bloom_write 29 / 0 / 40 B (the header's Thrift writer)
+//   k_chunk 56 / 0 / 248 B and k_leaf 56 / 0 / 248 B (the ChunkOut record built in local memory, written once)
+//   k_row_max 12 / 0 / 0   k_index<false> 89 / 0 / 40 B and k_index<true> 96 / 0 / 48 B (a fixed-width bound's bytes;
+//   no spills: __maxnreg__(96) instead of the launch bound, which left ptxas at 64 registers and spilling)
+//   k_index_place 30 / 0 / 0   k_footer<false> 96 / 0 / 40 B and k_footer<true> 96 / 0 / 40 B (the Thrift writer;
+//   __maxnreg__(96), as k_index: a 128-thread launch bound left them at 64 registers, one spilling)   k_fill 16 / 0 / 0
+//   k_chunk_nn 14 / 0 / 0   k_bloom 55 / 0 / 0   k_bloom_write 29 / 0 / 40 B (the header's Thrift writer)
 //   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan<unsigned long long> 32 / 8192 B,
 //   k_offsets<uint64_t> 18 / 8192 B

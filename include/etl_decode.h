@@ -952,6 +952,51 @@ int etl_dec_parquet_metrics(const etl_parquet_file*, uint32_t leaf, etl_parquet_
 int etl_dec_parquet_required_null(const etl_parquet_file*, uint32_t* column, uint64_t* row);
 void etl_dec_parquet_free(etl_parquet_file*);
 
+/* ---------------------------------------------------------------- Parquet: many files in one call
+ * Every file of a partitioned write (or of a batch cut into files) in one device call: one plan, one set of allocations
+ * and at most three host syncs (the plan; the sizes, offsets and metrics; with to_host the pinned copy), whatever
+ * n_files is.  No per-file launch, copy or allocation.
+ * Byte identity: file k is exactly the bytes etl_dec_parquet_write_bloom(a, fields, bloom, n_fields, row_offsets[k],
+ * row_offsets[k + 1], codec, to_host) writes, and its metrics per leaf are that call's.  So row groups of at most
+ * 1 048 576 rows restart in every file; RowGroup.ordinal, file_offset and every offset in the footer, page index and
+ * bloom filters are relative to the file; each column chunk of each file has its own dictionary, statistics, page cuts
+ * and bloom bitset (ndv 0: that chunk's own non-null count).
+ * row_offsets: host memory, n_files + 1 non-decreasing emit rows, row_offsets[n_files] <= etl_dec_arrow_rows;
+ * row_offsets[0] may be above 0.  An empty range is the zero-row file the single call writes for it.  n_files == 0 is
+ * ETL_OK with no files (one offset, 0), so a partition result of zero rows can be passed as it is:
+ * etl_dec_parquet_write_files(etl_dec_iceberg_partitioned_arrow(p), …, etl_dec_iceberg_partition_rows(p, 1),
+ * etl_dec_iceberg_partitions(p), …).
+ * Result: etl_dec_parquet_files_offsets gives n_files + 1 byte offsets (host memory); file k is bytes [offs[k],
+ * offs[k + 1]) of etl_dec_parquet_files_bytes(fs, host) (host = 1: the pinned image, NULL without to_host; 0: device
+ * memory), packed in order with no gaps.  etl_dec_parquet_files_metrics gives file k's record of a leaf.
+ * Required nulls: a null in a required column anywhere in [row_offsets[0], row_offsets[n_files]) writes no file (every
+ * offset 0, no bytes, no metrics: ETL_ERR_INVALID_ARG from _metrics) and etl_dec_parquet_files_required_null reports
+ * what the single call over that whole range reports (RecordBatch::try_new fails for the whole batch before any file
+ * is written); a null outside the range does not count.
+ * ETL_ERR_INVALID_ARG, before any launch: everything the single call rejects, a NULL row_offsets or out, n_files >=
+ * 2^32 - 1, decreasing offsets, a last offset past the emit, 2^31 column chunks or more in all (the sum over files of
+ * ceil(rows / 1 048 576) times n_fields: chunk indices and the page index's length scan are 32-bit); in the accessors
+ * an out-of-range file or leaf.  A CUDA failure is ETL_ERR_CUDA and leaks nothing.
+ * Scratch: that of one single call over [row_offsets[0], row_offsets[n_files]) whose row groups are the files', plus
+ * the terms that grow with the files.  Every file has at least one page per leaf (and with ETL_PQ_DICTIONARY a
+ * dictionary slot per non-Boolean leaf), and each page costs about 0.4 KiB of scratch: its 216 B record, 32 B of slot
+ * scans, 64 B of level scratch and, compressed, 8 B plus 32 B per 64 KiB fragment beyond its payload's 7/6 (its
+ * compressed slot is sized by its own payload); and in the output buffer 48 B of header room (+ 189 B with
+ * ETL_PQ_PAGE_INDEX).  Per file: a 72 B record, 8 B of size / offset, its footer's bound (the schema prefix + about
+ * 0.3 KiB per column chunk) in the output buffer, and one metrics record per leaf (248 B on the device, its copy on
+ * the host); per row group 12 B of table; once the schema prefix, leaf names and created_by.  The output buffer is
+ * kept by the result until etl_dec_parquet_files_free. */
+typedef struct etl_parquet_files etl_parquet_files;
+int etl_dec_parquet_write_files(const etl_arrow_batch*, const etl_parquet_field* fields, const etl_parquet_bloom* bloom /* NULL: no filters */,
+                                uint32_t n_fields, const uint64_t* row_offsets /* host, n_files + 1 */, uint64_t n_files,
+                                uint32_t codec, int to_host, etl_parquet_files** out);
+uint64_t etl_dec_parquet_files_count(const etl_parquet_files*);
+const uint64_t* etl_dec_parquet_files_offsets(const etl_parquet_files*);        /* host, n_files + 1 byte offsets */
+const uint8_t* etl_dec_parquet_files_bytes(const etl_parquet_files*, int host);  /* every file, back to back */
+int etl_dec_parquet_files_metrics(const etl_parquet_files*, uint64_t file, uint32_t leaf, etl_parquet_metrics* out);
+int etl_dec_parquet_files_required_null(const etl_parquet_files*, uint32_t* column, uint64_t* row);
+void etl_dec_parquet_files_free(etl_parquet_files*);
+
 /* ---------------------------------------------------------------- Iceberg partitioning
  * Rows [row_begin, row_end) of an Arrow emit grouped by the partition tuple of an Iceberg partition spec, on the device:
  * a permuted copy of the emit in which every partition is one contiguous row range, so that each partition's data file

@@ -37,7 +37,11 @@ k_ice_reps and the radix sort), the length scans and the gather (k_ice_gather_*)
 partitioned emit read from the source and written once: 2 × its column bytes) per second as a kernel share of the
 3.35 TB/s data sheet figure, P, and the whole partitioned write (partition + P file writes) against the unpartitioned
 write.  Before timing, the partition offsets, values and every column of the partitioned emit are compared with
-tests/iceberg_partition_ref.py; every timed file must have the bytes of the first repetition's.
+tests/iceberg_partition_ref.py; every timed file must have the bytes of the first repetition's.  The one-call leg writes
+the same files with one etl_dec_parquet_write_files call over the partition offsets, alternated with the per-partition
+loop and the unpartitioned write in every repetition (its file sizes must be the loop's); one torch.profiler pass
+splits it into kernel time, copies, launches and the call's wall time. A --c1-scale, --c2-scale or --c5-scale of 0 leaves that
+workload out of the --partition run.
 Prints the card name and power limit in the same run.
 """
 import argparse
@@ -283,6 +287,7 @@ def partition_emits(lib, emits, reps, warmup):
     spec = OPTS["spec"]
     codec = abi.PQ_SNAPPY
     call, whole, plain, files, parts, moved, group, scan, gather = [], [], [], 0, 0, 0, 0.0, 0.0, 0.0
+    one, one_spread, prof = [], [], dict(kernel_ms=0.0, memcpy_ms=0.0, launches=0, wall_ms=0.0)
     for a in emits:
         fields = fields_for(emit_columns(lib, a))
         n = lib.etl_dec_arrow_rows(a)
@@ -290,7 +295,7 @@ def partition_emits(lib, emits, reps, warmup):
         g, s, k = _partition_kernel_ms(lib, a, spec, n)
         group, scan, gather = group + g, scan + s, gather + k
         moved += 2 * _emit_bytes(lib, a)
-        first, t_call, t_whole, t_plain = None, [], [], []
+        first, t_call, t_whole, t_plain, t_one = None, [], [], [], []
         for r in range(warmup + reps):
             e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
             e[0].record()
@@ -312,6 +317,22 @@ def partition_emits(lib, emits, reps, warmup):
                 first = sizes
                 files += P
             assert sizes == first
+            # the one-call leg: every partition's file in one etl_dec_parquet_write_files over the same offsets
+            h = _partition(lib, a, spec, n)
+            pa_ = lib.etl_dec_iceberg_partitioned_arrow(h)
+            rows = np.frombuffer((C.c_uint64 * (P + 1)).from_address(lib.etl_dec_iceberg_partition_rows(h, 1)), dtype=np.uint64).copy()
+            o0, o1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            o0.record()
+            rc, fs = write_files(lib, pa_, fields, None, rows, codec, 0)
+            o1.record()
+            o1.synchronize()
+            assert rc == 0
+            offs = np.frombuffer((C.c_uint64 * (P + 1)).from_address(lib.etl_dec_parquet_files_offsets(fs)), dtype=np.uint64)
+            assert np.diff(offs).tolist() == first
+            lib.etl_dec_parquet_files_free(fs)
+            if r == warmup:                                  # one torch.profiler pass (not timed)
+                prof_one(lib, pa_, fields, rows, codec, prof)
+            lib.etl_dec_iceberg_partition_free(h)
             p0, p1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             p0.record()
             rc, fh = pq_write(lib, a, fields, 0, n, codec, 0)
@@ -323,7 +344,10 @@ def partition_emits(lib, emits, reps, warmup):
                 t_call.append(e[0].elapsed_time(e[1]))
                 t_whole.append(e[0].elapsed_time(e[2]))
                 t_plain.append(p0.elapsed_time(p1))
+                t_one.append(o0.elapsed_time(o1))
         call.append(float(np.median(t_call)))
+        one.append(float(np.median(t_one)))
+        one_spread.append([round(min(t_one), 3), round(max(t_one), 3)])
         whole.append(float(np.median(t_whole)))
         plain.append(float(np.median(t_plain)))
     c, w, p = sum(call), sum(whole), sum(plain)
@@ -333,7 +357,42 @@ def partition_emits(lib, emits, reps, warmup):
                 gather_bytes_moved=int(moved), gather_GBps=round(gbps, 1) if gbps else None,
                 gather_kernel_share_of_3_35TBps_pct=round(100 * gbps / 3350, 1) if gbps else None,
                 partitioned_write_ms=round(w, 3), unpartitioned_snappy_write_ms=round(p, 3),
-                ratio=round(w / p, 2) if p else None, ms_per_file=round((w - c) / files, 3) if files else None)
+                ratio=round(w / p, 2) if p else None, ms_per_file=round((w - c) / files, 3) if files else None,
+                one_call_write_ms=round(sum(one), 3), one_call_min_max_per_emit=one_spread,
+                loop_over_one_call=round((w - c) / sum(one), 1) if sum(one) else None,
+                one_call_over_unpartitioned=round(sum(one) / p, 2) if p else None,
+                one_call_profile={k: round(v, 3) if isinstance(v, float) else v for k, v in prof.items()})
+
+
+def write_files(lib, a, fields, bloom, ro, codec, to_host):
+    arr = (abi.ParquetField * max(1, len(fields)))()
+    for i, f in enumerate(fields):
+        arr[i].name, arr[i].field_id, arr[i].element_field_id, arr[i].required = f[0].encode(), f[1], f[2], f[3]
+    offs = np.ascontiguousarray(ro, dtype=np.uint64)
+    h = C.c_void_p()
+    rc = lib.etl_dec_parquet_write_files(a, arr, None, len(fields), offs.ctypes.data_as(C.POINTER(C.c_uint64)), len(offs) - 1,
+                                         codec, to_host, C.byref(h))
+    return rc, h
+
+
+def prof_one(lib, a, fields, ro, codec, acc):
+    """one torch.profiler pass over one etl_dec_parquet_write_files call: the kernels' device time, the copies', the
+    launches and the call's wall time (the rest is host work and the syncs' waits)"""
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as p:
+        t0 = time.perf_counter()
+        rc, fs = write_files(lib, a, fields, None, ro, codec, 0)
+        acc["wall_ms"] += (time.perf_counter() - t0) * 1e3
+    assert rc == 0
+    lib.etl_dec_parquet_files_free(fs)
+    for e in p.key_averages():
+        us = getattr(e, "device_time_total", 0) or getattr(e, "cuda_time_total", 0)
+        if "Memcpy" in e.key or "Memset" in e.key:
+            acc["memcpy_ms"] += us / 1e3
+        elif e.key.startswith(("void", "k_")) or "k_" in e.key:
+            acc["kernel_ms"] += us / 1e3
+            acc["launches"] += e.count
 
 
 def leg(lib, emits, reps, warmup):
@@ -525,6 +584,8 @@ def main():
                                   ("copy", 0, [(0, abi.ICE_BUCKET, 16), (5, abi.ICE_TRUNCATE, 1)]),
                                   ("c5", a.c5_scale, [(0, abi.ICE_BUCKET, 16)])):
             OPTS["spec"] = spec
+            if name != "copy" and not scale:                 # a scale of 0 skips the workload
+                continue
             if name == "copy":
                 copy_table(a.copy_rows, a.reps, a.warmup, a.tag)
             else:
