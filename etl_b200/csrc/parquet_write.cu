@@ -65,7 +65,9 @@
 // (248 B) per leaf; per row group 12 B of table; once the schema prefix, names and created_by.  Per page (a file has
 // at least one per leaf): a 216 B Page, 32 B of slot scans, 64 B of level scratch, a compressed slot sized by its own
 // payload (8 B + the bound of each fragment, 32 B + 7/6 of its bytes), and 48 B of header room in the output.
-// Scratch: per (row, leaf) 3 × 4 B lengths + 3 × 8 B prefix sums; per level entry 2 B (+ 64 B per page of the leaf);
+// Scratch: two cudaMalloc blocks, what the plan needs and then the rest once sized, cut into the named regions of
+// Call::regions, each 256-aligned with 64 B of slack behind it: at most 16 KiB per call on top of the terms here.
+// Per (row, leaf) 3 × 4 B lengths + 3 × 8 B prefix sums; per level entry 2 B (+ 64 B per page of the leaf);
 // Boolean leaves 1 bit per item (+ 4 B per page of the leaf); per page a bounded payload slot (the PLAIN value bytes + levels_bound per section) and,
 // with Snappy, a compressed slot of snappy_bound per fragment; with ETL_PQ_ZSTD, one of zstd_bound (64 KiB + 3 B) per
 // fragment, and 1 B of literal + 2 B of sequence scratch per payload byte (+ 8 B per fragment).  ETL_PQ_DICTIONARY adds, per item of an eligible leaf
@@ -81,6 +83,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -1206,18 +1209,8 @@ uint32_t plain_width(uint32_t at) {
 
 }  // namespace
 
-struct etl_parquet_file {
-  uint8_t* dev = nullptr;
-  uint8_t* host = nullptr;
-  uint64_t size = 0;
-  std::vector<etl_parquet_metrics> metrics;
-  std::vector<uint8_t> stats;                       // min / max bytes of the metrics
-  uint32_t null_column = UINT32_MAX;
-  uint64_t null_row = UINT64_MAX;
-};
 struct etl_parquet_files {
-  uint8_t* dev = nullptr;
-  uint8_t* host = nullptr;
+  uint8_t *dev = nullptr, *host = nullptr;
   uint64_t n_files = 0;
   uint32_t n_leaves = 0;
   std::vector<uint64_t> offs;                       // n_files + 1 byte offsets of the files in dev / host
@@ -1225,29 +1218,124 @@ struct etl_parquet_files {
   std::vector<uint8_t> stats;                       // min / max bytes of the metrics
   uint32_t null_column = UINT32_MAX;
   uint64_t null_row = UINT64_MAX;
+  ~etl_parquet_files() { if (dev) cudaFree(dev); if (host) cudaFreeHost(host); }
 };
+struct etl_parquet_file : etl_parquet_files {};     // etl_dec_parquet_write(_bloom): the K = 1 result
 
 namespace {
 
-// The writer: files k < K, file k the rows [ro[k], ro[k + 1]) of the emit, in one device buffer (and with to_host one
-// pinned image), packed in order.  etl_dec_parquet_write(_bloom) is K = 1.  Fs is filled on ETL_OK; on an error
-// everything the call allocated is freed (Fs owns nothing yet).
-int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom, uint32_t n_fields,
-                const uint64_t* ro, uint64_t K, uint32_t codec, int to_host, etl_parquet_files* Fs) {
+// the slot of each scan's total (k_fill's `which` is its scan's slot; every dictionary scan shares kTotDict)
+enum TotSlot : uint32_t { kTotUslot, kTotCslot, kTotFbase, kTotFoff, kTotDict, kTotIndex, kTotFiles, kTotSlots };
+// places regions one after another (from 0 to size a block, then from the block), each 256-aligned as a cudaMalloc of
+// its own, with kSlack bytes + its extra behind it: a zero-count region is still a valid, distinct pointer
+constexpr uint64_t kAlign = 256, kSlack = 64;
+struct Carve {
+  uintptr_t base;
+  uint64_t at = 0;
+  template <class T> void operator()(T*& p, uint64_t count, uint64_t extra = 0) {
+    p = reinterpret_cast<T*>(base + at);
+    at = (at + sizeof(T) * count + extra + kSlack + kAlign - 1) / kAlign * kAlign;
+  }
+};
+struct Totals {                                     // the plan's results (SYNC 1): per chunk the data pages and
+  std::vector<uint32_t> np;                         // (bloom filters) the non-null values; per leaf the level entries |
+  std::vector<unsigned long long> cnn, tot, req;    // non-null values | PLAIN bytes, a required column's first null row
+  std::vector<unsigned int> vmax;                   // (kNone: none) and (ETL_PQ_PAGE_INDEX) its longest row's PLAIN bytes
+};
+struct Sizes {                                      // every bound and host table, from the description and the totals
+  std::vector<LeafDev> hl;                          // the leaves with their scratch offsets (bscr, dscr, hscr)
+  std::vector<uint64_t> page_base, leaf_page_base, pages_of, lscr_base;
+  uint64_t P, U, n_frag_bound, C_bound, bool_words, d_items, d_heads, d_slots, d_maxI, bloom_total, bloom_words;
+  std::vector<BloomChunk> hb; std::vector<FileRec> hf;
+  std::vector<uint8_t> prefix; std::vector<LeafMeta> lm;   // the footers' schema prefix and leaves
+  uint64_t meta_bytes, data_bound, index_bound, footer_bound;
+};
+constexpr char kCreatedBy[] = "etl-b200 parquet writer";
+constexpr uint32_t kCreatedByLen = sizeof kCreatedBy - 1;
+
+// One writer call: its stages share this record, which owns the scratch blocks until the call returns and the output
+// until collect() hands it over.  Aggregate initialisation zeroes every member it does not name.
+struct Call {
+  const etl_arrow_batch* a; const etl_parquet_field* fields; const etl_parquet_bloom* bloom;
+  uint32_t nL; const uint64_t* ro; uint64_t K; uint32_t codec; int to_host;   // nL: the leaves, one per field
+  uint32_t cc; int dict, pidx, snappy, zstd; bool any_bloom;   // describe(); snappy: compressed fragments (Snappy or Zstandard)
+  std::vector<LeafDev> hl; std::vector<Leaf> meta;
+  std::vector<uint64_t> values, frg, rgb;           // items of each leaf's value column; first row group of each file;
+  std::vector<uint32_t> rgf;                        // row-group starts (local rows), then n; each row group's file
+  uint64_t row_begin, n; uint32_t n_rg, n_chunks;
+  Totals t; Sizes s;                                // plan(), size()
+  // the device scratch: regions of two cudaMalloc blocks, laid out by regions(); a region of a feature the call does
+  // not use stays null (the kernels test for it)
+  LeafDev* d_leaves; Page* d_pages; ChunkOut *d_cout, *d_lout; FileRec* d_files; DictChunk* d_dch; IndexChunk* d_ix; BloomChunk* d_bch;
+  uint32_t *d_ent, *d_nn, *d_vb, *d_np, *d_rgf, *d_bool, *d_fsz, *d_tab, *d_dpos, *d_dflag, *d_desz, *d_dhead, *d_bwords;
+  uint64_t *d_E, *d_NN, *d_V, *d_rgb, *d_pbase, *d_lpbase, *d_lbase, *d_uslot, *d_cslot, *d_fbase, *d_foff, *d_zseq,
+      *d_fplace, *d_dfirst, *d_desum;
+  unsigned long long *d_blk, *d_tot, *d_req, *d_cnn, *d_stot, *d_tabn, *d_dblk, *d_ixlen; unsigned int* d_vmax;
+  uint8_t *d_lscr, *d_u, *d_c, *d_zlit, *d_meta;
+  void* blk[2]; uint8_t *dev, *host;
+  cudaStream_t st = cudaStreamPerThread;
+  ~Call() { for (void* p : blk) if (p) cudaFree(p); if (dev) cudaFree(dev); if (host) cudaFreeHost(host); }
+  bool bloomed(uint32_t l) const { return bloom && bloom[l].fpp > 0.0; }
+  // ETL_PQ_DICTIONARY: every chunk of a non-Boolean leaf has a dictionary slot in front of its data pages
+  bool has_dict(uint32_t l) const { return dict && hl[l].atype != ETL_ARROW_BOOLEAN; }
+  void regions(int b, Carve& r); bool carve(int b);
+  int describe(); int plan(); Sizes size() const; int launch(); int collect(etl_parquet_files* Fs);   // the stages
+};
+
+// block 0 holds what the plan needs (before SYNC 1), block 1 the rest (sized from the totals)
+void Call::regions(int b, Carve& r) {
+  if (b == 0) {
+    const uint64_t nr1 = (uint64_t)nL * (n + 1);    // per (leaf, row): level entries, non-null values, PLAIN value
+    r(d_leaves, nL + 1);                            // bytes, and their prefix sums
+    r(d_ent, nr1); r(d_nn, nr1); r(d_vb, nr1); r(d_E, nr1); r(d_NN, nr1); r(d_V, nr1);
+    r(d_blk, 3ull * nL * (scan_blocks(n) + 1)); r(d_tot, 3ull * nL);
+    r(d_req, nL); r(d_vmax, nL); r(d_np, n_chunks);
+    if (any_bloom) r(d_cnn, n_chunks);
+    r(d_rgb, n_rg + 1ull); r(d_rgf, n_rg + 1ull);
+    return;
+  }
+  const uint64_t P = s.P, nc = n_chunks;
+  r(d_pages, P + 1); r(d_pbase, nc + 1); r(d_lpbase, nc + 1); r(d_lbase, nL + 1ull); r(d_lscr, s.lscr_base[nL], 16);
+  r(d_uslot, P + 1); r(d_cslot, P + 1); r(d_fbase, P + 1); r(d_foff, P + 1); r(d_stot, kTotSlots);
+  r(d_u, s.U, 16); r(d_bool, s.bool_words, 8);
+  if (snappy) { r(d_c, s.C_bound, 16); r(d_fsz, s.n_frag_bound + 1); }
+  if (zstd) { r(d_zlit, s.U, 16); r(d_zseq, s.U / 4 + s.n_frag_bound + 1); }   // k_zstd's literals and sequences
+  r(d_cout, nc, 16 * nc);                           // + the chunks' (min, max) candidates k_leaf reads at cout + nc
+  r(d_lout, K * nL); r(d_files, K); r(d_fplace, K + 1); r(d_meta, s.meta_bytes);
+  if (s.d_items && P) {
+    r(d_dch, nc); r(d_tabn, nc + 1); r(d_dblk, scan_blocks(s.d_maxI) + 2ull); r(d_tab, s.d_slots); r(d_dhead, s.d_heads);
+    r(d_dpos, s.d_items); r(d_dflag, s.d_items); r(d_desz, s.d_items); r(d_dfirst, s.d_items); r(d_desum, s.d_items);
+  }
+  if (pidx && P) { r(d_ix, nc); r(d_ixlen, 2 * nc + 1); }
+  if (s.bloom_total) { r(d_bch, nc); r(d_bwords, s.bloom_words); }
+}
+// sizes block b, allocates it and places its regions
+bool Call::carve(int b) {
+  Carve r{0};
+  regions(b, r);
+  if (cudaMalloc(&blk[b], r.at) != cudaSuccess) { blk[b] = nullptr; return false; }
+  r = Carve{(uintptr_t)blk[b]};
+  regions(b, r);
+  return true;
+}
+
+#define CK(call) do { if ((call) != cudaSuccess) return ETL_ERR_CUDA; } while (0)
+
+// Describe: check the arguments, build the leaves, their schema and the row-group table (no CUDA call)
+int Call::describe() {
   // a file needs at least one column (an emit of a zero-column table without ETL_ARROW_CDC_COLUMNS has none)
-  if (!a || !ro || !n_fields || !fields || n_fields != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
-  const uint32_t cc = codec & 0xFFu;                  // the compression codec; the flag bits are ETL_PQ_DICTIONARY and
+  if (!a || !ro || !nL || !fields || nL != etl_dec_arrow_cols(a)) return ETL_ERR_INVALID_ARG;
+  cc = codec & 0xFFu;                               // the compression codec; the flag bits are ETL_PQ_DICTIONARY and
   if ((codec & ~(0xFFu | ETL_PQ_DICTIONARY | ETL_PQ_PAGE_INDEX)) ||   // ETL_PQ_PAGE_INDEX
       (cc != ETL_PQ_UNCOMPRESSED && cc != ETL_PQ_SNAPPY && cc != ETL_PQ_ZSTD))
     return ETL_ERR_INVALID_ARG;
   if (K >= UINT32_MAX) return ETL_ERR_INVALID_ARG;
   for (uint64_t k = 0; k < K; k++) if (ro[k + 1] < ro[k]) return ETL_ERR_INVALID_ARG;
   if (ro[K] > etl_dec_arrow_rows(a)) return ETL_ERR_INVALID_ARG;
-  const int dict = (codec & ETL_PQ_DICTIONARY) != 0;
-  const int pidx = (codec & ETL_PQ_PAGE_INDEX) != 0;
-  std::vector<LeafDev> hl(n_fields);
-  std::vector<Leaf> meta(n_fields);
-  for (uint32_t c = 0; c < n_fields; c++) {
+  dict = (codec & ETL_PQ_DICTIONARY) != 0; pidx = (codec & ETL_PQ_PAGE_INDEX) != 0;
+  snappy = cc != ETL_PQ_UNCOMPRESSED; zstd = cc == ETL_PQ_ZSTD;
+  hl.resize(nL); meta.resize(nL); values.resize(nL);
+  for (uint32_t c = 0; c < nL; c++) {
     const etl_parquet_field& F = fields[c];
     if (!F.name) return ETL_ERR_INVALID_ARG;
     const size_t nl = strnlen(F.name, 1025);
@@ -1258,10 +1346,10 @@ int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const
     memset(&L, 0, sizeof L);
     L.is_list = col.arrow_type == ETL_ARROW_LIST;
     L.required = F.required != 0;
+    values[c] = etl_dec_arrow_rows(a);
     if (L.is_list) {
       etl_arrow_column kid;
-      uint64_t ne = 0;
-      if (etl_dec_arrow_list_child(a, c, 0, &kid, &ne) != ETL_OK) return ETL_ERR_INVALID_ARG;
+      if (etl_dec_arrow_list_child(a, c, 0, &kid, &values[c]) != ETL_OK) return ETL_ERR_INVALID_ARG;
       L.lvalid = col.validity; L.loffs = (const int32_t*)col.offsets;
       col = kid;
     }
@@ -1279,6 +1367,7 @@ int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const
           (Bf.fpp > 0.0 && L.atype == ETL_ARROW_BOOLEAN))
         return ETL_ERR_INVALID_ARG;
     }
+    any_bloom |= bloomed(c);
     Leaf& M = meta[c];
     M.name.assign(F.name, nl);
     M.field_id = F.field_id; M.element_field_id = F.element_field_id;
@@ -1295,166 +1384,125 @@ int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const
       default: break;
     }
   }
-  const uint32_t nL = n_fields;
   // the row-group table: row groups restart in every file; chunk indices are 32-bit, and the page index's length scan
   // runs over 2 × chunks + 1 entries in 32 bits, so at most 2^31 - 1 chunks
-  std::vector<uint64_t> frg;
   const std::vector<RowGroup> rgt = row_group_table(ro, K, frg);
   if ((uint64_t)rgt.size() * nL >= (1ull << 31)) return ETL_ERR_INVALID_ARG;
-  Fs->n_files = K; Fs->n_leaves = nL;
-  Fs->offs.assign(K + 1, 0);
   if (!K) return ETL_OK;
-  const uint64_t row_begin = ro[0], n = ro[K] - ro[0];
-  const uint32_t n_rg = (uint32_t)rgt.size();
-  const uint32_t n_chunks = n_rg * nL;
-  std::vector<uint64_t> rgb(n_rg + 1, n);             // row-group starts (local rows), then n
-  std::vector<uint32_t> rgf(n_rg + 1, 0);             // the file of each row group
+  row_begin = ro[0]; n = ro[K] - ro[0];
+  n_rg = (uint32_t)rgt.size(); n_chunks = n_rg * nL;
+  rgb.assign(n_rg + 1, n); rgf.assign(n_rg + 1, 0);
   for (uint32_t g = 0; g < n_rg; g++) { rgb[g] = rgt[g].row0; rgf[g] = (uint32_t)rgt[g].file; }
-  const int snappy = cc != ETL_PQ_UNCOMPRESSED;        // Snappy or Zstandard: compressed fragments
-  const int zstd = cc == ETL_PQ_ZSTD;
-  auto bloomed = [&](uint32_t l) { return bloom && bloom[l].fpp > 0.0; };
-  bool any_bloom = false;
-  for (uint32_t l = 0; l < nL; l++) any_bloom |= bloomed(l);
-  cudaStream_t st = cudaStreamPerThread;
-  uint8_t* dev = nullptr;
-  uint8_t* host = nullptr;
-  std::vector<void*> pool;
-  auto dalloc = [&](uint64_t bytes) -> void* { void* p = nullptr; if (cudaMalloc(&p, bytes + 64) != cudaSuccess) return nullptr; pool.push_back(p); return p; };
-  auto fail = [&](int rc) { cudaGetLastError(); for (void* p : pool) cudaFree(p); if (dev) cudaFree(dev); if (host) cudaFreeHost(host); return rc; };
-#define CK(call) do { if ((call) != cudaSuccess) return fail(ETL_ERR_CUDA); } while (0)
-  // 1. plan
-  LeafDev* d_leaves = (LeafDev*)dalloc(sizeof(LeafDev) * (nL + 1));
-  const uint64_t nr1 = (uint64_t)nL * (n + 1);
-  uint32_t* d_len = (uint32_t*)dalloc(3 * nr1 * 4);
-  uint64_t* d_pre = (uint64_t*)dalloc(3 * nr1 * 8);
+  return ETL_OK;
+}
+
+// Plan (block 0): k_plan and the length scans, the counting k_cut, k_row_max, k_chunk_nn; SYNC 1 reads the totals
+int Call::plan() {
+  if (!carve(0)) return ETL_ERR_ALLOC;
   const uint32_t lb = scan_blocks(n);
-  unsigned long long* d_blk = (unsigned long long*)dalloc(3ull * nL * (lb + 1) * 8);
-  unsigned long long* d_tot = (unsigned long long*)dalloc(3ull * nL * 8);
-  unsigned long long* d_req = (unsigned long long*)dalloc(nL * 8ull + 4ull * nL);   // | ETL_PQ_PAGE_INDEX: k_row_max
-  uint32_t* d_np = (uint32_t*)dalloc(n_chunks * 4ull);
-  unsigned long long* d_cnn = any_bloom ? (unsigned long long*)dalloc(n_chunks * 8ull) : nullptr;   // bloom: per chunk
-  uint64_t* d_rgb = (uint64_t*)dalloc(8ull * (n_rg + 1) + 4ull * (n_rg + 1));        // row-group starts | files
-  if (!d_leaves || !d_len || !d_pre || !d_blk || !d_tot || !d_req || !d_np || (any_bloom && !d_cnn) || !d_rgb) return fail(ETL_ERR_ALLOC);
-  uint32_t* d_rgf = (uint32_t*)(d_rgb + n_rg + 1);
   CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_rgb, rgb.data(), 8ull * (n_rg + 1), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_rgf, rgf.data(), 4ull * (n_rg + 1), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_req, 0xff, nL * 8ull, st));
-  unsigned int* d_vmax = (unsigned int*)(d_req + nL);
   if (pidx) CK(cudaMemsetAsync(d_vmax, 0, 4ull * nL, st));
   CK(cudaMemsetAsync(d_tot, 0, 3ull * nL * 8, st));
-  CK(cudaMemsetAsync(d_pre, 0, 3 * nr1 * 8, st));
-  uint32_t* ent = d_len; uint32_t* nn = d_len + nr1; uint32_t* vb = d_len + 2 * nr1;
-  uint64_t* E = d_pre; uint64_t* NN = d_pre + nr1; uint64_t* V = d_pre + 2 * nr1;
-  if (n && nL) {
-    k_plan<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, row_begin, n, ent, nn, vb, d_req);
+  uint32_t* lens[3] = {d_ent, d_nn, d_vb}; uint64_t* pre[3] = {d_E, d_NN, d_V};
+  for (uint64_t* p : pre) CK(cudaMemsetAsync(p, 0, 8ull * nL * (n + 1), st));
+  if (n) {
+    k_plan<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, row_begin, n, d_ent, d_nn, d_vb, d_req);
     for (uint32_t s = 0; s < 3; s++)
       for (uint32_t l = 0; l < nL; l++) {
         const uint64_t at = (uint64_t)(s * nL + l);
-        uint32_t* lens = d_len + s * nr1 + (uint64_t)l * (n + 1);
-        scan_lengths(lens, n, d_blk + at * (lb + 1), d_tot + at, d_pre + s * nr1 + (uint64_t)l * (n + 1), st);
+        scan_lengths(lens[s] + (uint64_t)l * (n + 1), n, d_blk + at * (lb + 1), d_tot + at, pre[s] + (uint64_t)l * (n + 1), st);
       }
-    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, d_rgb, n, E, NN, V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
-    if (pidx) k_row_max<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, n, vb, d_vmax);
-    if (any_bloom) k_chunk_nn<<<(n_chunks + 255) / 256, 256, 0, st>>>(nL, n_chunks, n, d_rgb, NN, d_cnn);
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, d_rgb, n, d_E, d_NN, d_V, d_np, nullptr, nullptr, nullptr, nullptr, 0);
+    if (pidx) k_row_max<<<dim3((uint32_t)((n + 255) / 256), nL), 256, 0, st>>>(d_leaves, n, d_vb, d_vmax);
+    if (any_bloom) k_chunk_nn<<<(n_chunks + 255) / 256, 256, 0, st>>>(nL, n_chunks, n, d_rgb, d_NN, d_cnn);
   }
   // SYNC 1: page counts, totals, required-column nulls (bloom filters: the chunks' non-null values)
-  std::vector<uint32_t> np(n_chunks);
-  std::vector<unsigned long long> cnn(n_chunks);
-  if (any_bloom && n_chunks) CK(cudaMemcpyAsync(cnn.data(), d_cnn, n_chunks * 8ull, cudaMemcpyDeviceToHost, st));
-  std::vector<unsigned long long> tot(3ull * nL), req(nL);
-  std::vector<unsigned int> vmax(nL);
-  if (n_chunks) CK(cudaMemcpyAsync(np.data(), d_np, n_chunks * 4ull, cudaMemcpyDeviceToHost, st));
-  if (nL) {
-    CK(cudaMemcpyAsync(tot.data(), d_tot, 3ull * nL * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(req.data(), d_req, nL * 8ull, cudaMemcpyDeviceToHost, st));
-    if (pidx) CK(cudaMemcpyAsync(vmax.data(), d_vmax, 4ull * nL, cudaMemcpyDeviceToHost, st));
-  }
+  t.np.assign(n_chunks, 0); t.cnn.assign(n_chunks, 0); t.tot.assign(3ull * nL, 0); t.req.assign(nL, 0); t.vmax.assign(nL, 0);
+  if (any_bloom && n_chunks) CK(cudaMemcpyAsync(t.cnn.data(), d_cnn, n_chunks * 8ull, cudaMemcpyDeviceToHost, st));
+  if (n_chunks) CK(cudaMemcpyAsync(t.np.data(), d_np, n_chunks * 4ull, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(t.tot.data(), d_tot, 3ull * nL * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(t.req.data(), d_req, nL * 8ull, cudaMemcpyDeviceToHost, st));
+  if (pidx) CK(cudaMemcpyAsync(t.vmax.data(), d_vmax, 4ull * nL, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  for (uint32_t l = 0; l < nL; l++)
-    if (req[l] != kNone) {                            // RecordBatch::try_new fails before anything is written
-      Fs->null_column = l; Fs->null_row = req[l];
-      for (void* p : pool) cudaFree(p);
-      return ETL_OK;
-    }
-  // ETL_PQ_DICTIONARY: every chunk of a non-Boolean leaf has a dictionary slot in front of its data pages
-  auto has_dict = [&](uint32_t l) { return dict && hl[l].atype != ETL_ARROW_BOOLEAN; };
-  std::vector<uint64_t> page_base(n_chunks + 1, 0);
-  for (uint32_t c = 0; c < n_chunks; c++) page_base[c + 1] = page_base[c] + np[c] + (has_dict(c % nL) ? 1 : 0);
-  const uint64_t P = page_base[n_chunks];
+  return ETL_OK;
+}
+
+// Size: every bound and host table, a function of the description and the totals
+Sizes Call::size() const {
+  const std::vector<unsigned long long>& tot = t.tot;
+  Sizes o{};
+  o.hl = hl;
+  o.page_base.assign(n_chunks + 1, 0);
+  for (uint32_t c = 0; c < n_chunks; c++) o.page_base[c + 1] = o.page_base[c] + t.np[c] + (has_dict(c % nL) ? 1 : 0);
+  o.P = o.page_base[n_chunks];
   // bounds of every buffer from the totals
-  std::vector<uint64_t> pages_of(nL, 0), lscr_base(nL + 1, 0);
-  for (uint32_t c = 0; c < n_chunks; c++) pages_of[c % nL] += np[c];
-  uint64_t U = 0;
+  o.pages_of.assign(nL, 0);
+  for (uint32_t c = 0; c < n_chunks; c++) o.pages_of[c % nL] += t.np[c];
   for (uint32_t l = 0; l < nL; l++) {
-    const uint64_t El = tot[l], NNl = tot[nL + l], Vl = tot[2 * nL + l], Pl = pages_of[l];
+    const uint64_t El = tot[l], NNl = tot[nL + l], Vl = tot[2 * nL + l], Pl = o.pages_of[l];
     const uint64_t lev = 14 * Pl + (El / 8 + Pl) * (hl[l].w + 2);
-    U += (hl[l].atype == ETL_ARROW_BOOLEAN ? NNl / 8 + Pl : Vl) + (hl[l].max_def ? lev : 0) + (hl[l].max_rep ? 14 * Pl + (El / 8 + Pl) * 3 : 0);
-    if (has_dict(l)) U += std::min<uint64_t>(Vl, n_rg * kDictBytes) + 32 * Pl;   // the dictionary slots, the index runs
+    o.U += (hl[l].atype == ETL_ARROW_BOOLEAN ? NNl / 8 + Pl : Vl) + (hl[l].max_def ? lev : 0) + (hl[l].max_rep ? 14 * Pl + (El / 8 + Pl) * 3 : 0);
+    if (has_dict(l)) o.U += std::min<uint64_t>(Vl, n_rg * kDictBytes) + 32 * Pl;   // the dictionary slots, the index runs
   }
   // dictionary scratch: per item bound (a leaf's level entries) slot, flag, entry size / index, two prefix sums; run
   // heads per 8 items + 3 per page; the chunks' tables of at most 4 × non-null values (+ 1) slots
-  uint64_t d_items = 0, d_heads = 0, d_slots = 0, d_maxI = 0;
   for (uint32_t l = 0; l < nL; l++) {
     if (!has_dict(l)) continue;
-    hl[l].dscr = d_items; hl[l].hscr = d_heads;
-    d_items += tot[l] + 1;
-    d_heads += tot[l] / 8 + 3 * (pages_of[l] + 1) + 8;
-    d_slots += 4 * tot[nL + l] + n_rg;
-    d_maxI = std::max<uint64_t>(d_maxI, tot[l]);
+    o.hl[l].dscr = o.d_items; o.hl[l].hscr = o.d_heads;
+    o.d_items += tot[l] + 1;
+    o.d_heads += tot[l] / 8 + 3 * (o.pages_of[l] + 1) + 8;
+    o.d_slots += 4 * tot[nL + l] + n_rg;
+    o.d_maxI = std::max<uint64_t>(o.d_maxI, tot[l]);
   }
-  // level scratch: per leaf 2 × (entries + 16 per page (alignment) + slack); page_base enters the per-page offset
   // level scratch of a leaf: rep | def of each page, 8-aligned, at 2 * align8(e0) + 64 * (page index within the leaf)
-  for (uint32_t l = 0; l < nL; l++) lscr_base[l + 1] = lscr_base[l] + 2 * ((tot[l] + 7) & ~7ull) + 64 * (pages_of[l] + 1) + 64;
-  std::vector<uint64_t> leaf_page_base(n_chunks + 1, 0);   // pages of the chunk's leaf in the row groups before it
-  for (uint32_t c = nL; c < n_chunks; c++) leaf_page_base[c] = leaf_page_base[c - nL] + np[c - nL];
-  const uint64_t n_frag_bound = snappy ? U / kFragment + P + 1 : 0;
+  o.lscr_base.assign(nL + 1, 0);
+  for (uint32_t l = 0; l < nL; l++) o.lscr_base[l + 1] = o.lscr_base[l] + 2 * ((tot[l] + 7) & ~7ull) + 64 * (o.pages_of[l] + 1) + 64;
+  o.leaf_page_base.assign(n_chunks + 1, 0);         // pages of the chunk's leaf in the row groups before it
+  for (uint32_t c = nL; c < n_chunks; c++) o.leaf_page_base[c] = o.leaf_page_base[c - nL] + t.np[c - nL];
+  o.n_frag_bound = snappy ? o.U / kFragment + o.P + 1 : 0;
   // compressed slots: 8 B per page and each fragment's bound (affine in its bytes: 32 + 7 n / 6 at most), the
   // fragments' bytes adding up to at most U
-  const uint64_t C_bound = snappy ? 8 * P + 32 * n_frag_bound + U + U / 6 : 0;
+  o.C_bound = snappy ? 8 * o.P + 32 * o.n_frag_bound + o.U + o.U / 6 : 0;
   // bit scratch: page lp of a Boolean leaf starts at word bscr + it0 / 32 + lp
-  uint64_t bool_words = 0;
   for (uint32_t l = 0; l < nL; l++)
     if (hl[l].atype == ETL_ARROW_BOOLEAN) {
-      etl_arrow_column col; uint64_t ne = 0;
-      if (hl[l].is_list) etl_dec_arrow_list_child(a, l, 0, &col, &ne); else ne = etl_dec_arrow_rows(a);
-      hl[l].bscr = bool_words;
-      bool_words += ne / 32 + pages_of[l] + 2;
+      o.hl[l].bscr = o.bool_words;
+      o.bool_words += values[l] / 32 + o.pages_of[l] + 2;
     }
   // bloom filters: each filtered chunk's bitset size from its ndv (or non-null count), its header, its place among the
   // call's filters (row-group major, column minor: each file's run follows its pages) and its bitset's place in the
   // zeroed scratch
-  std::vector<BloomChunk> hb(n_chunks, BloomChunk{0, 0, 0, 0});
+  o.hb.assign(n_chunks, BloomChunk{0, 0, 0, 0});
   std::vector<uint64_t> bloom_at(n_chunks + 1, 0);
-  uint64_t bloom_total = 0, bloom_words = 0;
   for (uint32_t c = 0; c < n_chunks; c++) {
     const uint32_t l = c % nL;
-    bloom_at[c] = bloom_total;
+    bloom_at[c] = o.bloom_total;
     if (!bloomed(l)) continue;
     const etl_parquet_bloom& Bf = bloom[l];
-    const uint64_t ndv = Bf.ndv ? Bf.ndv : std::max<uint64_t>(1, cnn[c]);
-    BloomChunk& Kb = hb[c];
+    const uint64_t ndv = Bf.ndv ? Bf.ndv : std::max<uint64_t>(1, t.cnn[c]);
+    BloomChunk& Kb = o.hb[c];
     Kb.bytes = (uint32_t)bloom_bytes(ndv, Bf.fpp, Bf.max_bytes ? Bf.max_bytes : kBloomDefaultBytes);
     Kb.hlen = bloom_header(nullptr, Kb.bytes);
-    Kb.off = bloom_total; Kb.word = bloom_words;
-    bloom_total += Kb.hlen + Kb.bytes; bloom_words += Kb.bytes / 4;
+    Kb.off = o.bloom_total; Kb.word = o.bloom_words;
+    o.bloom_total += Kb.hlen + Kb.bytes; o.bloom_words += Kb.bytes / 4;
   }
-  bloom_at[n_chunks] = bloom_total;
-  std::vector<FileRec> hf(K);
+  bloom_at[n_chunks] = o.bloom_total;
+  o.hf.resize(K);
   for (uint64_t k = 0; k < K; k++) {
     const uint64_t c0 = frg[k] * nL, c1 = frg[k + 1] * nL;
-    hf[k] = FileRec{frg[k], frg[k + 1], page_base[c0], page_base[c1], bloom_at[c0], bloom_at[c1], 0, 0, 0};
+    o.hf[k] = FileRec{frg[k], frg[k + 1], o.page_base[c0], o.page_base[c1], bloom_at[c0], bloom_at[c1], 0, 0, 0};
   }
   // footers: the schema prefix once; the tail's bound from one file of no row group and one of a row group whose every
   // field is at its widest (sizes and offsets 2^62, statistics of kStatMax bytes), with room for the varints that
   // grow with the row count and the row-group ordinal
-  const char* created_by = "etl-b200 parquet writer";
-  const uint32_t cb_len = (uint32_t)strlen(created_by);
   TWriter pw(nullptr);
   footer_prefix(pw, meta);
-  std::vector<uint8_t> prefix(pw.n);
-  { TWriter w(prefix.data()); footer_prefix(w, meta); }
-  const std::vector<LeafMeta> lm = leaf_meta(meta);
+  o.prefix.resize(pw.n);
+  { TWriter w(o.prefix.data()); footer_prefix(w, meta); }
+  o.lm = leaf_meta(meta);
   const std::string stat_x(kStatMax, 'x');
   auto wide = [&](uint64_t c) {
     const uint32_t l = (uint32_t)(c % nL);
@@ -1463,201 +1511,153 @@ int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const
                      true, has_dict(l), pidx != 0, (const uint8_t*)stat_x.data(), (const uint8_t*)stat_x.data()};
   };
   const uint64_t wide_rg[2] = {0, 1ull << 62};
-  const uint64_t tail0 = footer_tail(nullptr, lm.data(), nL, wide_rg, 0, wide, cc, (const uint8_t*)created_by, cb_len);
-  const uint64_t tail1 = footer_tail(nullptr, lm.data(), nL, wide_rg, 1, wide, cc, (const uint8_t*)created_by, cb_len);
-  const uint64_t footer_bound = K * (prefix.size() + tail0 + 20 + 8) + (uint64_t)n_rg * (tail1 - tail0 + 40);
-  const uint64_t data_bound = 4 * K + P * kPageHeaderMax + (snappy ? C_bound : U);
+  const uint64_t tail0 = footer_tail(nullptr, o.lm.data(), nL, wide_rg, 0, wide, cc, (const uint8_t*)kCreatedBy, kCreatedByLen);
+  const uint64_t tail1 = footer_tail(nullptr, o.lm.data(), nL, wide_rg, 1, wide, cc, (const uint8_t*)kCreatedBy, kCreatedByLen);
+  o.footer_bound = K * (o.prefix.size() + tail0 + 20 + 8) + (uint64_t)n_rg * (tail1 - tail0 + 40);
+  o.data_bound = 4 * K + o.P * kPageHeaderMax + (snappy ? o.C_bound : o.U);
   // ETL_PQ_PAGE_INDEX: per page a ColumnIndex entry (null flag, two bounds of at most 64 bytes + a 10-byte length, a
   // null count) and a PageLocation, per chunk the fields' and lists' headers; a byte-array maximum that cannot be
   // incremented stays whole, at most its page's longest row (bounded by the leaf's rows or its value bytes)
-  uint64_t index_bound = 0;
   if (pidx) {
-    index_bound = P * (1 + 2 * (10 + kIndexTruncate) + 10 + 30) + 64ull * n_chunks;
+    o.index_bound = o.P * (1 + 2 * (10 + kIndexTruncate) + 10 + 30) + 64ull * n_chunks;
     for (uint32_t l = 0; l < nL; l++)
-      if (vmax[l] > kIndexTruncate) index_bound += std::min<uint64_t>(tot[2 * nL + l], (pages_of[l] + n_rg) * (uint64_t)vmax[l]);
+      if (t.vmax[l] > kIndexTruncate) o.index_bound += std::min<uint64_t>(tot[2 * nL + l], (o.pages_of[l] + n_rg) * (uint64_t)t.vmax[l]);
   }
   // the footers' leaves, names, created_by and schema prefix, in one device block
+  o.meta_bytes = sizeof(LeafMeta) * nL + kCreatedByLen + o.prefix.size();
+  for (const Leaf& M : meta) o.meta_bytes += M.name.size();
+  return o;
+}
+
+// Launch (block 1 and the output buffer): the uploads, then every stage's kernels in order
+int Call::launch() {
+  if (!carve(1)) return ETL_ERR_ALLOC;
+  const uint64_t P = s.P;
+  if (cudaMalloc(&dev, s.data_bound + s.bloom_total + s.index_bound + s.footer_bound + 64) != cudaSuccess) { dev = nullptr; return ETL_ERR_ALLOC; }
+  // the footers' device block: the leaves (their names pointing into it), the names, created_by, the schema prefix
   const uint64_t lm_bytes = sizeof(LeafMeta) * nL;
-  uint64_t meta_bytes = lm_bytes + cb_len + prefix.size();
-  for (const Leaf& M : meta) meta_bytes += M.name.size();
-  Page* d_pages = (Page*)dalloc(sizeof(Page) * (P + 1));
-  uint64_t* d_pbase = (uint64_t*)dalloc(16 * (n_chunks + 1ull));   // page_base | leaf_page_base
-  uint64_t* d_lbase = (uint64_t*)dalloc(8 * (nL + 1ull));
-  uint8_t* d_lscr = (uint8_t*)dalloc(lscr_base[nL] + 16);
-  uint64_t* d_scan = (uint64_t*)dalloc(8 * 4 * (P + 1));   // uslot | cslot | fbase | file offsets, P + 1 each
-  unsigned long long* d_stot = (unsigned long long*)dalloc(8 * 8);
-  uint8_t* d_u = (uint8_t*)dalloc(U + 16);
-  uint32_t* d_bool = (uint32_t*)dalloc(bool_words * 4 + 8);
-  uint8_t* d_c = snappy ? (uint8_t*)dalloc(C_bound + 16) : nullptr;
-  uint32_t* d_fsz = snappy ? (uint32_t*)dalloc(n_frag_bound * 4 + 4) : nullptr;
-  uint8_t* d_zlit = zstd ? (uint8_t*)dalloc(U + 16) : nullptr;                            // ETL_PQ_ZSTD: literals and
-  uint64_t* d_zseq = zstd ? (uint64_t*)dalloc(8 * (U / 4 + n_frag_bound + 1)) : nullptr;  // sequences of k_zstd
-  ChunkOut* d_cout = (ChunkOut*)dalloc(sizeof(ChunkOut) * (n_chunks + K * nL) + 16ull * n_chunks);
-  ChunkOut* d_lout = d_cout ? (ChunkOut*)((uint8_t*)d_cout + sizeof(ChunkOut) * n_chunks + 16ull * n_chunks) : nullptr;
-  FileRec* d_files = (FileRec*)dalloc(sizeof(FileRec) * K + 8 * (K + 1));   // the files | their sizes, then places
-  uint8_t* d_meta = (uint8_t*)dalloc(meta_bytes);
-  if (!d_pages || !d_pbase || !d_lbase || !d_lscr || !d_scan || !d_stot || !d_u || !d_bool || !d_cout || (snappy && (!d_c || !d_fsz)) ||
-      (zstd && (!d_zlit || !d_zseq)) || !d_files || !d_meta)
-    return fail(ETL_ERR_ALLOC);
-  uint64_t* d_fplace = (uint64_t*)(d_files + K);
-  DictChunk* d_dch = nullptr;
-  unsigned long long* d_tabn = nullptr;
-  unsigned long long* d_dblk = nullptr;
-  uint32_t *d_tab = nullptr, *d_dpos = nullptr, *d_dflag = nullptr, *d_desz = nullptr, *d_dhead = nullptr;
-  uint64_t *d_dfirst = nullptr, *d_desum = nullptr;
-  const uint32_t dlb = scan_blocks(d_maxI);
-  if (d_items && P) {
-    d_dch = (DictChunk*)dalloc(sizeof(DictChunk) * n_chunks);
-    d_tabn = (unsigned long long*)dalloc(8 * (n_chunks + 1ull));
-    d_dblk = (unsigned long long*)dalloc(8 * (dlb + 2ull));
-    d_tab = (uint32_t*)dalloc(4 * d_slots);
-    d_dpos = (uint32_t*)dalloc(4 * d_items);
-    d_dflag = (uint32_t*)dalloc(4 * d_items);
-    d_desz = (uint32_t*)dalloc(4 * d_items);
-    d_dhead = (uint32_t*)dalloc(4 * d_heads);
-    d_dfirst = (uint64_t*)dalloc(8 * d_items);
-    d_desum = (uint64_t*)dalloc(8 * d_items);
-    if (!d_dch || !d_tabn || !d_dblk || !d_tab || !d_dpos || !d_dflag || !d_desz || !d_dhead || !d_dfirst || !d_desum) return fail(ETL_ERR_ALLOC);
+  std::vector<uint8_t> hmeta(s.meta_bytes);
+  std::vector<LeafMeta> dm = s.lm;
+  uint64_t o = lm_bytes;
+  for (uint32_t l = 0; l < nL; l++) {
+    memcpy(hmeta.data() + o, meta[l].name.data(), meta[l].name.size());
+    dm[l].name = d_meta + o;
+    o += meta[l].name.size();
   }
-  IndexChunk* d_ix = nullptr;
-  unsigned long long* d_ixlen = nullptr;
-  if (pidx && P) {
-    d_ix = (IndexChunk*)dalloc(sizeof(IndexChunk) * n_chunks);
-    d_ixlen = (unsigned long long*)dalloc(8 * (2ull * n_chunks + 1));
-    if (!d_ix || !d_ixlen) return fail(ETL_ERR_ALLOC);
-  }
-  BloomChunk* d_bch = nullptr;
-  uint32_t* d_bwords = nullptr;
-  if (bloom_total) {
-    d_bch = (BloomChunk*)dalloc(sizeof(BloomChunk) * n_chunks);
-    d_bwords = (uint32_t*)dalloc(4 * bloom_words);
-    if (!d_bch || !d_bwords) return fail(ETL_ERR_ALLOC);
-  }
-  if (cudaMalloc(&dev, data_bound + bloom_total + index_bound + footer_bound + 64) != cudaSuccess) { dev = nullptr; return fail(ETL_ERR_ALLOC); }
-  std::vector<uint8_t> hmeta(meta_bytes);
-  {
-    std::vector<LeafMeta> dm = lm;
-    uint64_t o = lm_bytes;
-    for (uint32_t l = 0; l < nL; l++) {
-      memcpy(hmeta.data() + o, meta[l].name.data(), meta[l].name.size());
-      dm[l].name = d_meta + o;
-      o += meta[l].name.size();
-    }
-    memcpy(hmeta.data(), dm.data(), lm_bytes);
-    memcpy(hmeta.data() + o, created_by, cb_len);
-    memcpy(hmeta.data() + o + cb_len, prefix.data(), prefix.size());
-  }
-  const FooterArgs fa{(const LeafMeta*)d_meta, d_meta + meta_bytes - prefix.size(), d_meta + meta_bytes - prefix.size() - cb_len,
-                      nL, (uint32_t)prefix.size(), cb_len, cc};
-  uint64_t* uslot = d_scan; uint64_t* cslot = d_scan + (P + 1); uint64_t* fbase = d_scan + 2 * (P + 1); uint64_t* foff = d_scan + 3 * (P + 1);
-  CK(cudaMemcpyAsync(d_leaves, hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_pbase, page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_pbase + n_chunks + 1, leaf_page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_lbase, lscr_base.data(), 8 * (nL + 1ull), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_files, hf.data(), sizeof(FileRec) * K, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_meta, hmeta.data(), meta_bytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(d_bool, 0, bool_words * 4 + 8, st));
-  CK(cudaMemsetAsync(d_lscr, 0, lscr_base[nL] + 16, st));
-  CK(cudaMemsetAsync(foff + P, 0, 8, st));
-  if (bloom_total) {
-    CK(cudaMemcpyAsync(d_bch, hb.data(), sizeof(BloomChunk) * n_chunks, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(d_bwords, 0, 4 * bloom_words, st));
+  memcpy(hmeta.data(), dm.data(), lm_bytes);
+  memcpy(hmeta.data() + o, kCreatedBy, kCreatedByLen);
+  memcpy(hmeta.data() + o + kCreatedByLen, s.prefix.data(), s.prefix.size());
+  const FooterArgs fa{(const LeafMeta*)d_meta, d_meta + s.meta_bytes - s.prefix.size(), d_meta + s.meta_bytes - s.prefix.size() - kCreatedByLen,
+                      nL, (uint32_t)s.prefix.size(), kCreatedByLen, cc};
+  CK(cudaMemcpyAsync(d_leaves, s.hl.data(), sizeof(LeafDev) * nL, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_pbase, s.page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_lpbase, s.leaf_page_base.data(), 8 * (n_chunks + 1ull), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_lbase, s.lscr_base.data(), 8 * (nL + 1ull), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_files, s.hf.data(), sizeof(FileRec) * K, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_meta, hmeta.data(), s.meta_bytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(d_bool, 0, s.bool_words * 4 + 8, st));
+  CK(cudaMemsetAsync(d_lscr, 0, s.lscr_base[nL] + 16, st));
+  CK(cudaMemsetAsync(d_foff + P, 0, 8, st));
+  if (s.bloom_total) {
+    CK(cudaMemcpyAsync(d_bch, s.hb.data(), sizeof(BloomChunk) * n_chunks, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_bwords, 0, 4 * s.bloom_words, st));
   }
   const uint32_t kb = (uint32_t)((K + 1 + kFootWarps - 1) / kFootWarps);   // a warp per file (+ the scan's last entry)
+  const uint32_t xb = (n_chunks + kIdxWarps) / kIdxWarps;            // k_index: a warp per chunk
   if (P) {
-    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, d_rgb, n, E, NN, V, d_np, d_pbase, d_pbase + n_chunks + 1, d_lbase, d_pages, dict);
+    k_cut<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, nL, n_rg, row_begin, d_rgb, n, d_E, d_NN, d_V, d_np, d_pbase, d_lpbase, d_lbase, d_pages, dict);
     // payload slots: exclusive scan of the page bounds (and, with Snappy, of the fragment slots)
-    auto fill_scan = [&](int which, uint64_t* dst) {
+    auto fill_scan = [&](TotSlot which, uint64_t* dst) {
       k_fill<<<(uint32_t)((P + 256) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, which, cc, dst);
       k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)dst, (uint32_t)(P + 1), d_stot + which);
     };
-    fill_scan(0, uslot);
+    fill_scan(kTotUslot, d_uslot);
     if (d_dch) {
       // dictionaries: tables, inserts, first-occurrence flags and their scans, decisions, dictionary pages
-      k_dict_setup<<<(n_chunks + 256) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, d_rgb, n, NN, d_pbase, d_dch, d_tabn);
-      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_tabn, n_chunks + 1, d_stot + 4);
+      k_dict_setup<<<(n_chunks + 256) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, d_rgb, n, d_NN, d_pbase, d_dch, d_tabn);
+      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_tabn, n_chunks + 1, d_stot + kTotDict);
       k_dict_place<<<(n_chunks + 255) / 256, 256, 0, st>>>(n_chunks, d_tabn, d_dch);
-      CK(cudaMemsetAsync(d_tab, 0xff, 4 * d_slots, st));
+      CK(cudaMemsetAsync(d_tab, 0xff, 4 * s.d_slots, st));
       for (uint32_t l = 0; l < nL; l++) {
         if (!has_dict(l)) continue;
-        const uint64_t I = tot[l];
+        const uint64_t I = t.tot[l], at = s.hl[l].dscr;
         const uint32_t ib = (uint32_t)((I + 255) / 256);
         k_dict_insert<<<std::min<uint32_t>(kInsBlocks, ib), kInsThreads, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, d_dch, d_tab, d_dpos);
         const bool bytes = hl[l].atype == ETL_ARROW_UTF8 || hl[l].atype == ETL_ARROW_LARGE_BINARY;
         k_dict_mark<<<ib, 256, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, I, d_dch, d_tab, d_dpos, d_dflag, bytes ? d_desz : nullptr);
-        scan_lengths(d_dflag + hl[l].dscr, I, d_dblk, d_stot + 4, d_dfirst + hl[l].dscr, st);
-        if (bytes) scan_lengths(d_desz + hl[l].dscr, I, d_dblk, d_stot + 4, d_desum + hl[l].dscr, st);
+        scan_lengths(d_dflag + at, I, d_dblk, d_stot + kTotDict, d_dfirst + at, st);
+        if (bytes) scan_lengths(d_desz + at, I, d_dblk, d_stot + kTotDict, d_desum + at, st);
       }
       k_dict_finish<<<(n_chunks + 255) / 256, 256, 0, st>>>(d_leaves, nL, n_chunks, row_begin, d_dfirst, d_desum, d_dch, d_pages);
       for (uint32_t l = 0; l < nL; l++)
         if (has_dict(l))
-          k_dict_page<<<(uint32_t)((tot[l] + 255) / 256), 256, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, tot[l], d_dch, d_dfirst, d_desum, d_u, uslot);
+          k_dict_page<<<(uint32_t)((t.tot[l] + 255) / 256), 256, 0, st>>>(d_leaves, l, nL, n_rg, row_begin, t.tot[l], d_dch, d_dfirst, d_desum, d_u, d_uslot);
       const DictArgs da{d_dch, d_tab, d_dpos, d_dfirst, d_desz, d_dhead};
-      k_encode<true><<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, E, n, d_lscr, d_u, uslot, d_bool, da);
+      k_encode<true><<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, d_E, n, d_lscr, d_u, d_uslot, d_bool, da);
     } else {
-      k_encode<false><<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, E, n, d_lscr, d_u, uslot, d_bool, DictArgs{});
+      k_encode<false><<<(uint32_t)P, kEncThreads, 0, st>>>(d_leaves, d_pages, row_begin, d_E, n, d_lscr, d_u, d_uslot, d_bool, DictArgs{});
     }
     if (snappy) {
-      fill_scan(1, cslot);
-      fill_scan(2, fbase);
-      if (zstd) k_zstd<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz, d_zlit, d_zseq);
-      else k_snappy<<<(uint32_t)n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, fbase, d_u, uslot, d_c, cslot, d_fsz);
+      fill_scan(kTotCslot, d_cslot);
+      fill_scan(kTotFbase, d_fbase);
+      if (zstd) k_zstd<<<(uint32_t)s.n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, d_fbase, d_u, d_uslot, d_c, d_cslot, d_fsz, d_zlit, d_zseq);
+      else k_snappy<<<(uint32_t)s.n_frag_bound, 32, 0, st>>>(d_pages, (uint32_t)P, d_fbase, d_u, d_uslot, d_c, d_cslot, d_fsz);
     }
-    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, cc, fbase, d_fsz, foff, d_dch);
-    k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)foff, (uint32_t)(P + 1), d_stot + 3);
-    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, foff, d_rgf, d_files, d_bch, pidx, d_cout, d_dch);
+    k_page<<<(uint32_t)((P + 255) / 256), 256, 0, st>>>(d_pages, (uint32_t)P, cc, d_fbase, d_fsz, d_foff, d_dch);
+    k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)d_foff, (uint32_t)(P + 1), d_stot + kTotFoff);
+    k_chunk<<<(n_chunks + 63) / 64, 64, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_foff, d_rgf, d_files, d_bch, pidx, d_cout, d_dch);
     if (d_ix) {
       // page index: sizes and boundary orders, their places in each file behind its pages and filters
-      const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
-      k_index<false><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_rgb, d_rgf, d_files, d_fplace, foff, d_ix, d_ixlen, dev, d_cout);
-      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + 5);
-      k_index_place<<<(n_chunks + 63) / 64, 64, 0, st>>>(n_chunks, nL, d_rgf, d_files, foff, d_ix, d_ixlen, d_cout);
+      k_index<false><<<xb, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_rgb, d_rgf, d_files, d_fplace, d_foff, d_ix, d_ixlen, dev, d_cout);
+      k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>(d_ixlen, 2 * n_chunks + 1, d_stot + kTotIndex);
+      k_index_place<<<(n_chunks + 63) / 64, 64, 0, st>>>(n_chunks, nL, d_rgf, d_files, d_foff, d_ix, d_ixlen, d_cout);
     }
   }
   // every file's footer length and size, their scan (the files' places), then every byte at its place
-  k_footer<false><<<kb, 32 * kFootWarps, 0, st>>>(fa, K, d_rgb, d_files, foff, d_ixlen, d_cout, d_fplace, dev);
-  k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)d_fplace, (uint32_t)(K + 1), d_stot + 6);
+  k_footer<false><<<kb, 32 * kFootWarps, 0, st>>>(fa, K, d_rgb, d_files, d_foff, d_ixlen, d_cout, d_fplace, dev);
+  k_blk_scan<unsigned long long><<<1, 1024, 0, st>>>((unsigned long long*)d_fplace, (uint32_t)(K + 1), d_stot + kTotFiles);
   if (P) {
-    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, cc, foff, d_u, uslot, d_c, cslot, fbase, d_fsz, nL, d_rgf, d_files, d_fplace, dev);
-    if (bloom_total) {
+    k_gather<<<(uint32_t)P, 256, 0, st>>>(d_pages, cc, d_foff, d_u, d_uslot, d_c, d_cslot, d_fbase, d_fsz, nL, d_rgf, d_files, d_fplace, dev);
+    if (s.bloom_total) {
       // bloom filters: the bitsets in scratch, then headers and bitsets behind each file's pages
       for (uint32_t l = 0; l < nL; l++)
         if (bloomed(l))
-          k_bloom<<<std::min<uint32_t>(kInsBlocks, (uint32_t)((tot[l] + kInsThreads - 1) / kInsThreads) + 1), kInsThreads, 0, st>>>(
+          k_bloom<<<std::min<uint32_t>(kInsBlocks, (uint32_t)((t.tot[l] + kInsThreads - 1) / kInsThreads) + 1), kInsThreads, 0, st>>>(
               d_leaves, l, nL, n_rg, row_begin, d_rgb, d_bch, d_bwords);
       k_bloom_write<<<dim3(n_chunks, 16), 256, 0, st>>>(d_bch, d_bwords, nL, d_rgf, d_fplace, d_cout, dev);
     }
-    if (d_ix) {
-      const uint32_t ib = (n_chunks + kIdxWarps) / kIdxWarps;
-      k_index<true><<<ib, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_rgb, d_rgf, d_files, d_fplace, foff, d_ix, d_ixlen, dev, d_cout);
-    }
+    if (d_ix)
+      k_index<true><<<xb, 32 * kIdxWarps, 0, st>>>(d_leaves, d_pages, d_pbase, n_chunks, nL, d_rgb, d_rgf, d_files, d_fplace, d_foff, d_ix, d_ixlen, dev, d_cout);
   }
-  k_footer<true><<<kb, 32 * kFootWarps, 0, st>>>(fa, K, d_rgb, d_files, foff, d_ixlen, d_cout, d_fplace, dev);
+  k_footer<true><<<kb, 32 * kFootWarps, 0, st>>>(fa, K, d_rgb, d_files, d_foff, d_ixlen, d_cout, d_fplace, dev);
   k_leaf<<<(uint32_t)((K * nL + 63) / 64), 64, 0, st>>>(d_leaves, nL, K, n_chunks, d_files, d_cout, d_lout);
-  // SYNC 2: the files' places and every (file, leaf) record
+  return ETL_OK;
+}
+
+// Collect: SYNC 2 (the files' places and every (file, leaf) record), SYNC 3 with to_host (the pinned image) and the
+// metrics; the output moves to Fs
+int Call::collect(etl_parquet_files* Fs) {
   std::vector<ChunkOut> hlo(K * nL);
   CK(cudaMemcpyAsync(Fs->offs.data(), d_fplace, 8 * (K + 1), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(hlo.data(), d_lout, sizeof(ChunkOut) * K * nL, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (cudaGetLastError() != cudaSuccess) return fail(ETL_ERR_CUDA);
+  CK(cudaGetLastError());
   const uint64_t total = Fs->offs[K];
   if (to_host) {
-    if (cudaHostAlloc((void**)&host, total + 1, cudaHostAllocDefault) != cudaSuccess) { host = nullptr; return fail(ETL_ERR_ALLOC); }
+    if (cudaHostAlloc((void**)&host, total + 1, cudaHostAllocDefault) != cudaSuccess) { host = nullptr; return ETL_ERR_ALLOC; }
     CK(cudaMemcpyAsync(host, dev, total, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));                    // SYNC 3
+    CK(cudaStreamSynchronize(st));                  // SYNC 3
   }
-  for (void* p : pool) cudaFree(p);
   // metrics: one record per (file, leaf); their statistic bytes in one block
   uint64_t sb = 0;
   for (const ChunkOut& R : hlo) if (R.has) sb += R.min_len + R.max_len;
   Fs->stats.resize(sb);
   Fs->metrics.resize(K * nL);
   uint64_t so = 0;
-  for (uint64_t t = 0; t < K * nL; t++) {
-    const ChunkOut& R = hlo[t];
-    const uint32_t l = (uint32_t)(t % nL);
-    etl_parquet_metrics& M = Fs->metrics[t];
-    memset(&M, 0, sizeof M);
+  for (uint64_t i = 0; i < K * nL; i++) {
+    const ChunkOut& R = hlo[i];
+    const uint32_t l = (uint32_t)(i % nL);
+    etl_parquet_metrics& M = Fs->metrics[i];           // zeroed by resize
     M.field_id = hl[l].is_list ? fields[l].element_field_id : fields[l].field_id;
     M.flags = R.has ? ETL_PQ_HAS_MIN_MAX : 0;
     M.num_values = R.num_values; M.null_count = R.null_count; M.nan_count = R.nan_count;
@@ -1668,8 +1668,31 @@ int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const
     }
   }
   Fs->dev = dev; Fs->host = host;
+  dev = host = nullptr;
   return ETL_OK;
+}
 #undef CK
+
+// The writer: files k < K, file k the rows [ro[k], ro[k + 1]) of the emit, in one device buffer (and with to_host one
+// pinned image), packed in order.  etl_dec_parquet_write(_bloom) is K = 1.  Fs is filled on ETL_OK; on an error
+// everything the call allocated is freed (Fs owns nothing yet).
+int write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom, uint32_t n_fields,
+                const uint64_t* ro, uint64_t K, uint32_t codec, int to_host, etl_parquet_files* Fs) {
+  Call c{a, fields, bloom, n_fields, ro, K, codec, to_host};
+  int rc = c.describe();
+  if (rc != ETL_OK) return rc;
+  Fs->n_files = K; Fs->n_leaves = n_fields; Fs->offs.assign(K + 1, 0);
+  if (!K) return ETL_OK;
+  rc = c.plan();
+  if (rc == ETL_OK) {
+    for (uint32_t l = 0; l < n_fields; l++)           // RecordBatch::try_new fails before anything is written
+      if (c.t.req[l] != kNone) { Fs->null_column = l; Fs->null_row = c.t.req[l]; return ETL_OK; }
+    c.s = c.size();
+    rc = c.launch();
+    if (rc == ETL_OK) rc = c.collect(Fs);
+  }
+  if (rc != ETL_OK) cudaGetLastError();             // a failed call leaves no CUDA error behind for the next
+  return rc;
 }
 
 }  // namespace
@@ -1686,46 +1709,26 @@ int etl_dec_parquet_write_bloom(const etl_arrow_batch* a, const etl_parquet_fiel
                                 etl_parquet_file** out) {
   if (!out) return ETL_ERR_INVALID_ARG;
   const uint64_t ro[2] = {row_begin, row_end};
-  etl_parquet_files Fs;
-  const int rc = write_files(a, fields, bloom, n_fields, ro, 1, codec, to_host, &Fs);
-  if (rc != ETL_OK) return rc;
-  etl_parquet_file* Fo = new etl_parquet_file();
-  Fo->dev = Fs.dev; Fo->host = Fs.host; Fo->size = Fs.offs[1];
-  Fo->metrics = std::move(Fs.metrics);              // their min / max point into the moved block
-  Fo->stats = std::move(Fs.stats);
-  Fo->null_column = Fs.null_column; Fo->null_row = Fs.null_row;
-  *out = Fo;
-  return ETL_OK;
+  std::unique_ptr<etl_parquet_file> f(new etl_parquet_file());
+  const int rc = write_files(a, fields, bloom, n_fields, ro, 1, codec, to_host, f.get());
+  if (rc == ETL_OK) *out = f.release();
+  return rc;
 }
-uint64_t etl_dec_parquet_size(const etl_parquet_file* f) { return f ? f->size : 0; }
-const uint8_t* etl_dec_parquet_bytes(const etl_parquet_file* f, int host) { return f ? (host ? f->host : f->dev) : nullptr; }
-int etl_dec_parquet_metrics(const etl_parquet_file* f, uint32_t leaf, etl_parquet_metrics* out) {
-  if (!f || !out || leaf >= f->metrics.size()) return ETL_ERR_INVALID_ARG;
-  *out = f->metrics[leaf];
-  return ETL_OK;
-}
-int etl_dec_parquet_required_null(const etl_parquet_file* f, uint32_t* column, uint64_t* row) {
-  if (!f) return ETL_ERR_INVALID_ARG;
-  if (column) *column = f->null_column;
-  if (row) *row = f->null_row;
-  return ETL_OK;
-}
-void etl_dec_parquet_free(etl_parquet_file* f) {
-  if (!f) return;
-  if (f->dev) cudaFree(f->dev);
-  if (f->host) cudaFreeHost(f->host);
-  delete f;
-}
+// file 0 of its etl_parquet_files (offs[1]: its size, 0 after a required null)
+uint64_t etl_dec_parquet_size(const etl_parquet_file* f) { return f ? etl_dec_parquet_files_offsets(f)[1] : 0; }
+const uint8_t* etl_dec_parquet_bytes(const etl_parquet_file* f, int host) { return etl_dec_parquet_files_bytes(f, host); }
+int etl_dec_parquet_metrics(const etl_parquet_file* f, uint32_t leaf, etl_parquet_metrics* out) { return etl_dec_parquet_files_metrics(f, 0, leaf, out); }
+int etl_dec_parquet_required_null(const etl_parquet_file* f, uint32_t* column, uint64_t* row) { return etl_dec_parquet_files_required_null(f, column, row); }
+void etl_dec_parquet_free(etl_parquet_file* f) { delete f; }
 
 int etl_dec_parquet_write_files(const etl_arrow_batch* a, const etl_parquet_field* fields, const etl_parquet_bloom* bloom,
                                 uint32_t n_fields, const uint64_t* row_offsets, uint64_t n_files, uint32_t codec, int to_host,
                                 etl_parquet_files** out) {
   if (!out) return ETL_ERR_INVALID_ARG;
-  etl_parquet_files* Fs = new etl_parquet_files();
-  const int rc = write_files(a, fields, bloom, n_fields, row_offsets, n_files, codec, to_host, Fs);
-  if (rc != ETL_OK) { delete Fs; return rc; }
-  *out = Fs;
-  return ETL_OK;
+  std::unique_ptr<etl_parquet_files> Fs(new etl_parquet_files());
+  const int rc = write_files(a, fields, bloom, n_fields, row_offsets, n_files, codec, to_host, Fs.get());
+  if (rc == ETL_OK) *out = Fs.release();
+  return rc;
 }
 uint64_t etl_dec_parquet_files_count(const etl_parquet_files* fs) { return fs ? fs->n_files : 0; }
 const uint64_t* etl_dec_parquet_files_offsets(const etl_parquet_files* fs) { return fs ? fs->offs.data() : nullptr; }
@@ -1741,17 +1744,12 @@ int etl_dec_parquet_files_required_null(const etl_parquet_files* fs, uint32_t* c
   if (row) *row = fs->null_row;
   return ETL_OK;
 }
-void etl_dec_parquet_files_free(etl_parquet_files* fs) {
-  if (!fs) return;
-  if (fs->dev) cudaFree(fs->dev);
-  if (fs->host) cudaFreeHost(fs->host);
-  delete fs;
-}
+void etl_dec_parquet_files_free(etl_parquet_files* fs) { delete fs; }
 
 }  // extern "C"
 
 // ptxas -v, sm_90a, CUDA 12.9 (registers / shared memory / stack):
-//   k_plan 32 / 0 / 0      k_cut 53 / 0 / 0       k_encode<false> 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 10 / 0 / 0
+//   k_plan 32 / 0 / 0      k_cut 53 / 0 / 0       k_encode<false> 48 / 4176 B / 8 B (one 8-byte spill)    k_fill 16 / 0 / 0
 //   k_encode<true> 64 / 4200 B / 16 B (two 8-byte spills)
 //   k_snappy 50 / 8192 B / 0                      k_page 29 / 0 / 40 B (the header bytes)   k_gather 22 / 0 / 0 (+ a load
 //   of its file's place)
@@ -1762,7 +1760,7 @@ void etl_dec_parquet_files_free(etl_parquet_files* fs) {
 //   k_row_max 12 / 0 / 0   k_index<false> 89 / 0 / 40 B and k_index<true> 96 / 0 / 48 B (a fixed-width bound's bytes;
 //   no spills: __maxnreg__(96) instead of the launch bound, which left ptxas at 64 registers and spilling)
 //   k_index_place 30 / 0 / 0   k_footer<false> 96 / 0 / 40 B and k_footer<true> 96 / 0 / 40 B (the Thrift writer;
-//   __maxnreg__(96), as k_index: a 128-thread launch bound left them at 64 registers, one spilling)   k_fill 16 / 0 / 0
+//   __maxnreg__(96), as k_index: a 128-thread launch bound left them at 64 registers, one spilling)
 //   k_chunk_nn 14 / 0 / 0   k_bloom 55 / 0 / 0   k_bloom_write 29 / 0 / 40 B (the header's Thrift writer)
 //   the shared scans of emit_scan.cuh: k_len_blocks 22 / 256 B, k_blk_scan<unsigned long long> 32 / 8192 B,
-//   k_offsets<uint64_t> 18 / 8192 B
+//   k_offsets<uint64_t> 18 / 8192 B, k_copy_sel 12 / 0 / 0

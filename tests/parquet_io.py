@@ -1,6 +1,6 @@
-"""ctypes helpers around etl_dec_parquet_write shared by the GPU tests and tools/parquet_measure.py: the columns of an
-Arrow emit's host image as tests/parquet_ref.py columns, the field list the tests use, one write, the file bytes and the
-metrics."""
+"""ctypes helpers around the Parquet writer shared by the GPU tests and tools/parquet_measure.py: the columns of an
+Arrow emit's host image as tests/parquet_ref.py columns, the field list the tests use, the three write calls, the file
+bytes (from the host image or device memory) and the metrics."""
 import ctypes as C
 
 import numpy as np
@@ -60,14 +60,57 @@ def fields_for(cols, required=()):
              1 if (i >= n - 2 or i in required) else 0) for i in range(n)]
 
 
-def pq_write(lib, a, fields, rb, re, codec, to_host=1):
+def _arrays(fields, bloom):
+    """the etl_parquet_field array of fields [(name as str or bytes, field_id, element_field_id, required)] and the
+    etl_parquet_bloom array of bloom [(fpp, ndv, max_bytes)] (None: a NULL array)"""
     arr = (abi.ParquetField * max(1, len(fields)))()
-    names = [f[0].encode() if isinstance(f[0], str) else f[0] for f in fields]
-    for i, (f, nm) in enumerate(zip(fields, names)):
-        arr[i].name, arr[i].field_id, arr[i].element_field_id, arr[i].required = nm, f[1], f[2], f[3]
+    for i, f in enumerate(fields):
+        arr[i].name = f[0].encode() if isinstance(f[0], str) else f[0]
+        arr[i].field_id, arr[i].element_field_id, arr[i].required = f[1], f[2], f[3]
+    barr = None
+    if bloom is not None:
+        barr = (abi.ParquetBloom * max(1, len(bloom)))()
+        for i, (fpp, ndv, mb) in enumerate(bloom):
+            barr[i].fpp, barr[i].ndv, barr[i].max_bytes = fpp, ndv, mb
+    return arr, barr
+
+
+def pq_write(lib, a, fields, rb, re, codec, to_host=1):
+    arr, _ = _arrays(fields, None)
     h = C.c_void_p()
     rc = lib.etl_dec_parquet_write(a, arr, len(fields), rb, re, codec, to_host, C.byref(h))
     return rc, h
+
+
+def pq_write_bloom(lib, a, fields, bloom, rb, re, codec, to_host=1):
+    """etl_dec_parquet_write_bloom; bloom: [(fpp, ndv, max_bytes)] or None (a NULL array)"""
+    arr, barr = _arrays(fields, bloom)
+    h = C.c_void_p()
+    rc = lib.etl_dec_parquet_write_bloom(a, arr, barr, len(fields), rb, re, codec, to_host, C.byref(h))
+    return rc, h
+
+
+def write_files(lib, a, fields, bloom, ro, codec, to_host=1):
+    """etl_dec_parquet_write_files over row offsets ro (len(ro) - 1 files); bloom: [(fpp, ndv, max_bytes)] or None"""
+    arr, barr = _arrays(fields, bloom)
+    offs = (C.c_uint64 * max(1, len(ro)))(*[int(x) for x in ro])
+    h = C.c_void_p()
+    rc = lib.etl_dec_parquet_write_files(a, arr, barr, len(fields), offs, max(0, len(ro) - 1), codec, to_host, C.byref(h))
+    return rc, h
+
+
+def _cudart():
+    rt = C.CDLL("libcudart.so.12")
+    rt.cudaMemcpy.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]
+    return rt
+
+
+def device_bytes(ptr, n):
+    """n bytes of device memory at ptr"""
+    buf = C.create_string_buffer(max(1, n))
+    if n:
+        assert _cudart().cudaMemcpy(buf, ptr, n, 2) == 0                    # cudaMemcpyDeviceToHost
+    return buf.raw[:n]
 
 
 def file_bytes(lib, h):

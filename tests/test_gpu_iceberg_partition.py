@@ -17,12 +17,11 @@ import iceberg_partition_ref as P
 import parquet_index_ref as X
 import parquet_ref as R
 import scenarios as sc
-from parquet_io import emit_columns, fields_for, file_bytes, pq_write
+from parquet_io import emit_columns, fields_for, file_bytes, pq_write, pq_write_bloom
 from etl_b200 import abi, pgoutput as pg, workloads as wl
 from test_gpu_arrow_copy import copy_batch
 from test_gpu_copy import synth_rows
 from test_gpu_parquet import ERR_INVALID_ARG, INT4, TEXT, _decode_stream, _emit, _norm_ref, check_pyarrow, check_write
-from test_gpu_parquet_bloom import pq_write_bloom
 from test_gpu_rowbinary import hand_built
 
 pytestmark = pytest.mark.gpu

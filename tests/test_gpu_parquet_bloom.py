@@ -18,7 +18,7 @@ import parquet_bloom_ref as B
 import parquet_index_ref as X
 import parquet_ref as R
 import scenarios as sc
-from parquet_io import emit_columns, fields_for, file_bytes, metrics, pq_write
+from parquet_io import emit_columns, fields_for, file_bytes, metrics, pq_write, pq_write_bloom
 from etl_b200 import abi, pgoutput as pg, workloads as wl
 from test_gpu_arrow_copy import copy_batch
 from test_gpu_copy import synth_rows
@@ -39,22 +39,6 @@ def gpu():
         pytest.skip("no CUDA device")
     from etl_b200 import decoder
     return decoder
-
-
-def pq_write_bloom(lib, a, fields, bloom, rb, re, codec, to_host=1):
-    """etl_dec_parquet_write_bloom; bloom: [(fpp, ndv, max_bytes)] or None (a NULL array)"""
-    arr = (abi.ParquetField * max(1, len(fields)))()
-    names = [f[0].encode() for f in fields]
-    for i, (f, nm) in enumerate(zip(fields, names)):
-        arr[i].name, arr[i].field_id, arr[i].element_field_id, arr[i].required = nm, f[1], f[2], f[3]
-    barr = None
-    if bloom is not None:
-        barr = (abi.ParquetBloom * max(1, len(bloom)))()
-        for i, (fpp, ndv, mb) in enumerate(bloom):
-            barr[i].fpp, barr[i].ndv, barr[i].max_bytes = fpp, ndv, mb
-    h = C.c_void_p()
-    rc = lib.etl_dec_parquet_write_bloom(a, arr, barr, len(fields), rb, re, codec, to_host, C.byref(h))
-    return rc, h
 
 
 def _write(lib, a, fields, bloom, rb, re, codec):

@@ -13,13 +13,11 @@ import numpy as np
 import pytest
 
 import iceberg_partition_ref as P
-from parquet_io import emit_columns, fields_for, file_bytes, metrics
+from parquet_io import device_bytes, emit_columns, fields_for, file_bytes, metrics, pq_write_bloom, write_files
 from etl_b200 import abi, pgoutput as pg, workloads as wl
 from test_gpu_copy import synth_rows
 from test_gpu_iceberg_partition import EDGE_OIDS, _copy_emit, _edge_rows, _u64, partition
 from test_gpu_parquet import ERR_INVALID_ARG, _decode_stream, _emit
-from test_gpu_parquet_bloom import pq_write_bloom
-from test_gpu_parquet_zstd import _cudart
 from test_gpu_rowbinary import hand_built
 import scenarios as sc
 
@@ -39,23 +37,6 @@ def gpu():
     return decoder
 
 
-def write_files(lib, a, fields, bloom, ro, codec, to_host=1):
-    """etl_dec_parquet_write_files over row offsets ro (len(ro) - 1 files); bloom: [(fpp, ndv, max_bytes)] or None"""
-    arr = (abi.ParquetField * max(1, len(fields)))()
-    names = [f[0].encode() for f in fields]
-    for i, (f, nm) in enumerate(zip(fields, names)):
-        arr[i].name, arr[i].field_id, arr[i].element_field_id, arr[i].required = nm, f[1], f[2], f[3]
-    barr = None
-    if bloom is not None:
-        barr = (abi.ParquetBloom * max(1, len(bloom)))()
-        for i, (fpp, ndv, mb) in enumerate(bloom):
-            barr[i].fpp, barr[i].ndv, barr[i].max_bytes = fpp, ndv, mb
-    offs = (C.c_uint64 * max(1, len(ro)))(*[int(x) for x in ro])
-    h = C.c_void_p()
-    rc = lib.etl_dec_parquet_write_files(a, arr, barr, len(fields), offs, max(0, len(ro) - 1), codec, to_host, C.byref(h))
-    return rc, h
-
-
 def files_offsets(lib, h):
     k = lib.etl_dec_parquet_files_count(h)
     return _u64(lib.etl_dec_parquet_files_offsets(h), k + 1).tolist()
@@ -68,9 +49,7 @@ def files_image(lib, h, host=1):
         return b""
     if host:
         return bytes((C.c_uint8 * n).from_address(lib.etl_dec_parquet_files_bytes(h, 1)))
-    buf = (C.c_uint8 * n)()
-    assert _cudart().cudaMemcpy(buf, lib.etl_dec_parquet_files_bytes(h, 0), n, 2) == 0     # cudaMemcpyDeviceToHost
-    return bytes(buf)
+    return device_bytes(lib.etl_dec_parquet_files_bytes(h, 0), n)
 
 
 def files_metrics(lib, h, k, n_leaves):

@@ -18,12 +18,11 @@ import pytest
 import parquet_bloom_ref as B
 import parquet_index_ref as X
 import scenarios as sc
-from parquet_io import emit_columns, fields_for, file_bytes, metrics, pq_write
+from parquet_io import device_bytes, emit_columns, fields_for, file_bytes, metrics, pq_write, pq_write_bloom
 from etl_b200 import abi, pgoutput as pg, workloads as wl
 from test_gpu_arrow_copy import copy_batch
 from test_gpu_copy import synth_rows
 from test_gpu_parquet import ERR_INVALID_ARG, INT4, TEXT, _decode_stream, _emit, check_pyarrow
-from test_gpu_parquet_bloom import pq_write_bloom
 from test_gpu_rowbinary import hand_built
 from test_parquet_zstd_cpu import CODEC, FRAG, _build, walk, zstd
 
@@ -54,23 +53,13 @@ def host():
     return lib
 
 
-def _cudart():
-    rt = C.CDLL("libcudart.so.12")
-    rt.cudaMemcpy.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]
-    return rt
-
-
 def _write(lib, a, fields, rb, re, codec, bloom=None, to_host=1):
     rc, h = pq_write_bloom(lib, a, fields, bloom, rb, re, codec, to_host)
     assert rc == 0, hex(codec)
     if to_host:
         data = file_bytes(lib, h)
     else:                                                # the device copy
-        n = lib.etl_dec_parquet_size(h)
-        buf = C.create_string_buffer(max(1, n))
-        if n:
-            assert _cudart().cudaMemcpy(buf, lib.etl_dec_parquet_bytes(h, 0), n, 2) == 0   # cudaMemcpyDeviceToHost
-        data = buf.raw[:n]
+        data = device_bytes(lib.etl_dec_parquet_bytes(h, 0), lib.etl_dec_parquet_size(h))
     m = metrics(lib, h, len(fields))
     lib.etl_dec_parquet_free(h)
     return data, m
