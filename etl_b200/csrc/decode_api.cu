@@ -22,6 +22,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -169,11 +170,35 @@ NcclApi& nccl_api() {
   return api;
 }
 
-constexpr size_t kScalarWords = 16;
-// device scalar block: 16 words followed by the DevCarry
-//  [0] first_error key  [1..3] insert/update/delete bytes  [4] events  [5] heap_top  [7] long_count  [8] copy_count  [9] heap_overflow
-//  [10] arr_top  [11] perm_len  [12] n_act (k_act_scan)  [13] ABORT_* bits (k_chase, k_records)  [14] n_frames (k_chase)  [15] CTAs of k_chase that have published their state aggregate (shards)
+// The device scalar block: one 64-bit word per slot, then the DevCarry.  The host uploads it with the batch and reads
+// it back once after pass C.
+enum ScalarSlot : size_t {
+  kScFirstError,                                           // atomicMin key: rec_index << 24 | seq << 6 | code (~0: none)
+  kScInsertBytes, kScUpdateBytes, kScDeleteBytes, kScEvents,   // the metrics (P.metrics[0..3])
+  kScHeapTop,
+  kScUnused,                                               // not used
+  kScLongCount, kScCopyCount, kScHeapOverflow, kScArrTop, kScPermLen,
+  kScNAct,                                                 // live segments (k_act_scan)
+  kScAbort,                                                // ABORT_* bits (k_chase, k_records)
+  kScNFrames,                                              // frames of the batch (k_chase)
+  kScChaseDone,                                            // CTAs of k_chase that have published their state aggregate (shards)
+  kScalarWords,
+  // the slots from here on hold what the index pass left for pass C: a re-run of pass C (or decode_finish after
+  // decode_begin) resets only the ones before, and the abort bits on their own
+  kScIndexKept = kScNAct,
+};
 constexpr size_t kScalarBlockBytes = kScalarWords * 8 + sizeof(DevCarry);
+
+// points the scalar fields of P at their slots of the device block `sc`, and the carry at the DevCarry after them
+void bind_scalars(DecodeParams& P, unsigned long long* sc) {
+  P.first_error = sc + kScFirstError; P.metrics = sc + kScInsertBytes;
+  P.heap_top = sc + kScHeapTop; P.arr_top = sc + kScArrTop;
+  P.long_count = (unsigned int*)(sc + kScLongCount); P.copy_count = (unsigned int*)(sc + kScCopyCount);
+  P.heap_overflow = (unsigned int*)(sc + kScHeapOverflow); P.perm_len = (unsigned int*)(sc + kScPermLen);
+  P.n_act = (unsigned int*)(sc + kScNAct); P.abort_flag = (unsigned int*)(sc + kScAbort);
+  P.n_frames = (unsigned int*)(sc + kScNFrames); P.chase_done = (unsigned int*)(sc + kScChaseDone);
+  P.dc = reinterpret_cast<const DevCarry*>(sc + kScalarWords); P.dc_out = reinterpret_cast<DevCarry*>(sc + kScalarWords);
+}
 
 }  // namespace
 
@@ -211,7 +236,6 @@ struct etl_dec_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  bool lines_launched = false;
   std::string last_error;
   std::map<uint32_t, StoredTable> tables;
   std::map<uint32_t, RelVersion> current;  // SharedTableCache Ready state (table_cache.rs:36-130)
@@ -241,11 +265,10 @@ struct etl_dec_ctx {
   uint8_t* h_rel_x = nullptr; size_t h_rel_x_cap = 0; // pinned staging of the relation-update exchange
   uint64_t pending_h2d_bytes = 0;
   Summ* h_total = nullptr;               // pinned
-  unsigned long long* h_scalars = nullptr;  // pinned, kScalarWords + DevCarry
+  unsigned long long* h_scalars = nullptr;  // pinned, kScalarBlockBytes
   cudaEvent_t ev[6]{};
   cudaEvent_t evk[4]{};
-  cudaStream_t side = nullptr;           // k_utf8_dead runs here, underneath the tuple pass
-  cudaEvent_t ev_in = nullptr, ev_l0 = nullptr, ev_l1 = nullptr;
+  cudaEvent_t ev_l0 = nullptr, ev_l1 = nullptr;    // around k_utf8_dead (spans_ms)
   // decode in flight
   bool pending = false;
   DecodeParams P{};
@@ -391,10 +414,8 @@ static void ctx_release(etl_dec_ctx* ctx) {
   if (ctx->h_scalars) cudaFreeHost(ctx->h_scalars);
   for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
   for (auto& e : ctx->evk) if (e) cudaEventDestroy(e);
-  if (ctx->ev_in) cudaEventDestroy(ctx->ev_in);
   if (ctx->ev_l0) cudaEventDestroy(ctx->ev_l0);
   if (ctx->ev_l1) cudaEventDestroy(ctx->ev_l1);
-  if (ctx->side) cudaStreamDestroy(ctx->side);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->comm && nccl_api().ok) nccl_api().CommDestroy(ctx->comm);
   delete ctx;
@@ -407,16 +428,14 @@ int etl_dec_create(int device_id, etl_dec_ctx** out) {
   etl_dec_ctx* ctx = new etl_dec_ctx();
   ctx->device = device_id;
   bool ok = cudaSetDevice(device_id) == cudaSuccess;
-  // the latency-bound chain runs at the highest priority, the HBM-bound side pass at the lowest: when both have CTAs
-  // pending the scheduler places the chain's first
+  // the decode is a latency-bound chain of kernels: its stream runs at the highest priority, so that when other work on
+  // the device has CTAs pending the scheduler places the chain's first
   int prio_lo = 0, prio_hi = 0;
   ok = ok && cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi) == cudaSuccess;
   ok = ok && cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;
   ctx->own_stream = ok;
-  ok = ok && cudaStreamCreateWithPriority(&ctx->side, cudaStreamNonBlocking, prio_lo) == cudaSuccess;
   for (auto& e : ctx->ev) ok = ok && cudaEventCreate(&e) == cudaSuccess;
   for (auto& e : ctx->evk) ok = ok && cudaEventCreate(&e) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&ctx->ev_in, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaEventCreate(&ctx->ev_l0) == cudaSuccess && cudaEventCreate(&ctx->ev_l1) == cudaSuccess;
   ok = ok && cudaHostAlloc((void**)&ctx->h_total, sizeof(Summ), cudaHostAllocDefault) == cudaSuccess;
   ok = ok && cudaHostAlloc((void**)&ctx->h_scalars, kScalarBlockBytes, cudaHostAllocDefault) == cudaSuccess;
@@ -444,7 +463,6 @@ void etl_dec_destroy(etl_dec_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  cudaStreamSynchronize(ctx->side);
   if (trace_on() && ctx->tr_n)
     fprintf(stderr, "[etl trace] %llu decodes, mean us: prepare %.1f | enqueue %.1f | wait %.1f | results+d2h %.1f | summary %.1f\n",
             (unsigned long long)ctx->tr_n, ctx->tr[0] / ctx->tr_n, ctx->tr[1] / ctx->tr_n, ctx->tr[2] / ctx->tr_n, ctx->tr[3] / ctx->tr_n, ctx->tr[4] / ctx->tr_n);
@@ -594,22 +612,15 @@ void etl_dec_batch_free(etl_dec_batch* b) {
   free_batch_blocks(b);
   delete b;
 }
+// the owner of a batch under construction: an error return frees it (its planes on the context's stream)
+struct BatchFree { void operator()(etl_dec_batch* b) const { etl_dec_batch_free(b); } };
+using BatchPtr = std::unique_ptr<etl_dec_batch, BatchFree>;
 
-// Where the structure-blind UTF-8 pass (k_utf8_dead, HBM-bound) runs relative to the latency-bound passes.
-// 0: side stream from the start of the index pass; 1: side stream from the start of the tuple pass (default);
-// 2 (default): main stream after the tuple pass; 3: inside k_rows — its warps stream the dead segments after their rows.
-// Measured on C5 (10 GiB): 2 is the fastest, then 0, 1 and 3: k_rows fills the register file and
-// is bound by instruction issue, the UTF-8 pass needs every SM's warps to saturate HBM — sharing the SMs helps neither.
-// ETL_DEAD_MODE is a tuning knob for measurement, not part of the ABI.
-static int dead_mode() {
-  static const int m = getenv("ETL_DEAD_MODE") ? atoi(getenv("ETL_DEAD_MODE")) : 2;
-  return m;
-}
 // No frame of the batch can hold a text value of kCoopLen bytes (the stager's max_frame_len says so): k_rows lists no
 // long cell, and the passes that exist for them — the structure-blind UTF-8 pass over dead segments, k_long_cells, the
 // line bitmap — are left out.  The hint is not trusted: should k_rows list a long cell after all, run_decode runs them.
 static bool long_passes_skippable(const etl_dec_ctx* ctx) {
-  return ctx->max_frame_hint && ctx->max_frame_hint < (uint32_t)kCoopLen && dead_mode() == 2;
+  return ctx->max_frame_hint && ctx->max_frame_hint < (uint32_t)kCoopLen;
 }
 static uint32_t dead_grid(const DecodeParams& P) {   // 8 warps per CTA, kDeadSegsPerWarp segments per warp; surplus CTAs return at once
   const uint64_t items = (uint64_t)P.n_anchors * (P.anchor_stride > 2048u ? P.anchor_stride / 2048u : 1u);
@@ -620,16 +631,9 @@ static int sm_count(etl_dec_ctx* ctx) {
   if (!sms) { sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device); }
   return sms;
 }
-static cudaError_t launch_dead_side(etl_dec_ctx* ctx, cudaStream_t st) {
-  cudaError_t e;
-  if ((e = cudaEventRecord(ctx->ev_in, st)) != cudaSuccess) return e;
-  if ((e = cudaStreamWaitEvent(ctx->side, ctx->ev_in, 0)) != cudaSuccess) return e;
-  if ((e = cudaEventRecord(ctx->ev_l0, ctx->side)) != cudaSuccess) return e;
-  k_utf8_dead<<<dead_grid(ctx->P), 256, 0, ctx->side>>>(ctx->P);
-  if ((e = cudaEventRecord(ctx->ev_l1, ctx->side)) != cudaSuccess) return e;
-  ctx->launches += 1;
-  ctx->lines_launched = true;
-  return cudaSuccess;
+// k_utf8_dead's line bitmap starts out clear: one bit per 128-byte line, 32 lines per word
+static cudaError_t clear_line_bitmap(etl_dec_ctx* ctx) {
+  return cudaMemsetAsync(ctx->P.line_bad, 0, ((ctx->P.len + 4095) / 4096 + 1) * 4, ctx->stream);
 }
 
 static int ensure_pinned(etl_dec_ctx* ctx, uint8_t** p, size_t* cap, size_t want) {
@@ -840,15 +844,9 @@ static int prepare(etl_dec_ctx* ctx, const etl_dec_input* in, uint32_t flags, bo
   P.line_bad = ctx->d_line_bad.ptr(); P.dead = ctx->d_dead.ptr();
   P.long_cap = (uint32_t)(in->len / 512) + 16;        // every listed cell is at least kCoopLen (512) bytes long
   CK(ctx->d_long.ensure(P.long_cap));
-  unsigned long long* sc = reinterpret_cast<unsigned long long*>(ctx->d_scalars.ptr());
-  P.long_cells = ctx->d_long.ptr(); P.long_count = (unsigned int*)(sc + 7);
+  P.long_cells = ctx->d_long.ptr();
   P.total = ctx->d_total.ptr();
-  P.first_error = sc; P.metrics = sc + 1;
-  P.heap_top = sc + 5; P.heap_overflow = (unsigned int*)(sc + 9); P.arr_top = sc + 10;
-  P.perm_len = (unsigned int*)(sc + 11); P.n_act = (unsigned int*)(sc + 12); P.abort_flag = (unsigned int*)(sc + 13);
-  P.n_frames = (unsigned int*)(sc + 14); P.chase_done = (unsigned int*)(sc + 15);
-  P.copy_count = (unsigned int*)(sc + 8);
-  P.dc = reinterpret_cast<const DevCarry*>(sc + kScalarWords); P.dc_out = reinterpret_cast<DevCarry*>(sc + kScalarWords);
+  bind_scalars(P, reinterpret_cast<unsigned long long*>(ctx->d_scalars.ptr()));
   const uint32_t act_blocks = (P.n_anchors + kActThreads - 1) / kActThreads;
   CK(ctx->d_act.ensure(P.n_anchors + 1)); CK(ctx->d_act_blk.ensure(act_blocks + 1));
   P.act = ctx->d_act.ptr(); P.act_blk = ctx->d_act_blk.ptr();
@@ -857,17 +855,16 @@ static int prepare(etl_dec_ctx* ctx, const etl_dec_input* in, uint32_t flags, bo
     CK(ctx->d_seam.ensure(1 + (size_t)ctx->n_ranks));
     P.seam_send = ctx->d_seam.ptr(); P.seam_all = ctx->d_seam.ptr() + 1;
   }
-  if (!long_passes_skippable(ctx)) CK(cudaMemsetAsync(P.line_bad, 0, line_words * 4, st));
+  if (!long_passes_skippable(ctx)) CK(clear_line_bitmap(ctx));
   ctx->pending_schemas = std::move(vers);
-  ctx->lines_launched = false;
   return ETL_OK;
 }
 
-// scalars [lo, hi) ← initial values (+ the carry block when `with_carry`)
+// scalars [lo, hi) ← initial values (+ the rest of the block and the carry when `carry` is given)
 static int upload_scalars(etl_dec_ctx* ctx, size_t lo, size_t hi, const DevCarry* carry) {
   unsigned long long* h = ctx->h_scalars;
   for (size_t i = lo; i < hi; i++) h[i] = 0;
-  if (lo == 0) h[0] = ~0ull;
+  if (lo == kScFirstError) h[kScFirstError] = ~0ull;
   size_t bytes = (hi - lo) * 8;
   if (carry) { memcpy(h + kScalarWords, carry, sizeof *carry); bytes = (kScalarWords - lo) * 8 + sizeof *carry; }
   CK(cudaMemcpyAsync(ctx->d_scalars.ptr() + lo * 8, h + lo, bytes, cudaMemcpyHostToDevice, ctx->stream));
@@ -927,14 +924,13 @@ static int launch_index(etl_dec_ctx* ctx, bool exact) {
       k_act_scatter<<<act_blocks, kActThreads, 0, st>>>(P);
       ctx->launches += 3;
     }
-    if (dead_mode() == 0) CK(launch_dead_side(ctx, st));   // underneath everything that follows (needs only the dead-segment list)
     if (!exact) launch_chase(ctx, 3u, P.seam_send != nullptr);
     else {
       P.frame_cap = ~0ull;
       launch_chase(ctx, 1u);
-      CK(cudaMemcpyAsync(ctx->h_scalars + 14, ctx->d_scalars.ptr() + 14 * 8, 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(ctx->h_scalars + kScNFrames, ctx->d_scalars.ptr() + kScNFrames * 8, 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      if (int rc = ensure_record_scratch(ctx, (uint32_t)ctx->h_scalars[14])) return rc;
+      if (int rc = ensure_record_scratch(ctx, (uint32_t)ctx->h_scalars[kScNFrames])) return rc;
       launch_chase(ctx, 2u);
     }
     CK(cudaGetLastError());
@@ -965,29 +961,40 @@ static PlaneLayout plane_layout(uint64_t nr, uint64_t nc, uint64_t nh) {
   L.total = cur ? cur : 256;
   return L;
 }
-static void fill_planes(etl_dec_planes& pl, uint8_t* bs, const PlaneLayout& L, uint64_t nr, uint64_t nc, uint64_t nh) {
+// The planes of layout L in the block at `bs`.  A COPY batch (`copy`) has no record planes — the emitters tell it by
+// rec_kind == nullptr — and its rec_off is the row-offset plane, rec_cell_base.
+static void fill_planes(etl_dec_planes& pl, uint8_t* bs, const PlaneLayout& L, uint64_t nr, uint64_t nc, uint64_t nh, bool copy) {
+  pl = etl_dec_planes{};
   pl.n_records = nr; pl.n_cells = nc; pl.heap_bytes = nh;
+  pl.rec_cell_base = (uint64_t*)(bs + L.cbase);
+  pl.cell_tag = bs + L.tag; pl.cell_val = (uint64_t*)(bs + L.val); pl.cell_aux = (uint32_t*)(bs + L.aux); pl.heap = bs + L.heap;
+  if (copy) { pl.rec_off = pl.rec_cell_base; return; }
   pl.rec_off = (uint64_t*)(bs + L.rec_off); pl.rec_kind = bs + L.kind; pl.rec_flags = bs + L.flags;
   pl.rec_rel = (uint32_t*)(bs + L.rel); pl.rec_schema = (int32_t*)(bs + L.schema); pl.rec_start_lsn = (uint64_t*)(bs + L.start);
-  pl.rec_commit_lsn = (uint64_t*)(bs + L.commit); pl.rec_tx_ordinal = (uint64_t*)(bs + L.ord); pl.rec_cell_base = (uint64_t*)(bs + L.cbase);
+  pl.rec_commit_lsn = (uint64_t*)(bs + L.commit); pl.rec_tx_ordinal = (uint64_t*)(bs + L.ord);
   pl.rec_tuple_bytes = (uint32_t*)(bs + L.tb); pl.rec_heap_hint = (uint32_t*)(bs + L.hint);
-  pl.cell_tag = bs + L.tag; pl.cell_val = (uint64_t*)(bs + L.val); pl.cell_aux = (uint32_t*)(bs + L.aux); pl.heap = bs + L.heap;
 }
 
 // The kernels bump-allocate the scalar heap without checking its end (the bound is sized so that they cannot pass it);
 // a heap_top above the bound means cells point past what was reserved: an error, never a truncated result.
-static int check_scalar_heap(etl_dec_ctx* ctx, uint64_t scalar_heap) {
-  const uint64_t top = ctx->h_scalars[5];
-  if (top <= scalar_heap) return ETL_OK;
-  ctx->last_error = "scalar heap bound exceeded: the kernels allocated " + std::to_string(top) + " bytes of a " +
-                    std::to_string(scalar_heap) + "-byte scalar heap";
-  return ETL_ERR_CUDA;
+// Otherwise *used = the heap bytes the batch holds: the scalar region up to heap_top, or all of it and the array region
+// up to arr_top (the min only trims the 8-byte rounding of the last array reservation).
+static int measure_heap(etl_dec_ctx* ctx, uint64_t scalar_heap, uint64_t* used) {
+  const uint64_t top = ctx->h_scalars[kScHeapTop], arr_top = ctx->h_scalars[kScArrTop];
+  if (top > scalar_heap) {
+    ctx->last_error = "scalar heap bound exceeded: the kernels allocated " + std::to_string(top) + " bytes of a " +
+                      std::to_string(scalar_heap) + "-byte scalar heap";
+    return ETL_ERR_CUDA;
+  }
+  *used = std::min<uint64_t>(ctx->P.heap_cap, arr_top ? scalar_heap + arr_top : top);
+  return ETL_OK;
 }
 
 // ---------------------------------------------------------------- pass C into planes of capacity (cap_r, cap_c)
 // entries of the binned record order: the records plus at most 31 padding lanes per (tile, bin)
 static size_t perm_capacity(const DecodeParams& P) { return P.cap_records + 32ull * P.n_bin_tiles * P.n_bins + 256; }
-static int launch_emit(etl_dec_ctx* ctx, etl_dec_batch* b, uint64_t cap_r, uint64_t cap_c, uint64_t array_heap, PlaneLayout* Lout, uint64_t* scalar_heap_out) {
+// the planes of the batch (one stream-ordered allocation) and pass C's scratch, set in P
+static int reserve_planes(etl_dec_ctx* ctx, etl_dec_batch* b, uint64_t cap_r, uint64_t cap_c, uint64_t array_heap, PlaneLayout* Lout, uint64_t* scalar_heap_out) {
   DecodeParams& P = ctx->P;
   cudaStream_t st = ctx->stream;
   bool any_heap = false, any_array = false;
@@ -1006,7 +1013,7 @@ static int launch_emit(etl_dec_ctx* ctx, etl_dec_batch* b, uint64_t cap_r, uint6
   *Lout = L;
   b->block_bytes = L.total;
   CK(cudaMallocAsync(&b->dev_block, b->block_bytes, st));
-  fill_planes(b->dev, (uint8_t*)b->dev_block, L, cap_r, cap_c, nh);
+  fill_planes(b->dev, (uint8_t*)b->dev_block, L, cap_r, cap_c, nh, false);
   P.rec_off = (uint64_t*)b->dev.rec_off; P.rec_kind = (uint8_t*)b->dev.rec_kind; P.rec_flags = (uint8_t*)b->dev.rec_flags;
   P.rec_rel = (uint32_t*)b->dev.rec_rel; P.rec_schema = (int32_t*)b->dev.rec_schema; P.rec_start_lsn = (uint64_t*)b->dev.rec_start_lsn;
   P.rec_commit_lsn = (uint64_t*)b->dev.rec_commit_lsn; P.rec_tx_ordinal = (uint64_t*)b->dev.rec_tx_ordinal;
@@ -1038,8 +1045,6 @@ static int launch_emit_kernels(etl_dec_ctx* ctx) {
   if (P.n_anchors) {
     launch_records(ctx, true, cap_r);
     cudaEventRecord(ctx->evk[0], st);
-    if (dead_mode() == 1 && !ctx->lines_launched) CK(launch_dead_side(ctx, st));   // underneath the tuple pass
-    P.dead_in_rows = (dead_mode() == 3 && cap_r) ? 1u : 0u;
     if (cap_r) {
       k_bin_scan<<<1, 1024, 0, st>>>(P);
       k_perm<<<(uint32_t)((cap_r + kPermThreads - 1) / kPermThreads), kPermThreads, 0, st>>>(P);
@@ -1050,15 +1055,10 @@ static int launch_emit_kernels(etl_dec_ctx* ctx) {
       ctx->launches += 5;
     } else cudaEventRecord(ctx->evk[2], st);
     cudaEventRecord(ctx->evk[1], st);
-    if (ctx->lines_launched) CK(cudaStreamWaitEvent(st, ctx->ev_l1, 0));   // join: the bitmap is complete
-    else if (P.dead_in_rows) { cudaEventRecord(ctx->ev_l0, st); cudaEventRecord(ctx->ev_l1, st); }   // done by k_rows
-    else if (ctx->long_skipped) { cudaEventRecord(ctx->ev_l0, st); cudaEventRecord(ctx->ev_l1, st); }
-    else {                                            // ETL_DEAD_MODE=2 (or a batch without DML records): the same pass on the main stream
-      cudaEventRecord(ctx->ev_l0, st);
-      k_utf8_dead<<<dead_grid(P), 256, 0, st>>>(P);
-      cudaEventRecord(ctx->ev_l1, st);
-      ctx->launches += 1;
-    }
+    // the structure-blind UTF-8 pass after the tuple pass, on the same stream (DESIGN §3: measured the fastest place)
+    cudaEventRecord(ctx->ev_l0, st);
+    if (!ctx->long_skipped) { k_utf8_dead<<<dead_grid(P), 256, 0, st>>>(P); ctx->launches += 1; }
+    cudaEventRecord(ctx->ev_l1, st);
     cudaEventRecord(ctx->evk[3], st);
     if (cap_r && !ctx->long_skipped) { k_long_cells<<<sm_count(ctx) * 8, 256, 0, st>>>(P); ctx->launches += 1; }
     CK(cudaGetLastError());
@@ -1088,29 +1088,122 @@ static Summ carry_of(const etl_stream_state* cin) {
   return carry;
 }
 
-// one decode, common to every entry point.  mode 0: one-shot (optimistic sizing); 1: after decode_begin (totals known).
-// `sizing`: ETL_SIZING_* bits of an abandoned attempt (scratch restart), reported together with this one's
-static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64_t record_index_base, bool sharded, bool totals_known,
-                      etl_dec_batch** out, bool force_exact = false, uint32_t sizing = 0) {
+// the abort bits ← 0, on their own (the slots of the index pass stay)
+static cudaError_t reset_abort(etl_dec_ctx* ctx) {
+  ctx->h_scalars[kScAbort] = 0;
+  return cudaMemcpyAsync(ctx->d_scalars.ptr() + kScAbort * 8, ctx->h_scalars + kScAbort, 8, cudaMemcpyHostToDevice, ctx->stream);
+}
+
+// ---------------------------------------------------------------- the tail of every entry point
+// ETL_DECODE_RESULTS_TO_HOST: the final planes of `b` (device layout L) into the pinned host image, laid out for their
+// counts — one copy when the two layouts coincide up to the used heap, one per plane otherwise — and the last
+// synchronisation.  Without it only the last event, for the timings.
+static int stage_results(etl_dec_ctx* ctx, etl_dec_batch* b, const PlaneLayout& L, uint32_t flags, uint64_t* d2h) {
+  cudaStream_t st = ctx->stream;
+  if (!(flags & ETL_DECODE_RESULTS_TO_HOST)) {
+    if (!(flags & ETL_DECODE_NO_TIMING)) { CK(cudaEventRecord(ctx->ev[5], st)); CK(cudaEventSynchronize(ctx->ev[5])); }
+    return ETL_OK;
+  }
+  const uint64_t nr = b->dev.n_records, nc = b->dev.n_cells, nh = b->dev.heap_bytes;
+  const PlaneLayout H = plane_layout(nr, nc, nh);
+  if (ctx->h_result_cap < H.total) {
+    if (ctx->h_result) cudaFreeHost(ctx->h_result);
+    ctx->h_result = nullptr; ctx->h_result_cap = 0;
+    size_t want = H.total + H.total / 8;
+    CK(cudaHostAlloc(&ctx->h_result, want, cudaHostAllocDefault));
+    ctx->h_result_cap = want;
+  }
+  b->host_block = ctx->h_result;
+  uint8_t* hb = (uint8_t*)b->host_block;
+  const uint8_t* db = (const uint8_t*)b->dev_block;
+  if (!b->copy && L.rec_off == H.rec_off && L.heap + nh <= H.total && L.tag == H.tag && L.heap == H.heap) {
+    CK(cudaMemcpyAsync(hb, db, H.heap + nh, cudaMemcpyDeviceToHost, st));
+    *d2h += H.heap + nh;
+  } else {
+    const uint64_t rn = b->copy ? 0 : nr;   // a COPY batch has no record planes, only its row offsets (rec_cell_base)
+    auto cp = [&](uint64_t ho, uint64_t dof, uint64_t bytes) { if (bytes) cudaMemcpyAsync(hb + ho, db + dof, bytes, cudaMemcpyDeviceToHost, st); *d2h += bytes; };
+    cp(H.rec_off, L.rec_off, rn * 8); cp(H.kind, L.kind, rn); cp(H.flags, L.flags, rn); cp(H.rel, L.rel, rn * 4); cp(H.schema, L.schema, rn * 4);
+    cp(H.start, L.start, rn * 8); cp(H.commit, L.commit, rn * 8); cp(H.ord, L.ord, rn * 8); cp(H.cbase, L.cbase, (nr + 1) * 8);
+    cp(H.tb, L.tb, rn * 4); cp(H.hint, L.hint, rn * 4); cp(H.tag, L.tag, nc); cp(H.val, L.val, nc * 8); cp(H.aux, L.aux, nc * 4); cp(H.heap, L.heap, nh);
+    CK(cudaGetLastError());
+  }
+  fill_planes(b->host, hb, H, nr, nc, nh, b->copy);
+  b->has_host = true;
+  CK(cudaEventRecord(ctx->ev[5], st));
+  CK(cudaStreamSynchronize(st));
+  return ETL_OK;
+}
+// The summary fields every entry point fills alike.  Events: ev[0] → ev[1] uploads, ev[1] → ev[2] index pass,
+// ev[3] → ev[4] pass C, ev[4] → ev[5] the copies to the host.
+static void fill_summary(etl_dec_ctx* ctx, etl_dec_batch* b, uint32_t flags, uint64_t h2d, uint64_t d2h, uint32_t sizing) {
+  etl_dec_summary& S = b->summary;
+  memset(&S, 0, sizeof S);
+  if (!(flags & ETL_DECODE_NO_TIMING)) {          // ten event queries: host time an 8 MiB batch notices
+    cudaEventElapsedTime(&S.h2d_ms, ctx->ev[0], ctx->ev[1]);
+    cudaEventElapsedTime(&S.index_ms, ctx->ev[1], ctx->ev[2]);
+    cudaEventElapsedTime(&S.emit_ms, ctx->ev[3], ctx->ev[4]);
+    cudaEventElapsedTime(&S.d2h_ms, ctx->ev[4], ctx->ev[5]);
+    if (flags & ETL_DECODE_RESULTS_TO_HOST) { float whole = 0; cudaEventElapsedTime(&whole, ctx->ev[3], ctx->ev[5]); S.emit_ms = whole - S.d2h_ms; }
+    if (ctx->P.n_anchors) {
+      cudaEventElapsedTime(&S.frames_ms, ctx->ev[3], ctx->evk[0]);
+      cudaEventElapsedTime(&S.walk_ms, ctx->evk[0], ctx->evk[2]);    // k_bin_scan + k_perm
+      cudaEventElapsedTime(&S.cells_ms, ctx->evk[2], ctx->evk[1]);   // k_rows
+      cudaEventElapsedTime(&S.spans_ms, ctx->ev_l0, ctx->ev_l1);     // k_utf8_dead
+      cudaEventElapsedTime(&S.long_ms, ctx->evk[3], ctx->ev[4]);     // k_long_cells
+    }
+  }
+  S.kernel_ms = S.index_ms + S.emit_ms;
+  S.h2d_bytes = h2d;
+  S.d2h_bytes = d2h;
+  S.gpu_launches = ctx->launches;
+  S.abi_version = ETL_DECODE_ABI_VERSION;
+  S.sizing = sizing;
+  const unsigned long long key = ctx->h_scalars[kScFirstError];
+  if (key == ~0ull) S.first_error.record_index = UINT64_MAX;
+  else {
+    S.first_error.record_index = key >> 24;  // global index
+    S.first_error.seq = (uint32_t)((key >> 6) & 0x3FFFFu);
+    S.first_error.code = (uint32_t)(key & 63u);
+    S.first_error.kind = error_kind_of(S.first_error.code);
+  }
+}
+
+// ---------------------------------------------------------------- one decode of the replication stream
+// One decode after prepare(), common to every entry point.  Its stages share this record, which owns the batch until
+// run_decode hands it out.  totals_known: after decode_begin (the index pass ran and its totals are on the host).
+struct Decode {
+  etl_dec_ctx* ctx;
+  const etl_stream_state* carry_in;
+  uint64_t record_index_base;
+  bool sharded, totals_known;
+  bool force_exact;               // after a scratch restart: no optimistic sizes
+  uint32_t sizing;                // ETL_SIZING_* bits, those of an abandoned attempt included
+  BatchPtr b;
+  Summ host_carry;
+  bool exact, restart;            // restart: the offset scratch overflowed, start over on the exact path
+  PlaneLayout L;                  // of the device planes
+  uint64_t scalar_heap;
+  std::vector<SeamBlock> seams;   // sharded: every rank's totals (read back after the first pass)
+  int size(); int pass_c(); void summarise(uint64_t d2h); int note_ready();   // the stages
+};
+
+// Initial sizing: a new batch, the scalars and the carry, then the index pass.  Optimistic (sizes from what earlier
+// batches needed per byte): the planes and the offset scratch first, then the pipeline without a host round trip.
+// Exact (the first batch of a context, or after a scratch restart): the index pass, then its totals read back.
+// After decode_begin the totals are on the host already: only the scalars are reset.
+int Decode::size() {
   cudaStream_t st = ctx->stream;
   DecodeParams& P = ctx->P;
-  etl_dec_batch* b = new etl_dec_batch();
+  b.reset(new etl_dec_batch());
   b->ctx = ctx;
   b->schemas = ctx->pending_schemas;
-  auto fail = [&](int rc) { if (b->dev_block) cudaFreeAsync(b->dev_block, st); delete b; return rc; };
-#define CKB(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { ctx->last_error = std::string(#call) + ": " + cudaGetErrorString(_e); return fail(ETL_ERR_CUDA); } } while (0)
-  const Summ host_carry = carry_of(carry_in);
+  host_carry = carry_of(carry_in);
   P.host_carry = host_carry;
   DevCarry dc; dc.carry = host_carry; dc.record_index_base = record_index_base;
-  auto reset_abort = [&]() -> cudaError_t {
-    ctx->h_scalars[13] = 0;
-    return cudaMemcpyAsync(ctx->d_scalars.ptr() + 13 * 8, ctx->h_scalars + 13, 8, cudaMemcpyHostToDevice, st);
-  };
-
   uint64_t cap_r = 0, cap_c = 0;
-  bool exact = totals_known;
+  exact = totals_known;
   if (!totals_known) {
-    if (int rc = upload_scalars(ctx, 0, kScalarWords, &dc)) return fail(rc);
+    if (int rc = upload_scalars(ctx, 0, kScalarWords, &dc)) return rc;
     // optimistic sizes from what earlier batches needed per byte; the first batch has no history: exact path
     if (ctx->rec_per_byte > 0 && !force_exact) {
       cap_r = (uint64_t)(P.len * ctx->rec_per_byte * 1.08) + 4096;
@@ -1119,213 +1212,169 @@ static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64
     P.cap_records = exact ? ~0ull : cap_r; P.cap_cells = exact ? ~0ull : cap_c;   // k_chase / k_records decide with these
     P.rec_cell_base = nullptr;
   } else {
-    if (int rc = upload_scalars(ctx, 0, 12, nullptr)) return fail(rc);           // [12] n_act, [14] n_frames survive from decode_begin
-    CKB(reset_abort());
+    if (int rc = upload_scalars(ctx, 0, kScIndexKept, nullptr)) return rc;
+    CK(reset_abort(ctx));
     memcpy(ctx->h_scalars + kScalarWords, &dc, sizeof dc);
-    CKB(cudaMemcpyAsync(ctx->d_scalars.ptr() + kScalarWords * 8, ctx->h_scalars + kScalarWords, sizeof dc, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->d_scalars.ptr() + kScalarWords * 8, ctx->h_scalars + kScalarWords, sizeof dc, cudaMemcpyHostToDevice, st));
   }
   sizing |= exact ? ETL_SIZING_EXACT : ETL_SIZING_OPTIMISTIC;
-  PlaneLayout L{};
-  uint64_t scalar_heap = 0, array_heap = 0, heap_used = 0;
   if (!totals_known && !exact) {
-    // planes and offset scratch first, then the whole pipeline without a host round trip.  The scratch is cheap
-    // (8 bytes per frame): twice the expected count, so that only the planes can realistically be too small.
-    if (int rc = launch_emit(ctx, b, cap_r, cap_c, 0, &L, &scalar_heap)) return fail(rc);
-    if (int rc = ensure_record_scratch(ctx, 2 * cap_r + 65536)) return fail(rc);
-    if (int rc = launch_index(ctx, false)) return fail(rc);
-    if (sharded && !P.n_anchors) { if (int rc = launch_summary(ctx)) return fail(rc); }   // (an empty range: the identity seam; otherwise k_chase wrote the seam block)
+    // The offset scratch is cheap (8 bytes per frame): twice the expected count, so that only the planes can
+    // realistically be too small.
+    if (int rc = reserve_planes(ctx, b.get(), cap_r, cap_c, 0, &L, &scalar_heap)) return rc;
+    if (int rc = ensure_record_scratch(ctx, 2 * cap_r + 65536)) return rc;
+    if (int rc = launch_index(ctx, false)) return rc;
+    if (sharded && !P.n_anchors) { if (int rc = launch_summary(ctx)) return rc; }   // (an empty range: the identity seam; otherwise k_chase wrote the seam block)
   } else if (!totals_known) {
-    if (int rc = launch_index(ctx, true)) return fail(rc);
-    if (int rc = launch_summary(ctx)) return fail(rc);
-    if (!sharded) {
-      CKB(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
-      CKB(cudaStreamSynchronize(st));
-    }
+    if (int rc = launch_index(ctx, true)) return rc;
+    if (int rc = launch_summary(ctx)) return rc;
   }
   if (sharded) {
-    if (int rc = ctx_allgather(ctx, P.seam_send, (void*)P.seam_all, sizeof(SeamBlock))) return fail(rc);
+    if (int rc = ctx_allgather(ctx, P.seam_send, (void*)P.seam_all, sizeof(SeamBlock))) return rc;
     k_seam_fold<<<1, 32, 0, st>>>(P);
     ctx->launches += 2;
-    if (exact && !totals_known) {
-      CKB(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
-      CKB(cudaStreamSynchronize(st));
-    }
   }
-  std::vector<SeamBlock> seams;                        // sharded: every rank's totals (read back after the first pass)
+  if (exact && !totals_known) {
+    CK(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  return ETL_OK;
+}
+
+// Pass C into the planes, and its re-runs: at the exact sizes when the optimistic planes were too small, with a larger
+// array region when an array reservation did not fit.  Sets `restart` when the offset scratch overflowed.
+int Decode::pass_c() {
+  cudaStream_t st = ctx->stream;
+  DecodeParams& P = ctx->P;
+  uint64_t array_heap = 0;
   for (int attempt = 0;; attempt++) {
     if (exact) {
       const Summ T = *ctx->h_total;
-      if (b->dev_block) { CKB(cudaFreeAsync(b->dev_block, st)); b->dev_block = nullptr; }
-      if (int rc = launch_emit(ctx, b, T.n_rec, T.n_cells, array_heap, &L, &scalar_heap)) return fail(rc);
+      if (b->dev_block) { CK(cudaFreeAsync(b->dev_block, st)); b->dev_block = nullptr; }
+      if (int rc = reserve_planes(ctx, b.get(), T.n_rec, T.n_cells, array_heap, &L, &scalar_heap)) return rc;
       if (attempt > 0 || totals_known) {              // a re-run of pass C: fresh scalars, the carry block stays
-        if (int rc = upload_scalars(ctx, 0, 12, nullptr)) return fail(rc);
-        CKB(reset_abort());
+        if (int rc = upload_scalars(ctx, 0, kScIndexKept, nullptr)) return rc;
+        CK(reset_abort(ctx));
       }
     }
-    if (int rc = launch_emit_kernels(ctx)) return fail(rc);
+    if (int rc = launch_emit_kernels(ctx)) return rc;
     TRACE_MARK(1);
-    CKB(cudaStreamSynchronize(st));
+    CK(cudaStreamSynchronize(st));
     TRACE_MARK(2);
     if (sharded && seams.empty()) {
       seams.resize(ctx->n_ranks);
       memcpy(seams.data(), ctx->h_seam, sizeof(SeamBlock) * ctx->n_ranks);   // copied with the scalars, before the sync
     }
-    if (ctx->long_skipped && ctx->h_scalars[7] && !ctx->h_scalars[13]) {
+    if (ctx->long_skipped && ctx->h_scalars[kScLongCount] && !ctx->h_scalars[kScAbort]) {
       // the frame-length hint was wrong: long values exist.  Run the passes that were left out, read the scalars again.
       ctx->long_skipped = false;
       sizing |= ETL_SIZING_LONG_PASSES_LATE;
-      CKB(cudaMemsetAsync(P.line_bad, 0, ((P.len + 4095) / 4096 + 1) * 4, st));
+      CK(clear_line_bitmap(ctx));
       k_utf8_dead<<<dead_grid(P), 256, 0, st>>>(P);
       k_long_cells<<<sm_count(ctx) * 8, 256, 0, st>>>(P);
       ctx->launches += 2;
-      CKB(cudaGetLastError());
-      CKB(cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars.ptr(), kScalarWords * 8, cudaMemcpyDeviceToHost, st));
-      CKB(cudaStreamSynchronize(st));
+      CK(cudaGetLastError());
+      CK(cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars.ptr(), kScalarWords * 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
     }
-    const uint32_t aborted = (uint32_t)ctx->h_scalars[13];
+    const uint32_t aborted = (uint32_t)ctx->h_scalars[kScAbort];
     bool scratch_short = (aborted & ABORT_SCRATCH) != 0;
     for (const SeamBlock& sb : seams) scratch_short = scratch_short || (sb.total.flags & 0x80000000u);   // some rank could not form its totals
-    if (scratch_short) {
-      // more frames than the offset scratch holds (2x what earlier batches needed): start over on the exact path.
-      // Sharded: every rank sees the same gathered blocks, so every rank takes this branch and the exchange is repeated.
-      if (force_exact) { ctx->last_error = "offset scratch overflow on the exact path"; return fail(ETL_ERR_CUDA); }
-      fail(0);
-      return run_decode(ctx, carry_in, record_index_base, sharded, false, out, true, sizing | ETL_SIZING_SCRATCH_RESTART);
-    }
+    if (scratch_short) { restart = true; return ETL_OK; }
     if (aborted) {                                     // did not fit the optimistic planes: exact sizes, pass C again
       sizing |= ((aborted & ABORT_RECORDS) ? ETL_SIZING_RERUN_RECORDS : 0u) | ((aborted & ABORT_CELLS) ? ETL_SIZING_RERUN_CELLS : 0u);
-      CKB(reset_abort());
-      if (int rc = launch_summary(ctx)) return fail(rc);
-      CKB(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
-      CKB(cudaStreamSynchronize(st));
+      CK(reset_abort(ctx));
+      if (int rc = launch_summary(ctx)) return rc;
+      CK(cudaMemcpyAsync(ctx->h_total, P.total, sizeof(Summ), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
       exact = true;
-      ctx->lines_launched = false;
-      CKB(cudaMemsetAsync(P.line_bad, 0, ((P.len + 4095) / 4096 + 1) * 4, st));
+      CK(clear_line_bitmap(ctx));
       continue;
     }
-    const Summ T = *ctx->h_total;
-    if (int rc = check_scalar_heap(ctx, scalar_heap)) return fail(rc);
-    // (the min only trims the 8-byte rounding of the last array reservation: the scalar region was checked above)
-    heap_used = P.heap_cap;
-    if (P.heap_cap) heap_used = std::min<uint64_t>(P.heap_cap, ctx->h_scalars[10] ? scalar_heap + ctx->h_scalars[10] : ctx->h_scalars[5]);
-    if (ctx->h_scalars[9]) {                          // an array reservation did not fit: larger array region, pass C again
-      if (attempt >= 4) { ctx->last_error = "array heap reservation overflow after retries"; return fail(ETL_ERR_CUDA); }
+    uint64_t heap_used = 0;
+    if (int rc = measure_heap(ctx, scalar_heap, &heap_used)) return rc;
+    if (ctx->h_scalars[kScHeapOverflow]) {            // an array reservation did not fit: larger array region, pass C again
+      if (attempt >= 4) { ctx->last_error = "array heap reservation overflow after retries"; return ETL_ERR_CUDA; }
       array_heap = (P.heap_cap - scalar_heap) * 4;
       sizing |= ETL_SIZING_ARRAY_HEAP_RETRY;
       exact = true;
-      ctx->lines_launched = false;
-      CKB(cudaMemsetAsync(P.line_bad, 0, ((P.len + 4095) / 4096 + 1) * 4, st));
+      CK(clear_line_bitmap(ctx));
       continue;
     }
     // the planes describe exactly the batch
+    const Summ T = *ctx->h_total;
     b->dev.n_records = T.n_rec; b->dev.n_cells = T.n_cells; b->dev.heap_bytes = heap_used;
-    break;
+    return ETL_OK;
   }
-  const Summ T = *ctx->h_total;
-  if (P.len) { ctx->rec_per_byte = std::max(ctx->rec_per_byte * 0.97, (double)T.n_rec / P.len); ctx->cells_per_byte = std::max(ctx->cells_per_byte * 0.97, (double)T.n_cells / P.len); }
+}
 
-  uint64_t d2h_bytes = kScalarWords * 8 + sizeof(Summ);
-  if (ctx->pending_flags & ETL_DECODE_RESULTS_TO_HOST) {
-    // compact host image: planes laid out for the exact counts; one copy per plane, one synchronisation
-    const uint64_t nr = T.n_rec, nc = T.n_cells;
-    const PlaneLayout H = plane_layout(nr, nc, heap_used);
-    if (ctx->h_result_cap < H.total) {
-      if (ctx->h_result) cudaFreeHost(ctx->h_result);
-      ctx->h_result = nullptr; ctx->h_result_cap = 0;
-      size_t want = H.total + H.total / 8;
-      CKB(cudaHostAlloc(&ctx->h_result, want, cudaHostAllocDefault));
-      ctx->h_result_cap = want;
-    }
-    b->host_block = ctx->h_result;
-    uint8_t* hb = (uint8_t*)b->host_block;
-    const uint8_t* db = (const uint8_t*)b->dev_block;
-    CKB(cudaEventRecord(ctx->ev[4], st));
-    if (L.rec_off == H.rec_off && L.heap + heap_used <= H.total && L.tag == H.tag && L.heap == H.heap) {
-      CKB(cudaMemcpyAsync(hb, db, H.heap + heap_used, cudaMemcpyDeviceToHost, st));
-      d2h_bytes += H.heap + heap_used;
-    } else {
-      auto cp = [&](uint64_t ho, uint64_t dof, uint64_t bytes) { if (bytes) cudaMemcpyAsync(hb + ho, db + dof, bytes, cudaMemcpyDeviceToHost, st); d2h_bytes += bytes; };
-      cp(H.rec_off, L.rec_off, nr * 8); cp(H.kind, L.kind, nr); cp(H.flags, L.flags, nr); cp(H.rel, L.rel, nr * 4); cp(H.schema, L.schema, nr * 4);
-      cp(H.start, L.start, nr * 8); cp(H.commit, L.commit, nr * 8); cp(H.ord, L.ord, nr * 8); cp(H.cbase, L.cbase, (nr + 1) * 8);
-      cp(H.tb, L.tb, nr * 4); cp(H.hint, L.hint, nr * 4); cp(H.tag, L.tag, nc); cp(H.val, L.val, nc * 8); cp(H.aux, L.aux, nc * 4); cp(H.heap, L.heap, heap_used);
-      CKB(cudaGetLastError());
-    }
-    fill_planes(b->host, hb, H, nr, nc, heap_used);
-    b->has_host = true;
-    CKB(cudaEventRecord(ctx->ev[5], st));
-    CKB(cudaStreamSynchronize(st));
-  } else if (!(ctx->pending_flags & ETL_DECODE_NO_TIMING)) { CKB(cudaEventRecord(ctx->ev[5], st)); CKB(cudaEventSynchronize(ctx->ev[5])); }
-
-  TRACE_MARK(3);
-  // ---- summary
+// the summary fields of a replication batch: metrics, carry-out and the index of its first record
+void Decode::summarise(uint64_t d2h) {
+  const DecodeParams& P = ctx->P;
+  fill_summary(ctx, b.get(), ctx->pending_flags, ctx->pending_h2d_bytes, d2h, sizing);
   etl_dec_summary& S = b->summary;
-  memset(&S, 0, sizeof S);
-  float h2d_ms = 0, index_ms = 0, emit_ms = 0, d2h_ms = 0;
-  if (!(ctx->pending_flags & ETL_DECODE_NO_TIMING)) {          // ten event queries: host time an 8 MiB batch notices
-    cudaEventElapsedTime(&h2d_ms, ctx->ev[0], ctx->ev[1]);
-    cudaEventElapsedTime(&index_ms, ctx->ev[1], ctx->ev[2]);
-    cudaEventElapsedTime(&emit_ms, ctx->ev[3], ctx->ev[4]);
-    cudaEventElapsedTime(&d2h_ms, ctx->ev[4], ctx->ev[5]);
-    if (ctx->pending_flags & ETL_DECODE_RESULTS_TO_HOST) { float whole = 0; cudaEventElapsedTime(&whole, ctx->ev[3], ctx->ev[5]); emit_ms = whole - d2h_ms; }
-    if (P.n_anchors) {
-      cudaEventElapsedTime(&S.frames_ms, ctx->ev[3], ctx->evk[0]);
-      cudaEventElapsedTime(&S.walk_ms, ctx->evk[0], ctx->evk[2]);    // k_bin_scan + k_perm
-      cudaEventElapsedTime(&S.cells_ms, ctx->evk[2], ctx->evk[1]);   // k_rows
-      cudaEventElapsedTime(&S.spans_ms, ctx->ev_l0, ctx->ev_l1);     // k_utf8_dead
-      cudaEventElapsedTime(&S.long_ms, ctx->evk[3], ctx->ev[4]);     // k_long_cells
-    }
-  }
-  S.kernel_ms = index_ms + emit_ms;
-  S.index_ms = index_ms; S.emit_ms = emit_ms;
-  S.h2d_ms = h2d_ms; S.d2h_ms = d2h_ms;
-  S.h2d_bytes = ctx->pending_h2d_bytes;
-  // bytes k_utf8_dead streamed: the dead segments (h_scalars[12] = live segment count, left by k_act_scan)
-  S.span_bytes = P.n_anchors ? std::min<uint64_t>(P.len, (uint64_t)(P.n_anchors - (uint32_t)ctx->h_scalars[12]) * P.anchor_stride) : 0;
-  S.d2h_bytes = d2h_bytes;
-  S.gpu_launches = ctx->launches;
+  // bytes k_utf8_dead streamed: the dead segments (n_act = live segment count, left by k_act_scan)
+  S.span_bytes = P.n_anchors ? std::min<uint64_t>(P.len, (uint64_t)(P.n_anchors - (uint32_t)ctx->h_scalars[kScNAct]) * P.anchor_stride) : 0;
   S.n_schemas = (uint32_t)b->schemas.size();
-  unsigned long long key = ctx->h_scalars[0];
-  uint64_t err_off = ~0ull;
-  if (key == ~0ull) { S.first_error.record_index = UINT64_MAX; }
-  else {
-    S.first_error.record_index = key >> 24;  // global index
-    S.first_error.seq = (uint32_t)((key >> 6) & 0x3FFFFu);
-    S.first_error.code = (uint32_t)(key & 63u);
-    S.first_error.kind = error_kind_of(S.first_error.code);
-  }
-  S.insert_bytes = ctx->h_scalars[1]; S.update_bytes = ctx->h_scalars[2]; S.delete_bytes = ctx->h_scalars[3]; S.n_events = ctx->h_scalars[4];
+  S.insert_bytes = ctx->h_scalars[kScInsertBytes]; S.update_bytes = ctx->h_scalars[kScUpdateBytes];
+  S.delete_bytes = ctx->h_scalars[kScDeleteBytes]; S.n_events = ctx->h_scalars[kScEvents];
   // carry-out: this shard's end state (sharded: relative to the folded carry, read back only when asked for below)
-  Summ endst = fold(host_carry, T);
+  Summ endst = fold(host_carry, *ctx->h_total);
   if (sharded) {                                       // the stream state after the LAST shard = fold over all seams
-    const std::vector<SeamBlock>& all = seams;
     endst = host_carry;
     uint64_t base = 0;
-    for (int r = 0; r < ctx->n_ranks; r++) { if (r < ctx->rank) base += all[r].total.n_rec; endst = fold(endst, all[r].total); }
+    for (int r = 0; r < ctx->n_ranks; r++) { if (r < ctx->rank) base += seams[r].total.n_rec; endst = fold(endst, seams[r].total); }
     S.record_index_base = base;
   } else S.record_index_base = record_index_base;
   S.carry_out.in_tx = ((endst.flags & S_HAS_B) && !(endst.flags & S_CLOSED)) ? 1 : 0;
   S.carry_out.final_lsn = endst.lsn;
   S.carry_out.next_tx_ordinal = endst.ord;
-  S.abi_version = ETL_DECODE_ABI_VERSION;
-  S.sizing = sizing;
+}
 
-  // ---- note_ready (apply.rs:2079): the Relation frames of the valid prefix become the state of the next batch.
-  // After a data error the reference has bailed out before caching anything that follows it.
-  if (key != ~0ull) {
+// note_ready (apply.rs:2079): the Relation frames of the valid prefix become the state of the next batch.
+// After a data error the reference has bailed out before caching anything that follows it.
+int Decode::note_ready() {
+  const etl_dec_summary& S = b->summary;
+  const bool clean = S.first_error.record_index == UINT64_MAX;
+  uint64_t err_off = ~0ull;
+  if (!clean) {
     const uint64_t local = S.first_error.record_index - S.record_index_base;
-    if (local < T.n_rec) CKB(cudaMemcpy(&err_off, b->dev.rec_off + local, 8, cudaMemcpyDeviceToHost));
+    if (local < b->dev.n_records) CK(cudaMemcpy(&err_off, b->dev.rec_off + local, 8, cudaMemcpyDeviceToHost));
   }
   bool changed = false;
   for (const RelVersion& v : ctx->foreign_installs) if (v.effective_off == 0) { ctx->current[v.table_id] = v; ctx->current[v.table_id].effective_off = 0; changed = true; }
   for (auto& pr : ctx->pending_installs) if (pr.first < err_off) { ctx->current[pr.second.table_id] = pr.second; changed = true; }
-  if (key == ~0ull) for (const RelVersion& v : ctx->foreign_installs) if (v.effective_off == 1) { ctx->current[v.table_id] = v; ctx->current[v.table_id].effective_off = 0; changed = true; }
+  if (clean) for (const RelVersion& v : ctx->foreign_installs) if (v.effective_off == 1) { ctx->current[v.table_id] = v; ctx->current[v.table_id].effective_off = 0; changed = true; }
   if (changed) ctx->tables_valid = false;
   ctx->pending_installs.clear(); ctx->foreign_installs.clear();
-  b->dev_stream = P.buf;
-  *out = b;
+  return ETL_OK;
+}
+
+static int run_decode(etl_dec_ctx* ctx, const etl_stream_state* carry_in, uint64_t record_index_base, bool sharded, bool totals_known,
+                      etl_dec_batch** out) {
+  Decode D{ctx, carry_in, record_index_base, sharded, totals_known, false, 0};
+  for (;;) {
+    if (int rc = D.size()) return rc;
+    if (int rc = D.pass_c()) return rc;
+    if (!D.restart) break;
+    // more frames than the offset scratch holds (2x what earlier batches needed): start over on the exact path.
+    // Sharded: every rank sees the same gathered blocks, so every rank takes this branch and the exchange is repeated.
+    if (D.force_exact) { ctx->last_error = "offset scratch overflow on the exact path"; return ETL_ERR_CUDA; }
+    D = Decode{ctx, carry_in, record_index_base, sharded, false, true, D.sizing | ETL_SIZING_SCRATCH_RESTART};
+  }
+  const DecodeParams& P = ctx->P;
+  const Summ T = *ctx->h_total;
+  if (P.len) { ctx->rec_per_byte = std::max(ctx->rec_per_byte * 0.97, (double)T.n_rec / P.len); ctx->cells_per_byte = std::max(ctx->cells_per_byte * 0.97, (double)T.n_cells / P.len); }
+  uint64_t d2h = kScalarWords * 8 + sizeof(Summ);
+  if (ctx->pending_flags & ETL_DECODE_RESULTS_TO_HOST) CK(cudaEventRecord(ctx->ev[4], ctx->stream));   // d2h_ms: the plane copies alone
+  if (int rc = stage_results(ctx, D.b.get(), D.L, ctx->pending_flags, &d2h)) return rc;
+  TRACE_MARK(3);
+  D.summarise(d2h);
+  if (int rc = D.note_ready()) return rc;
+  D.b->dev_stream = P.buf;
+  *out = D.b.release();
   TRACE_MARK(4);
   return ETL_OK;
-#undef CKB
 }
 const uint8_t* etl_dec_batch_device_stream(const etl_dec_batch* b) { return b ? b->dev_stream : nullptr; }
 
@@ -1394,20 +1443,19 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
   cudaStream_t st = ctx->stream;
   ctx->launches = 0;
   ctx->tables_valid = false;                          // d_tables is reused for the column classes
-  etl_dec_batch* b = new etl_dec_batch();
+  BatchPtr b(new etl_dec_batch());
   b->ctx = ctx;
-  auto fail = [&](int rc) { if (b->dev_block) cudaFreeAsync(b->dev_block, st); delete b; return rc; };
-#define CKB(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { ctx->last_error = std::string(#call) + ": " + cudaGetErrorString(_e); return fail(ETL_ERR_CUDA); } } while (0)
+  b->copy = true;
   DecodeParams& P = ctx->P;
   memset(&P, 0, sizeof P);
   P.len = in->len; P.anchor_stride = 2048; P.copy_cols = n_cols;
-  CKB(cudaEventRecord(ctx->ev[0], st));
+  CK(cudaEventRecord(ctx->ev[0], st));
   uint64_t h2d = 0;
   if (in->dev_buf) P.buf = in->dev_buf;
   else {
-    CKB(ctx->d_stream.ensure(in->len + 64));
-    if (in->len) CKB(cudaMemcpyAsync(ctx->d_stream.ptr(), in->host_buf, in->len, cudaMemcpyHostToDevice, st));
-    CKB(cudaMemsetAsync(ctx->d_stream.ptr() + in->len, 0, 64, st));
+    CK(ctx->d_stream.ensure(in->len + 64));
+    if (in->len) CK(cudaMemcpyAsync(ctx->d_stream.ptr(), in->host_buf, in->len, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(ctx->d_stream.ptr() + in->len, 0, 64, st));
     P.buf = ctx->d_stream.ptr(); h2d += in->len;
   }
   const uint64_t nr = in->n_rows, nc = nr * n_cols;
@@ -1422,108 +1470,63 @@ int etl_dec_copy_decode(etl_dec_ctx* ctx, uint32_t table_id, const etl_copy_inpu
   uint64_t nh = in->len + 8 * nc + 64 + (any_heap ? in->len / 2 + 32 * nc + 256 : 0);
   nh = (nh + 15) & ~15ull;
   const uint64_t scalar_heap = nh;
-  uint64_t array_heap = any_array ? 3 * in->len + 4096 : 0;
+  const uint64_t first_array_heap = any_array ? 3 * in->len + 4096 : 0;
+  uint64_t array_heap = first_array_heap, heap_used = 0;
+  PlaneLayout L{};
   for (int attempt = 0;; attempt++) {
     const uint64_t heap_total = scalar_heap + array_heap;
-    const PlaneLayout L = plane_layout(nr, nc, heap_total);
-    if (b->dev_block) { CKB(cudaFreeAsync(b->dev_block, st)); b->dev_block = nullptr; }
+    L = plane_layout(nr, nc, heap_total);
+    if (b->dev_block) { CK(cudaFreeAsync(b->dev_block, st)); b->dev_block = nullptr; }
     b->block_bytes = L.total;
-    CKB(cudaMallocAsync(&b->dev_block, b->block_bytes, st));
-    fill_planes(b->dev, (uint8_t*)b->dev_block, L, nr, nc, heap_total);
+    CK(cudaMallocAsync(&b->dev_block, b->block_bytes, st));
+    fill_planes(b->dev, (uint8_t*)b->dev_block, L, nr, nc, heap_total, true);
     uint64_t* d_rows = (uint64_t*)b->dev.rec_cell_base;             // the (n_rows + 1)-entry plane holds the row offsets
-    if (in->dev_row_offsets) CKB(cudaMemcpyAsync(d_rows, in->dev_row_offsets, (nr + 1) * 8, cudaMemcpyDeviceToDevice, st));
-    else if (nr) { CKB(cudaMemcpyAsync(d_rows, in->row_offsets, (nr + 1) * 8, cudaMemcpyHostToDevice, st)); h2d += (nr + 1) * 8; }
-    else CKB(cudaMemsetAsync(d_rows, 0, 8, st));
-    b->dev.rec_off = d_rows;
-    b->dev.rec_kind = nullptr; b->dev.rec_flags = nullptr; b->dev.rec_rel = nullptr; b->dev.rec_schema = nullptr; b->dev.rec_start_lsn = nullptr;
-    b->dev.rec_commit_lsn = nullptr; b->dev.rec_tx_ordinal = nullptr; b->dev.rec_tuple_bytes = nullptr; b->dev.rec_heap_hint = nullptr;
+    if (in->dev_row_offsets) CK(cudaMemcpyAsync(d_rows, in->dev_row_offsets, (nr + 1) * 8, cudaMemcpyDeviceToDevice, st));
+    else if (nr) { CK(cudaMemcpyAsync(d_rows, in->row_offsets, (nr + 1) * 8, cudaMemcpyHostToDevice, st)); h2d += (nr + 1) * 8; }
+    else CK(cudaMemsetAsync(d_rows, 0, 8, st));
     P.rec_off = d_rows; P.rec_cell_base = d_rows;
     P.cell_tag = (uint8_t*)b->dev.cell_tag; P.cell_val = (uint64_t*)b->dev.cell_val; P.cell_aux = (uint32_t*)b->dev.cell_aux; P.heap = (uint8_t*)b->dev.heap;
     P.heap_cap = heap_total; P.arr_base = scalar_heap;
-    CKB(ctx->d_tables.ensure(n_cols + 16));
-    if (int rc = ensure_pinned(ctx, &ctx->h_up, &ctx->h_up_cap, n_cols + 16)) return fail(rc);
+    CK(ctx->d_tables.ensure(n_cols + 16));
+    if (int rc = ensure_pinned(ctx, &ctx->h_up, &ctx->h_up_cap, n_cols + 16)) return rc;
     memcpy(ctx->h_up, kinds.data(), n_cols);
-    if (n_cols) CKB(cudaMemcpyAsync(ctx->d_tables.ptr(), ctx->h_up, n_cols, cudaMemcpyHostToDevice, st));
+    if (n_cols) CK(cudaMemcpyAsync(ctx->d_tables.ptr(), ctx->h_up, n_cols, cudaMemcpyHostToDevice, st));
     P.col_kind = ctx->d_tables.ptr(); P.col_flags = ctx->d_tables.ptr();
-    unsigned long long* sc = reinterpret_cast<unsigned long long*>(ctx->d_scalars.ptr());
-    P.first_error = sc; P.metrics = sc + 1; P.heap_top = sc + 5; P.long_count = (unsigned int*)(sc + 7); P.copy_count = (unsigned int*)(sc + 8);
-    P.heap_overflow = (unsigned int*)(sc + 9); P.arr_top = sc + 10; P.perm_len = (unsigned int*)(sc + 11); P.n_act = (unsigned int*)(sc + 12);
-    P.abort_flag = (unsigned int*)(sc + 13);
-    P.dc = reinterpret_cast<const DevCarry*>(sc + kScalarWords); P.dc_out = reinterpret_cast<DevCarry*>(sc + kScalarWords);
+    bind_scalars(P, reinterpret_cast<unsigned long long*>(ctx->d_scalars.ptr()));
     P.total = ctx->d_total.ptr();
     DevCarry dc; dc.carry = summ_identity(); dc.record_index_base = 0;
-    if (int rc = upload_scalars(ctx, 0, kScalarWords, &dc)) return fail(rc);
+    if (int rc = upload_scalars(ctx, 0, kScalarWords, &dc)) return rc;
     Summ T = summ_identity(); T.n_rec = (uint32_t)nr; T.n_cells = nc;
     *ctx->h_total = T;
-    CKB(cudaMemcpyAsync(P.total, ctx->h_total, sizeof(Summ), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(P.total, ctx->h_total, sizeof(Summ), cudaMemcpyHostToDevice, st));
     P.cap_records = nr; P.cap_cells = nc;
-    if (nc) CKB(cudaMemsetAsync(P.cell_tag, 0, nc, st));   // a row that failed leaves cells unwritten: k_heavy must not see stale tags
-    CKB(cudaEventRecord(ctx->ev[1], st));
+    if (nc) CK(cudaMemsetAsync(P.cell_tag, 0, nc, st));   // a row that failed leaves cells unwritten: k_heavy must not see stale tags
+    for (int e = 1; e <= 3; e++) CK(cudaEventRecord(ctx->ev[e], st));   // no index pass: the kernels start where the uploads end
     if (nr) {
       k_copy_rows<<<(uint32_t)((nr + kRowsThreads - 1) / kRowsThreads), kRowsThreads, kCopySmemBytes, st>>>(P);
       k_heavy<<<std::min<uint32_t>((uint32_t)((nc + kHeavyTile - 1) / kHeavyTile) + 1u, (uint32_t)sm_count(ctx) * 3u), kHeavyThreads, kHeavySmemBytes, st>>>(P);
       ctx->launches += 2;
-      CKB(cudaGetLastError());
+      CK(cudaGetLastError());
     }
-    CKB(cudaEventRecord(ctx->ev[4], st));
-    CKB(cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars.ptr(), kScalarWords * 8, cudaMemcpyDeviceToHost, st));
-    CKB(cudaStreamSynchronize(st));
-    if (int rc = check_scalar_heap(ctx, scalar_heap)) return fail(rc);
-    if (!ctx->h_scalars[9]) break;
-    if (attempt >= 4) { ctx->last_error = "array heap reservation overflow after retries"; return fail(ETL_ERR_CUDA); }
+    CK(cudaEventRecord(ctx->ev[4], st));
+    CK(cudaMemcpyAsync(ctx->h_scalars, ctx->d_scalars.ptr(), kScalarWords * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (int rc = measure_heap(ctx, scalar_heap, &heap_used)) return rc;
+    if (!ctx->h_scalars[kScHeapOverflow]) break;
+    if (attempt >= 4) { ctx->last_error = "array heap reservation overflow after retries"; return ETL_ERR_CUDA; }
     array_heap *= 4;
   }
-  // (the min only trims the 8-byte rounding of the last array reservation: the scalar region was checked above)
-  const uint64_t heap_used = std::min<uint64_t>(P.heap_cap, ctx->h_scalars[10] ? scalar_heap + ctx->h_scalars[10] : ctx->h_scalars[5]);
   b->dev.heap_bytes = heap_used;
   uint64_t d2h = kScalarWords * 8;
-  if (flags & ETL_DECODE_RESULTS_TO_HOST) {
-    const PlaneLayout H = plane_layout(nr, nc, heap_used);
-    if (ctx->h_result_cap < H.total) {
-      if (ctx->h_result) cudaFreeHost(ctx->h_result);
-      ctx->h_result = nullptr; ctx->h_result_cap = 0;
-      size_t want = H.total + H.total / 8;
-      CKB(cudaHostAlloc(&ctx->h_result, want, cudaHostAllocDefault));
-      ctx->h_result_cap = want;
-    }
-    uint8_t* hb = (uint8_t*)ctx->h_result;
-    fill_planes(b->host, hb, H, nr, nc, heap_used);
-    b->host.rec_off = b->host.rec_cell_base;
-    b->host.rec_kind = nullptr; b->host.rec_flags = nullptr; b->host.rec_rel = nullptr; b->host.rec_schema = nullptr; b->host.rec_start_lsn = nullptr;
-    b->host.rec_commit_lsn = nullptr; b->host.rec_tx_ordinal = nullptr; b->host.rec_tuple_bytes = nullptr; b->host.rec_heap_hint = nullptr;
-    CKB(cudaMemcpyAsync((void*)b->host.rec_cell_base, b->dev.rec_cell_base, (nr + 1) * 8, cudaMemcpyDeviceToHost, st));
-    if (nc) {
-      CKB(cudaMemcpyAsync((void*)b->host.cell_tag, b->dev.cell_tag, nc, cudaMemcpyDeviceToHost, st));
-      CKB(cudaMemcpyAsync((void*)b->host.cell_val, b->dev.cell_val, nc * 8, cudaMemcpyDeviceToHost, st));
-      CKB(cudaMemcpyAsync((void*)b->host.cell_aux, b->dev.cell_aux, nc * 4, cudaMemcpyDeviceToHost, st));
-    }
-    if (heap_used) CKB(cudaMemcpyAsync((void*)b->host.heap, b->dev.heap, heap_used, cudaMemcpyDeviceToHost, st));
-    d2h += (nr + 1) * 8 + nc * 13 + heap_used;
-    b->host_block = hb; b->has_host = true;
-  }
-  CKB(cudaEventRecord(ctx->ev[5], st));
-  CKB(cudaStreamSynchronize(st));
-  etl_dec_summary& S = b->summary;
-  memset(&S, 0, sizeof S);
-  cudaEventElapsedTime(&S.h2d_ms, ctx->ev[0], ctx->ev[1]);
-  cudaEventElapsedTime(&S.emit_ms, ctx->ev[1], ctx->ev[4]);
-  cudaEventElapsedTime(&S.d2h_ms, ctx->ev[4], ctx->ev[5]);
-  S.kernel_ms = S.emit_ms; S.cells_ms = S.emit_ms;
-  S.h2d_bytes = h2d; S.d2h_bytes = d2h; S.gpu_launches = ctx->launches; S.abi_version = ETL_DECODE_ABI_VERSION;
-  S.sizing = ETL_SIZING_EXACT | (array_heap > (any_array ? 3 * in->len + 4096 : 0) ? ETL_SIZING_ARRAY_HEAP_RETRY : 0u);
-  const unsigned long long key = ctx->h_scalars[0];
-  if (key == ~0ull) S.first_error.record_index = UINT64_MAX;
-  else {
-    S.first_error.record_index = key >> 24; S.first_error.seq = (uint32_t)((key >> 6) & 0x3FFFFu);
-    S.first_error.code = (uint32_t)(key & 63u); S.first_error.kind = error_kind_of(S.first_error.code);
-  }
-  S.n_events = nr;
+  if (int rc = stage_results(ctx, b.get(), L, flags, &d2h)) return rc;
+  fill_summary(ctx, b.get(), flags, h2d, d2h, ETL_SIZING_EXACT | (array_heap > first_array_heap ? ETL_SIZING_ARRAY_HEAP_RETRY : 0u));
+  b->summary.cells_ms = b->summary.emit_ms;
+  b->summary.n_events = nr;
   b->dev_stream = P.buf;
-  b->copy = true; b->copy_table = table_id; b->copy_kinds = std::move(kinds);
+  b->copy_table = table_id; b->copy_kinds = std::move(kinds);
   for (uint32_t i = 0; i < n_cols; i++) b->copy_pk.push_back(t.cols[i].pk != -1 ? 1 : 0);
-  *out = b;
+  *out = b.release();
   return ETL_OK;
-#undef CKB
 }
 
 int etl_dec_batch_planes(const etl_dec_batch* b, int host, etl_dec_planes* out) {

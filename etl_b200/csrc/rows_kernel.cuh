@@ -563,23 +563,11 @@ __device__ __forceinline__ void rows_body(const DecodeParams& P, uint8_t* smem) 
   for (int d = 16; d > 0; d >>= 1) { si += __shfl_down_sync(0xffffffffu, si, d); su += __shfl_down_sync(0xffffffffu, su, d); sd += __shfl_down_sync(0xffffffffu, sd, d); }
   if (lane == 0) { if (si) atomicAdd(&P.metrics[0], si); if (su) atomicAdd(&P.metrics[1], su); if (sd) atomicAdd(&P.metrics[2], sd); }
 }
-// The kernel: the rows of this CTA's chunk, then — when the stream has segments without a frame start (TOAST-sized
-// values) and the host asked for it — this warp's share of the structure-blind UTF-8 pass.  The row work is bound by
-// instruction issue and shared-memory latency, the UTF-8 pass by HBM bandwidth: warps of one kernel that are in
-// different phases overlap the two without either waiting for thread slots held by the other's kernel.  Measured (C5):
-// not faster than running k_utf8_dead after k_rows — 20 warps per SM cannot keep enough bytes in flight to saturate
-// HBM — so this is a tuning knob (ETL_DEAD_MODE=3), not the default.
+// The kernel: the rows of this CTA's chunk.
 __global__ void __launch_bounds__(kRowsThreads, ETL_ROWS_CTAS) k_rows(DecodeParams P) {
   extern __shared__ __align__(128) uint8_t smem[];
   if (*P.abort_flag) return;
   rows_body(P, smem);
-  if (P.dead_in_rows) {
-    const uint32_t ppseg = dead_ppseg(P);
-    const uint32_t n_items = (P.n_anchors - *P.n_act) * ppseg;
-    const uint32_t n_warps = gridDim.x * kRowsWarps, gw = blockIdx.x * kRowsWarps + (threadIdx.x >> 5);
-    // item i goes to warp i % n_warps (consecutive warps stream consecutive 2 KiB)
-    for (uint32_t it = gw; it < n_items; it += n_warps) utf8_dead_items(P, it, n_warps, n_items, ppseg, threadIdx.x & 31u);
-  }
 }
 #undef W_DATA_ERROR
 #undef W_MALFORMED

@@ -116,7 +116,6 @@ struct DecodeParams {
   unsigned int* abort_flag;         // ABORT_* bits: the batch does not fit the planes / scratch the host reserved (k_chase, k_records)
   unsigned int* copy_count;         // unchanged-TOAST cells left for k_fix
   uint32_t copy_cols;               // COPY-row decode (copy_kernel.cuh): columns per row; 0 on the replication path
-  uint32_t dead_in_rows;            // 1: the warps of k_rows also stream the dead segments (no separate k_utf8_dead launch)
   uint64_t cap_records, cap_cells;  // capacity of the record / cell planes
   uint32_t* line_bad;               // k_utf8_dead: bit l set = line l (128 bytes) holds a UTF-8 rule violation (zeroed per batch)
   uint32_t* dead;                   // segments without a frame start (ascending); n_dead = n_anchors - *n_act
@@ -772,7 +771,7 @@ __device__ __forceinline__ void utf8_dead_verdict(const DecodeParams& P, const u
 // first byte is looked at; the three bytes before a lane's first chunk come from one 4-byte load that hits L1 — no shuffles
 // (round 1 paid three __shfl per 16 bytes).  Measured: 4 items (16 loads) per lane cost 102 registers and a quarter of the
 // warps, and the pass was slower on C5.
-__device__ __forceinline__ void utf8_dead_items(const DecodeParams& P, uint32_t it, uint32_t, uint32_t n_items, uint32_t ppseg, uint32_t lane) {
+__device__ __forceinline__ void utf8_dead_items(const DecodeParams& P, uint32_t it, uint32_t n_items, uint32_t ppseg, uint32_t lane) {
   uint4 x[4];
   uint32_t pw = 0;
   uint64_t off = 0, s1 = 0;
@@ -795,7 +794,7 @@ __global__ void __launch_bounds__(256) k_utf8_dead(DecodeParams P) {
   const uint32_t n_items = (P.n_anchors - *P.n_act) * ppseg;
   const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;      // warp w: items [w * kDeadSegsPerWarp, +kDeadSegsPerWarp)
   for (uint32_t it = w * kDeadSegsPerWarp; it < min(n_items, (w + 1u) * kDeadSegsPerWarp); it++)
-    utf8_dead_items(P, it, 1u, min(n_items, (w + 1u) * kDeadSegsPerWarp), ppseg, threadIdx.x & 31u);
+    utf8_dead_items(P, it, min(n_items, (w + 1u) * kDeadSegsPerWarp), ppseg, threadIdx.x & 31u);
 }
 // any flagged line in [l0, l1)?  One bitmap word per lane and step (a 64 KiB value spans 16 words: a single lane
 // testing them one after the other was a chain of 16 dependent-by-branch loads per cell)
