@@ -491,7 +491,9 @@ __device__ __forceinline__ void rows_body(const DecodeParams& P, uint8_t* smem) 
             LongCell lc;
             lc.rec_local = w.rec_local; lc.seq = tc.seq; lc.soff = soff; lc.len = len; lc.edges = defer ? 1u : 0u;
             P.long_cells[at] = lc;
-            if (!defer) { r0_hi = (uint32_t)(S0 - soff); r1_lo = (uint32_t)(S1 - soff); r1_hi = len; }
+            // the tail keeps at least the last byte (k_long_cells does the same): a sequence left open at the end of the
+            // interior is a violation only past the cell's end
+            if (!defer) { r0_hi = (uint32_t)(S0 - soff); r1_lo = min((uint32_t)(S1 - soff), len - 1u); r1_hi = len; }
           } else r0_hi = len;                          // cannot happen (the list holds every cell of ≥ kCoopLen bytes)
         }
       } else if (utf8_medium_bad(tv, len)) code = ETL_E_UTF8;

@@ -654,35 +654,8 @@ __device__ __forceinline__ uint64_t ld64u(const uint8_t* p) {
 __device__ __forceinline__ uint32_t bswap32(uint32_t v) { return __byte_perm(v, 0, 0x0123); }
 __device__ __forceinline__ uint64_t bswap64(uint64_t v) { return ((uint64_t)bswap32((uint32_t)v) << 32) | bswap32((uint32_t)(v >> 32)); }
 
-// UTF-8 check of a short/medium cell with word loads: all-ASCII words pass immediately
-// any byte >= 0x80 in [s, s+n)?  Aligned 8-byte loads with the edges masked off (the bytes around a cell are
-// readable: frame header before, padding after) — one load per word instead of the three of ld64u.
-__device__ __forceinline__ bool has_high_bits(const uint8_t* s, uint32_t n) {
-  if (n == 0) return false;
-  const uintptr_t a = reinterpret_cast<uintptr_t>(s);
-  const uint64_t* w = reinterpret_cast<const uint64_t*>(a & ~uintptr_t(7));
-  const uint32_t lead = (uint32_t)(a & 7u);
-  const uint32_t nw = (lead + n + 7u) >> 3;          // words touched
-  const uint32_t tail = (lead + n) & 7u;
-  // every load is independent of the others: issue them in groups of four so that a 60-byte cell costs two
-  // memory round trips instead of eight (a load-OR-load chain was the longest stall of the round-1 cell kernel)
-  const uint64_t first = w[0], last = w[nw - 1];
-  uint64_t acc = 0;
-  for (uint32_t i = 1; i + 1 < nw; i += 4) {
-    const uint64_t a0 = w[i];
-    const uint64_t a1 = i + 2 < nw ? w[i + 1] : 0ull;
-    const uint64_t a2 = i + 3 < nw ? w[i + 2] : 0ull;
-    const uint64_t a3 = i + 4 < nw ? w[i + 3] : 0ull;
-    acc |= a0 | a1 | a2 | a3;
-  }
-  const uint64_t lo_mask = ~0ull << (8u * lead);
-  const uint64_t hi_mask = tail ? (1ull << (8u * tail)) - 1ull : ~0ull;
-  if (nw == 1) acc = first & lo_mask & hi_mask;
-  else acc |= (first & lo_mask) | (last & hi_mask);
-  return (acc & 0x8080808080808080ull) != 0;
-}
-
 }  // namespace etl
+#include "utf8.cuh"         // has_high_bits, utf8_range_bad
 #include "array_parse.cuh"   // parse_text_cell_impl, parse_text_cell, parse_array_cell / parse_array_any
 namespace etl {
 
@@ -691,48 +664,6 @@ __device__ __forceinline__ void put_cell(const DecodeParams& P, uint64_t idx, ui
 }
 constexpr int kWideLen = 96;     // text cells at least this long are validated with 16-byte loads
 constexpr int kCoopLen = 512;    // ... these by the whole warp; the part that covers whole dead segments by k_utf8_dead
-// UTF-8 validation of bytes [lo, hi) of one text cell by `nthreads` cooperating threads (one thread, a warp,
-// or a half-warp of k_long_cells): 16-byte aligned chunks, 4 independent loads in flight per thread.
-// An all-ASCII chunk costs one load + one test; a chunk with high bits is checked with the
-// position-local rule over [clo, chi+3) so the following chunk never has to look back; the first 16
-// bytes of the range are always checked with look-back (a range may start in the middle of a cell).
-__device__ __forceinline__ bool utf8_range_bad(const uint8_t* cell, uint32_t cell_len, uint32_t lo, uint32_t hi, uint32_t t, uint32_t nthreads) {
-  bool bad = false;
-  if (hi <= lo) return false;
-  const uintptr_t a0 = reinterpret_cast<uintptr_t>(cell + lo);
-  const uint32_t headn = min(hi - lo, (uint32_t)((16u - (uint32_t)(a0 & 15u)) & 15u));
-  if (t == 0) {                                       // head: byte-serial only when it (or its look-back) has high bits
-    const uint32_t hhi = min(lo + headn + 19u, hi), hlo = lo >= 3u ? lo - 3u : 0u;
-    if (has_high_bits(cell + hlo, hhi - hlo)) bad |= !utf8_chunk_valid(cell, cell_len, lo, hhi);
-  }
-  const uint32_t body0 = lo + headn;
-  const uint32_t nchunks = (hi - body0) / 16u;
-  const uint4* body = reinterpret_cast<const uint4*>(cell + body0);
-  uint32_t c = t;
-  for (; c + 3 * nthreads < nchunks; c += 4 * nthreads) {
-    const uint4 x0 = body[c], x1 = body[c + nthreads], x2 = body[c + 2 * nthreads], x3 = body[c + 3 * nthreads];
-    const uint32_t h0 = (x0.x | x0.y | x0.z | x0.w), h1 = (x1.x | x1.y | x1.z | x1.w), h2 = (x2.x | x2.y | x2.z | x2.w), h3 = (x3.x | x3.y | x3.z | x3.w);
-    if ((h0 | h1 | h2 | h3) & 0x80808080u) {
-      if (h0 & 0x80808080u) { const uint32_t cl = body0 + c * 16u; bad |= !utf8_chunk_valid(cell, cell_len, cl, min(cl + 19u, hi)); }
-      if (h1 & 0x80808080u) { const uint32_t cl = body0 + (c + nthreads) * 16u; bad |= !utf8_chunk_valid(cell, cell_len, cl, min(cl + 19u, hi)); }
-      if (h2 & 0x80808080u) { const uint32_t cl = body0 + (c + 2 * nthreads) * 16u; bad |= !utf8_chunk_valid(cell, cell_len, cl, min(cl + 19u, hi)); }
-      if (h3 & 0x80808080u) { const uint32_t cl = body0 + (c + 3 * nthreads) * 16u; bad |= !utf8_chunk_valid(cell, cell_len, cl, min(cl + 19u, hi)); }
-    }
-  }
-  for (; c < nchunks; c += nthreads) {
-    const uint4 x = body[c];
-    if ((x.x | x.y | x.z | x.w) & 0x80808080u) {
-      const uint32_t cl = body0 + c * 16u;
-      bad |= !utf8_chunk_valid(cell, cell_len, cl, min(cl + 19u, hi));
-    }
-  }
-  const uint32_t tail0 = body0 + nchunks * 16u;
-  if (t == nthreads - 1 && tail0 < hi) {
-    const uint32_t tlo = tail0 >= 3u ? tail0 - 3u : 0u;
-    if (has_high_bits(cell + tlo, hi - tlo)) bad |= !utf8_chunk_valid(cell, cell_len, tail0, hi);
-  }
-  return bad;
-}
 // Structure-blind UTF-8 pass.  The position-local rule (utf8_step_bad) needs only the three preceding
 // bytes, so the verdict for position i of a cell is the verdict for stream position a+i whenever the
 // three predecessors lie inside the cell.  A segment without a frame start lies inside one frame; the
@@ -825,7 +756,10 @@ __global__ void __launch_bounds__(256) k_long_cells(DecodeParams P) {
       bad = lines_any_bad(P.line_bad, S0 >> 7, S1 >> 7, lane);
       if (c.edges) {                                     // head on lanes 0-15, tail on lanes 16-31: one latency chain, not two
         const bool tail = lane >= 16u;
-        bad |= utf8_range_bad(P.buf + c.soff, c.len, tail ? (uint32_t)(S1 - c.soff) : 0u, tail ? c.len : (uint32_t)(S0 - c.soff), lane & 15u, 16u);
+        // a cell that ends on a boundary keeps its last byte in the tail: a sequence left open at the end of the interior
+        // is a violation only past the cell's end, which the bitmap does not cover
+        const uint32_t t0 = min((uint32_t)(S1 - c.soff), c.len - 1u);
+        bad |= utf8_range_bad(P.buf + c.soff, c.len, tail ? t0 : 0u, tail ? c.len : (uint32_t)(S0 - c.soff), lane & 15u, 16u);
       }
     } else if (c.edges) bad = utf8_range_bad(P.buf + c.soff, c.len, 0u, c.len, lane, 32u);
     if (__any_sync(0xffffffffu, bad) && lane == 0) report_error(P, P.dc->record_index_base + c.rec_local, c.seq, ETL_E_UTF8);
